@@ -1,4 +1,4 @@
-# Build + CPU test image.  Run the GPU tiers with `docker run --gpus all` on a B200 host.
+# Build + CPU test image.  Run the GPU tiers with `docker run --gpus all` on a H100 host.
 FROM nvidia/cuda:12.9.0-devel-ubuntu24.04
 ENV DEBIAN_FRONTEND=noninteractive
 RUN apt-get update && apt-get install -y --no-install-recommends python3 python3-pip python3-venv git build-essential \

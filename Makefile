@@ -1,10 +1,10 @@
-# sparkflow_b200 developer targets.  GPU targets need a B200 (sm_100a); everything else runs on a CPU box.
+# sparkflow_b200 developer targets.  GPU targets need a H100 (sm_90a); everything else runs on a CPU box.
 PY ?= python
 NGPU ?= 8
 
 .PHONY: build test test-gpu smoke bench bench-scale bench-nccl gemm sanitize examples clean
 
-build:            ## nvcc -gencode arch=compute_100a,code=sm_100a -> sparkflow_b200/_C.so, _host.so
+build:            ## nvcc -gencode arch=compute_90a,code=sm_90a -> sparkflow_b200/_C.so, _host.so
 	$(PY) tools/build_ext.py
 
 test: build       ## API, formats, oracle, gloo world_size=2 (CPU)
@@ -25,7 +25,7 @@ bench-scale: build
 bench-nccl: build ## the PyTorch + NCCL(+cuBLAS) build of the same semantics
 	$(PY) -m torch.distributed.run --nnodes=1 --nproc-per-node $(NGPU) --master-addr 127.0.0.1 bench.py --gpus $(NGPU) --impl nccl
 
-gemm: build       ## one-CTA kernel vs persistent 2-CTA kernel vs cuBLAS
+gemm: build       ## one-CTA kernel vs persistent cluster-pair kernel vs cuBLAS
 	$(PY) tools/bench_gemm.py
 
 sanitize: build   ## compute-sanitizer over the kernel tests

@@ -15,7 +15,6 @@ Numbers per run (all through the public engine API, all timed on the device, max
               One CUDA-event pair around the K steps.
   e2e.value   the same K steps with the partition in PINNED HOST memory: every step copies its minibatch host->device
               and hands the step's loss back device->host.  One CUDA-event pair around the K steps.
-  sustained   `value` again over a longer run (so clocks can be sampled while the GPU is loaded).
   nccl_baseline_same_run / vs_baseline
               the stock PyTorch + NCCL(+cuBLAS/cuDNN) build of the same semantics (baseline/nccl_baseline.py: flat
               params, fused capturable Adam, the whole step incl. both collectives in ONE CUDA graph), measured the same
@@ -25,6 +24,8 @@ Numbers per run (all through the public engine API, all timed on the device, max
 ``--impl reference`` would run the unmodified lifeomic/sparkflow from baseline/_ref; it needs TensorFlow
 1.x + pyspark + flask + a JVM, none of which exist in this image, so it reports ``unavailable``.
 ``--impl nccl`` runs only the NCCL arm.
+``--dump-outputs DIR`` writes what the timed steps computed (the loss of the last step and the master parameters after
+it) as DIR/<name>.npy, so two builds can be compared output for output: the inputs are seeded and identical per run.
 """
 from __future__ import annotations
 
@@ -93,9 +94,24 @@ def _partition_rows(args, in_dim: int) -> int:
     return rows
 
 
-def _sustained_steps(K: int, ms_per_step: float) -> int:
-    """Long enough for nvidia-smi to see the load (~1.5 s), bounded."""
-    return int(max(K, min(20000, 1500.0 / max(ms_per_step, 1e-3))))
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, loss: float, params) -> None:
+    """loss.npy (float64) and param_NN.npy (float32, flattened); an array above its share of DUMP_BYTES is replaced by a
+    fixed, seeded sample of its elements (sample_NN.npy holds the flat indices)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([loss], dtype=np.float64))
+    cap = DUMP_BYTES // 8 // max(1, len(params))          # float32 values + their int32 sample indices
+    for i, a in enumerate(params):
+        flat = np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
+        if flat.size > cap:
+            idx = np.sort(np.random.default_rng(i).choice(flat.size, size=cap, replace=False)).astype(np.int32)
+            np.save(os.path.join(out_dir, f"sample_{i:02d}.npy"), idx)
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, f"param_{i:02d}.npy"), flat)
 
 
 def run_ours(args, ctx) -> dict:
@@ -165,10 +181,12 @@ def run_ours(args, ctx) -> dict:
     steps(eng_r, W, 0)
     eng_r.finish()
     dev_ms, _ = timed(eng_r, K, W)
-    Ks = _sustained_steps(K, dev_ms / K)
-    sus_ms, _ = timed(eng_r, Ks, W + K)
     last_loss = eng_r.last_loss()
     sess.sync_all()
+    if args.dump_outputs:
+        params = sess.weights()
+        if ctx.rank == 0:
+            dump_outputs(args.dump_outputs, last_loss, params)
     # exposed push / pull per step, measured on the device (%globaltimer) inside the pull / applier kernels
     exposed = None
     if getattr(eng.w, "sharded", False):
@@ -194,7 +212,6 @@ def run_ours(args, ctx) -> dict:
         "e2e": {"value": ctx.world * BATCH * K / (e2e_ms / 1e3), "unit": "samples/s", "ms_per_step": e2e_ms / K,
                 "h2d_bytes_per_step": int(h2d_per_step), "d2h_bytes_per_step": int(d2h_per_step), "wall_ms_per_step": wall_ms / K,
                 "host_us_per_step": host_us, "final_loss": e2e_loss},
-        "sustained": {"steps": Ks, "value": ctx.world * BATCH * Ks / (sus_ms / 1e3), "ms_per_step": sus_ms / Ks},
         "exposed_push_pull_us_per_step": exposed,
         "gpu_launches": int(launches * K * ctx.world),
         "clocks": clocks, "final_loss": last_loss, "master_counters": counters,
@@ -251,8 +268,6 @@ def run_nccl(args, ctx) -> dict:
     for k in range(W):
         step(k, False)
     dev_ms = timed(K, W, False)
-    Ks = _sustained_steps(K, dev_ms / K)
-    sus_ms = timed(Ks, W + K, False)
     clocks = sampler.stop() if sampler else {}
     torch.cuda.synchronize(dev)
     return {"metric": METRIC if args.model == "simple_dnn" else f"{args.model} samples/sec (device-timed, max over ranks)",
@@ -266,7 +281,6 @@ def run_nccl(args, ctx) -> dict:
                              "partition with a fresh H2D every step (e2e)"},
             "e2e": {"value": ctx.world * BATCH * K / (e2e_ms / 1e3), "unit": "samples/s", "ms_per_step": e2e_ms / K,
                     "h2d_bytes_per_step": BATCH * (in_dim + n_classes) * 4, "d2h_bytes_per_step": 4},
-            "sustained": {"steps": Ks, "value": ctx.world * BATCH * Ks / (sus_ms / 1e3), "ms_per_step": sus_ms / Ks},
             "gpu_launches": 0, "clocks": clocks, "final_loss": float(loss_host[0])}
 
 
@@ -286,13 +300,15 @@ def main() -> int:
     ap.add_argument("--no-baseline", action="store_true", help="skip the NCCL arm that normally runs in the same launch")
     ap.add_argument("--baseline-eager", action="store_true", help="NCCL arm without CUDA graphs")
     ap.add_argument("--baseline-compile", action="store_true", help="torch.compile the NCCL arm's forward/backward before capture")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write the last step's loss and the master parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return reference_arm(args)
     import torch
 
     if not torch.cuda.is_available():
-        print(json.dumps({"metric": METRIC, "error": "no CUDA device: bench.py measures the B200 engine"}))
+        print(json.dumps({"metric": METRIC, "error": "no CUDA device: bench.py measures the native GPU engine"}))
         return 1
     from sparkflow_b200.parallel import dist as D
 
@@ -312,7 +328,7 @@ def main() -> int:
         try:
             base = run_nccl(args, ctx)
             res["nccl_baseline_same_run"] = {"value": base["value"], "ms_per_step": base["ms_per_step"], "e2e_value": base["e2e"]["value"],
-                                             "e2e_ms_per_step": base["e2e"]["ms_per_step"], "sustained_value": base["sustained"]["value"],
+                                             "e2e_ms_per_step": base["e2e"]["ms_per_step"],
                                              "cuda_graph": base["config"]["cuda_graph"], "torch_compile": base["config"]["torch_compile"],
                                              "final_loss": base["final_loss"]}
             res["vs_baseline"] = res["value"] / base["value"]

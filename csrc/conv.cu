@@ -1,7 +1,7 @@
 // Convolution building blocks for the compiled CNN plan (reference ops K3/K4 of SURVEY.md section 2.4:
 // Conv2D + BiasAdd + Relu, MaxPool and their gradients; examples/cnn_example.py:10-22).
 //
-// Convolutions are lowered to the tcgen05 GEMM of gemm_sm100.cu:
+// Convolutions are lowered to the wgmma GEMM of gemm_sm90.cu:
 //   forward   out[M, Cout]   = patches[M, K] . W^T[Cout, K]^T  (+bias, ReLU in the GEMM epilogue)
 //   wgrad     dW[K, Cout]    = patches^T[K, M] . dz^T[Cout, M]^T      (split-K, atomic accumulate)
 //   dgrad     dpatch[M, K]   = dz[M, Cout] . W[K, Cout]^T             -> col2im gather
@@ -9,7 +9,7 @@
 // of TensorFlow's HWIO filter layout.  The kernels here produce the K-major operands those GEMMs need:
 // im2col writes patches AND patches^T; max-pool backward applies the ReLU derivative, scatters through
 // the arg-max mask and writes dz, dz^T and the bias gradient in one pass.
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "sf_api.h"
 
 namespace sf {
@@ -268,7 +268,7 @@ maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __rest
 
 static inline int grid_1d(size_t total) {
   size_t b = (total + 255) / 256;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > sf_num_sms() * 16) b = sf_num_sms() * 16;
   return static_cast<int>(b < 1 ? 1 : b);
 }
 
@@ -534,8 +534,8 @@ static int conv_first_fwd_launch(const __nv_bfloat16* x, int n, int h, int w, in
     if (e != cudaSuccess) return static_cast<int>(e);
     attr = smem;
   }
-  // work items = (image, part): pick the split whose wave count x pixels-per-thread is smallest on 148 SMs x 4 resident CTAs
-  const int slots = 148 * 4, n_grp = sf::kConv1Threads / cout, P = ((h - kh + 1) / 2) * ((w - kw + 1) / 2);
+  // work items = (image, part): pick the split whose wave count x pixels-per-thread is smallest on every SM x 4 resident CTAs
+  const int slots = sf_num_sms() * 4, n_grp = sf::kConv1Threads / cout, P = ((h - kh + 1) / 2) * ((w - kw + 1) / 2);
   int parts = 1;
   float best = 1e30f;
   for (int p = 1; p <= 8; ++p) {
@@ -566,7 +566,7 @@ static int conv_first_wgrad_launch(const __nv_bfloat16* x, int n, int h, int w, 
     if (e != cudaSuccess) return static_cast<int>(e);
     attr = smem;
   }
-  int grid = n < 148 * 2 ? n : 148 * 2;           // one (or a few) images per CTA; one atomic per gradient word and CTA
+  int grid = n < sf_num_sms() * 2 ? n : sf_num_sms() * 2;          // one (or a few) images per CTA; one atomic per gradient word and CTA
   if (grid < 1) grid = 1;
   return static_cast<int>(sf::launch(sf::conv_first_wgrad_kernel<KH, KW, CIN>, dim3(grid), dim3(sf::kConv1Threads), smem, st, x, n, h, w, cin, kh, kw,
                                      cout, g_pool, pooled, argmax, act, dW, db, stage));

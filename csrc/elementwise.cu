@@ -2,7 +2,7 @@
 // input cast+transpose (K11 feeder), softmax-cross-entropy (K5), MSE (K6), argmax (K7).
 // Reference semantics: tf.losses.softmax_cross_entropy / mean_squared_error with the default
 // SUM_BY_NONZERO_WEIGHTS reduction (examples/simple_dnn.py:20, autoencoder_example.py:15).
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "sf_api.h"
 
 namespace sf {
@@ -365,7 +365,7 @@ extern "C" int sf_softmax_xent(const float* logits, int ld_logits, const float* 
                                float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                                float* dbias, int rows, int cols, cudaStream_t st) {
   int blocks = (rows + 7) / 8;
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > sf_num_sms() * 4) blocks = sf_num_sms() * 4;
   return static_cast<int>(sf::launch(sf::softmax_xent_kernel, dim3(blocks), dim3(256), cols * sizeof(float), st,
                                      logits, ld_logits, labels, ld_labels, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
 }

@@ -1,4 +1,4 @@
-// Fused parameter-server push / pull for sm_100a.
+// Fused parameter-server push / pull for sm_90a.
 //
 // push  (reference: POST /update -> optimizer.apply_gradients, one optimizer step PER PUSH,
 //        sparkflow/HogwildSparkModel.py:219-242): the *worker* launches this kernel.  It streams
@@ -14,7 +14,7 @@
 //        fp32 params) into the local replica under the read side of the same lock.
 //
 // All ten TF-1.x optimizers of tensorflow_async.py:19-30 are implemented as update functors.
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "sf_api.h"
 
 namespace sf {
@@ -474,7 +474,7 @@ __device__ __forceinline__ void signal_done(float* loss_out, unsigned int* done_
 
 // End-of-step hand-off to the host: the mean loss and the step count.  With a spinning host (done_dev) both travel in
 // ONE aligned 8-byte store to the pinned word pair {loss, count} - single-copy atomic, so no system fence (measured
-// ~5 us on B200, on the critical path of every step) is needed to order "loss before count".
+// several us, on the critical path of every step) is needed to order "loss before count".
 __device__ __forceinline__ void publish_loss(float* loss_out, float* loss_acc, unsigned int* done_dev) {
   if (loss_acc != nullptr && done_dev != nullptr) {
     const float l = *loss_acc;
@@ -728,7 +728,7 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
   const bool leader = blockIdx.x == 0;
   const bool locked = a.push.lock_mode == SF_LOCK_RW;
   // One launch serves up to kMaxBatches passes.  With `linger` it keeps listening between passes: the same resident CTAs
-  // (instruction cache, TLB warm) serve the next push - measured on B200, a cold pass spends ~5 us just fetching code.
+  // (instruction cache, TLB warm) serve the next push - a cold pass spends microseconds just fetching code.
   constexpr int kMaxBatches = 256;
   for (int k = 0; k < kMaxBatches; ++k) {
     const uint32_t epoch = seq * 256u + static_cast<uint32_t>(k);
@@ -859,7 +859,9 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
     float* const vec0 = (a.dbuf && s_buf) ? a.vec_pub_alt : a.push.vec_pub[0];
     const int tile_lo = a.tile_end > a.tile_begin ? a.tile_begin : 0;
     const int tile_hi = a.tile_end > a.tile_begin ? a.tile_end : a.push.num_tiles;
-    unsigned long long tpt[3] = {0ull, 0ull, 0ull};
+    // probe timestamps in shared memory: a thread-local array whose address is passed down would get a stack frame
+    __shared__ unsigned long long tpt[3];
+    if (probe) tpt[0] = tpt[1] = tpt[2] = 0ull;
     const unsigned long long tpa = probe ? gtime_ns() : 0ull;          // s_grads built, barrier passed
     // warm mode: CTA 0 only coordinates (its tile code would be cold: it spends its idle time scanning the flags)
     const int tile_ctas = a.warm_polls > 0 ? static_cast<int>(gridDim.x) - 1 : static_cast<int>(gridDim.x);
@@ -1243,7 +1245,7 @@ extern "C" int sf_pull_launch(const SfPullArgs* a, uint32_t* local_sync, int gri
   if (grid <= 0) {
     const size_t n16 = a->n_bf16 / 8 + a->n_f32 / 4;
     grid = static_cast<int>((n16 + 256 * 4 - 1) / (256 * 4));
-    if (grid > 148) grid = 148;
+    if (grid > sf_num_sms()) grid = sf_num_sms();
     if (grid < 1) grid = 1;
   }
   if (a->scope_sys) return static_cast<int>(sf::launch(sf::pull_kernel<true>, dim3(grid), dim3(256), 0, st, *a, local_sync));
@@ -1253,7 +1255,7 @@ extern "C" int sf_pull_launch(const SfPullArgs* a, uint32_t* local_sync, int gri
 extern "C" int sf_post_launch(const SfPostArgs* a, uint32_t* local_sync, int grid, cudaStream_t st) {
   if (grid <= 0) {
     grid = static_cast<int>((a->n / 4 + 256 * 8 - 1) / (256 * 8));
-    if (grid > 148) grid = 148;
+    if (grid > sf_num_sms()) grid = sf_num_sms();
     if (grid < 1) grid = 1;
   }
   return static_cast<int>(sf::launch(sf::post_kernel, dim3(grid), dim3(256), 0, st, *a, local_sync));
@@ -1268,7 +1270,7 @@ static int launch_applier(const SfApplierArgs* a, unsigned int seq, int grid, cu
 
 extern "C" int sf_applier_launch(const SfApplierArgs* a, unsigned int seq, int grid, cudaStream_t st) {
   if (grid <= 0) grid = 96;
-  if (grid > 148) grid = 148;       // co-resident with the training kernels: 256 threads, ~5 KB smem per CTA
+  if (grid > sf_num_sms()) grid = sf_num_sms();       // co-resident with the training kernels: 256 threads, ~5 KB smem per CTA
   if (a->n_workers < 1 || a->n_workers > 8) return -6;
   switch (a->push.optimizer) {
     case SF_OPT_SGD: return launch_applier<SF_OPT_SGD>(a, seq, grid, st);
@@ -1289,7 +1291,7 @@ extern "C" int sf_applier_launch(const SfApplierArgs* a, unsigned int seq, int g
 extern "C" int sf_sync_pull_launch(const SfSyncPullArgs* a, cudaStream_t st) {
   if (a->n_shards < 1 || a->n_shards > SF_MAX_SHARDS || a->ctas_per_shard < 1) return -6;
   const int grid = a->n_shards * a->ctas_per_shard;
-  if (grid > 148) return -6;            // the agreement round needs every CTA of a shard resident
+  if (grid > sf_num_sms()) return -6;            // the agreement round needs every CTA of a shard resident
   return static_cast<int>(sf::launch(sf::sync_pull_kernel, dim3(grid), dim3(256), 0, st, *a));
 }
 

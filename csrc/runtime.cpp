@@ -117,7 +117,7 @@ struct Gemm {
 
 // ---------------------------------------------------------------------------
 // Mega: an ordered, dependency-annotated list of 128x32-tile GEMMs executed by ONE persistent launch
-// (csrc/mega_sm100.cu).  Built from prepared Gemm objects; owns the device copies of their descriptors.
+// (csrc/mega_sm90.cu).  Built from prepared Gemm objects; owns the device copies of their descriptors.
 // ---------------------------------------------------------------------------
 struct Mega {
   std::vector<std::shared_ptr<Gemm>> keep;
@@ -989,8 +989,8 @@ py::bytes pack_segs(const std::vector<std::vector<int64_t>>& rows) {
 }  // namespace
 
 PYBIND11_MODULE(_C, m) {
-  m.doc() = "sparkflow_b200 native runtime (sm_100a kernels + step-plan runner)";
-  m.attr("ARCH") = "sm_100a";
+  m.doc() = "sparkflow_b200 native runtime (sm_90a kernels + step-plan runner)";
+  m.attr("ARCH") = "sm_90a";
   m.attr("CTRL_WORDS") = static_cast<int>(SF_CTRL_WORDS);
   m.attr("CTRL_PUB") = static_cast<int>(SF_CTRL_PUB);
   m.attr("SEG_BYTES") = static_cast<int>(sizeof(SfTensorSeg));

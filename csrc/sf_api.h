@@ -1,4 +1,4 @@
-// C ABI between the sm_100a kernels (csrc/*.cu) and the host runtime (plan.cpp / bindings.cpp).
+// C ABI between the sm_90a kernels (csrc/*.cu) and the host runtime (plan.cpp / bindings.cpp).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -100,13 +100,13 @@ struct SfGemm {
   int mn_major;                   // 1: BOTH operands are MN-major: a is [K, lda] with M contiguous, b is [K, ldb] with N contiguous
                                   // (D = a^T . b, the weight-gradient form: activations / dz are consumed as they are
                                   // stored, no transposed copies); 0: both K-major (a [M, lda], b [N, ldb])
-  int pair;                       // in: -1 = auto, 0 = one-CTA kernel, 1 = force the 2-CTA persistent kernel; out: 0 / 1
-  int pair_ctas;                  // CTAs of the persistent 2-CTA kernel (0 = 148)
+  int pair;                       // in: -1 = auto, 0 = one-CTA kernel, 1 = force the persistent cluster-pair kernel; out: 0 / 1
+  int pair_ctas;                  // CTAs of the persistent cluster-pair kernel (0 = one per SM)
   SfGemmEpilogue ep;
 };
 
 // ---------------------------------------------------------------------------
-// Whole-chain GEMM kernel ("megakernel", csrc/mega_sm100.cu): ONE persistent launch executes an ordered list of
+// Whole-chain GEMM kernel ("megakernel", csrc/mega_sm90.cu): ONE persistent launch executes an ordered list of
 // 128 x 32-tile GEMMs (the forward / dgrad / wgrad chain of a dense network).  CTAs draw tile tickets from an atomic
 // counter; a tile of GEMM g starts once every tile of the GEMMs it depends on has been published (per-GEMM done
 // counters, release / acquire at gpu scope + a generic->async proxy fence before the TMA loads).
@@ -138,6 +138,7 @@ int sf_gemm_prepare(SfGemm* g);
 int sf_gemm_launch(const SfGemm* g, cudaStream_t st);
 int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st);
 int sf_gemm_pick_bn(int M, int N);
+int sf_num_sms();
 unsigned int sf_read_error_code();
 int sf_init_error_channel();
 unsigned int sf_read_host_error_code();

@@ -3,7 +3,7 @@ import os
 
 import numpy as np
 
-CANDIDATES = ["examples/mnist_train.csv", "mnist_train.csv", "/root/reference/examples/mnist_train.csv"]
+CANDIDATES = ["examples/mnist_train.csv", "mnist_train.csv"]
 
 
 def mnist_csv(rows: int = 4000) -> str:

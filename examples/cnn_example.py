@@ -1,5 +1,5 @@
 """MNIST convolutional network (conv 5x5x32 - pool - conv 3x3x64 - pool - dense 10) trained with SparkAsyncDL.
-On a B200 the step is the compiled sm_100a plan: im2col + tcgen05 GEMMs, pooling with an arg-max mask, pooling backward
+On an H100 the step is the compiled sm_90a plan: im2col + wgmma GEMMs, pooling with an arg-max mask, pooling backward
 fused with the ReLU gradient.  Same workload as the reference's cnn example.
 
     python examples/cnn_example.py [--rows N] [--iters K]

@@ -1,9 +1,9 @@
 """MNIST multi-layer perceptron (784-256-256-10) through the Spark-ML pipeline API: VectorAssembler + OneHotEncoder +
 SparkAsyncDL, saved, re-loaded through the carrier format and scored.  Same workload as the reference's simple_dnn
-example; here every partition trains on a B200 (or a CPU thread) against the device-resident parameter server.
+example; here every partition trains on an H100 (or a CPU thread) against the device-resident parameter server.
 
     python examples/simple_dnn.py [--rows N] [--iters K]           one worker per GPU / thread in this process
-    torchrun --nproc-per-node 8 examples/simple_dnn.py             one rank per B200, master on rank 0's GPU
+    torchrun --nproc-per-node 8 examples/simple_dnn.py             one rank per H100, master on rank 0's GPU
 """
 from _common import Stopwatch, mnist_frame, parse_args, pixel_columns
 

@@ -1,4 +1,4 @@
-"""Packaging for sparkflow_b200.  The native extensions are built IN-TREE by ``tools/build_ext.py`` (nvcc for sm_100a;
+"""Packaging for sparkflow_b200.  The native extensions are built IN-TREE by ``tools/build_ext.py`` (nvcc for sm_90a;
 ``sparkflow_b200/_C.so`` and ``_host.so`` sit next to the Python sources), so ``pip install -e .`` / ``python setup.py
 develop`` only has to trigger that build and register the package."""
 import os
@@ -16,7 +16,7 @@ def _build_native():
 
 
 class BuildNative(Command):
-    description = "compile the sm_100a CUDA kernels + C++ runtime into sparkflow_b200/_C.so and _host.so"
+    description = "compile the sm_90a CUDA kernels + C++ runtime into sparkflow_b200/_C.so and _host.so"
     user_options = []
 
     def initialize_options(self):
@@ -39,7 +39,7 @@ class BuildPyWithNative(build_py):
 setup(
     name="sparkflow_b200",
     version="0.1.0",
-    description="Blackwell-native asynchronous parameter-server training with the sparkflow API",
+    description="Hopper-native asynchronous parameter-server training with the sparkflow API",
     packages=find_packages(include=["sparkflow_b200", "sparkflow_b200.*"]),
     package_data={"sparkflow_b200": ["_C.so", "_host.so"]},
     python_requires=">=3.10",

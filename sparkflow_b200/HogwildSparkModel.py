@@ -1,9 +1,9 @@
 """``HogwildSparkModel``: asynchronous parameter-server training over the partitions of an RDD.
 
-Public API parity with /root/reference/sparkflow/HogwildSparkModel.py:103-272 (constructor keywords,
+Public API parity with lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:103-272 (constructor keywords,
 ``train(rdd) -> list of numpy weights``, ``stop_server()``, ``determine_master``, module-level
 ``get_server_weights`` / ``put_deltas_to_server``), with the Flask/HTTP/pickle machinery replaced by
-:class:`sparkflow_b200.parallel.session.TrainingSession` (fused NVLink push/pull kernels on B200,
+:class:`sparkflow_b200.parallel.session.TrainingSession` (fused NVLink push/pull kernels on H100,
 threads or gloo on CPU).  ``serverStartup`` is accepted and ignored: readiness is explicit, there is
 no start-up sleep.
 """

@@ -1,4 +1,4 @@
-"""sparkflow_b200 – a Blackwell-native asynchronous parameter-server training framework with the
+"""sparkflow_b200 – a Hopper-native asynchronous parameter-server training framework with the
 public API of lifeomic/sparkflow (SparkAsyncDL / SparkAsyncDLModel / HogwildSparkModel / build_graph /
 PysparkPipelineWrapper / load_tensorflow_model) and its artefact formats.
 
@@ -7,11 +7,11 @@ Layout
 ``graph/``     TF-compatible graph builder, MetaGraphDef codec, IR, PyTorch interpreter (oracle / CPU)
 ``models/``    graph -> layer-plan compiler and the model zoo
 ``ops/``       native-extension loader, flat parameter layout, optimizer rules
-``parallel/``  B200 device engine, host parameter server (threads / gloo), worker loop, sessions
+``parallel/``  H100 device engine, host parameter server (threads / gloo), worker loop, sessions
 ``spark/``     dependency-free stand-in for the used slice of PySpark (DataFrame, ML Pipeline, persistence)
 ``io/``        TF-V2 checkpoint bundles, CSV
 ``utils/``     timing, clocks, tracing, metrics, fault injection
-``csrc/``      (repo root) sm_100a kernels + C++ runtime
+``csrc/``      (repo root) sm_90a kernels + C++ runtime
 """
 __version__ = "0.2.0"
 

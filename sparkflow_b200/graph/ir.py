@@ -2,7 +2,7 @@
 
 The reference moves models around as ``json_format.MessageToJson(MetaGraphDef)`` strings and parses
 them back on the parameter server, on every worker and in ``predict_func``
-(/root/reference/sparkflow/HogwildSparkModel.py:45-53,131-132,188-192; ml_util.py:57-69).  GraphIR is
+(lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:45-53,131-132,188-192; ml_util.py:57-69).  GraphIR is
 our parsed form: nodes with decoded attrs, the trainable variables in collection order (this order
 is the order of every weights list in the public API) and the ``losses`` collection.
 """

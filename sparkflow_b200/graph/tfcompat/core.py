@@ -1,7 +1,7 @@
 """Graph / Tensor / Variable primitives of the TensorFlow-1.x compatible graph builder.
 
 The reference serialises user models with ``tf.train.export_meta_graph`` inside ``build_graph``
-(/root/reference/sparkflow/graph_utils.py:6-15).  TensorFlow cannot be installed here, so this
+(lifeomic/sparkflow/sparkflow/graph_utils.py:6-15).  TensorFlow cannot be installed here, so this
 package provides the slice of the TF-1.x graph-construction API that the reference, its examples
 and its tests use, emitting *TensorFlow-compatible* NodeDefs (same op names, attrs, variable /
 initializer / read-node naming, collections) so that the MetaGraphDef JSON we produce has the layout

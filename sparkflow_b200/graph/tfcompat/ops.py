@@ -1,6 +1,6 @@
 """Graph-building ops of the TF-1.x compatible builder: constants, variables + initializers, math,
 ``tf.nn`` / ``tf.layers`` / ``tf.losses``.  Node/attr layouts mirror what TF-1.x emits for the same
-calls (cf. the nodes decoded from /root/reference/tests/test_model/to_load.meta: ``dense/kernel``,
+calls (cf. the nodes decoded from lifeomic/sparkflow/tests/test_model/to_load.meta: ``dense/kernel``,
 ``dense/kernel/Initializer/random_uniform/{shape,min,max,RandomUniform,sub,mul}``, ``dense/kernel/
 Assign``, ``dense/kernel/read``, ``dense/MatMul``, ``dense/BiasAdd``, ``dense/Tanh`` ...).
 """

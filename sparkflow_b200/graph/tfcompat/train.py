@@ -1,9 +1,9 @@
 """``tf.train``: optimizer descriptors, MetaGraph import/export and a TF-bundle ``Saver``.
 
 The reference hands ``tf.train.*Optimizer`` instances to the parameter server, which only ever calls
-``optimizer.apply_gradients`` on the master (/root/reference/sparkflow/HogwildSparkModel.py:194).
+``optimizer.apply_gradients`` on the master (lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:194).
 Here the optimizer classes are thin constructors of :class:`OptimizerSpec`, which is what the master
-(torch on CPU, the fused push kernel on B200) consumes.
+(torch on CPU, the fused push kernel on H100) consumes.
 """
 from __future__ import annotations
 

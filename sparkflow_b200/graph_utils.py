@@ -1,6 +1,6 @@
 """``build_graph`` and the optimizer-config builders.
 
-API parity with /root/reference/sparkflow/graph_utils.py (build_graph :6-15, config builders :18-47).
+API parity with lifeomic/sparkflow/sparkflow/graph_utils.py (build_graph :6-15, config builders :18-47).
 ``build_graph(func)`` runs ``func`` inside a fresh graph and returns the MetaGraphDef as proto3 JSON.
 With real TensorFlow 1.x importable, its ``tf.Graph``/``export_meta_graph`` are used; otherwise the
 built-in TF-compatible builder (``sparkflow_b200.graph.tfcompat``) produces the same JSON layout.

@@ -1,7 +1,7 @@
 """TensorFlow V2 checkpoint bundles (``<prefix>.index`` + ``<prefix>.data-00000-of-00001``) and the
 ``checkpoint`` state file – read AND write, without TensorFlow.
 
-Layout (SURVEY.md section 2.5-5; decoded from /root/reference/tests/test_model): the index is a
+Layout (SURVEY.md section 2.5-5; decoded from lifeomic/sparkflow/tests/test_model): the index is a
 leveldb-format SSTable whose first key ``""`` maps to a ``BundleHeaderProto`` and every other key
 (a variable name, lexicographically sorted) to a ``BundleEntryProto{dtype, shape, shard_id, offset, size,
 crc32c}``; the data file is the raw little-endian tensor bytes at those offsets; ``crc32c`` is the

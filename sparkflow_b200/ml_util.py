@@ -1,8 +1,8 @@
-"""Tensor / batching / prediction utilities (API parity with /root/reference/sparkflow/ml_util.py).
+"""Tensor / batching / prediction utilities (API parity with lifeomic/sparkflow/sparkflow/ml_util.py).
 
 Differences by design: weights are bound by name to the parsed graph (no per-call assign ops – the
 reference leaks a placeholder+assign pair per variable per pull, ml_util.py:16-28), and prediction
-runs the compiled sm_100a forward plan when a GPU is present.
+runs the compiled sm_90a forward plan when a GPU is present.
 """
 from __future__ import annotations
 
@@ -96,7 +96,7 @@ _PREDICTORS: Dict[Tuple[int, str, str], Any] = {}
 
 def run_inference(graph_json: str, weights: Sequence[np.ndarray], features: np.ndarray, tf_input: str, tf_output: str,
                   tf_dropout: Optional[str] = None, to_keep_dropout: bool = False) -> np.ndarray:
-    """Forward pass of ``tf_output`` for a feature matrix.  GPU: compiled forward plan (tcgen05 GEMMs with
+    """Forward pass of ``tf_output`` for a feature matrix.  GPU: compiled forward plan (wgmma GEMMs with
     fused bias/activation, ArgMax kernel); otherwise (or for graphs outside the compiled family) the
     interpreter."""
     import torch

@@ -1,6 +1,6 @@
-"""GraphIR -> LayerPlan: recognise the layer structure the B200 engine has hand-written kernels for.
+"""GraphIR -> LayerPlan: recognise the layer structure the H100 engine has hand-written kernels for.
 
-The reference runs whatever graph the user serialised through a TF session.  The B200 engine
+The reference runs whatever graph the user serialised through a TF session.  The H100 engine
 instead executes a *compiled* plan: the forward chain between ``tfInput`` and the loss is pattern-
 matched into dense / conv / pool / reshape layers with fused bias+activation, the loss into
 softmax-cross-entropy or mean-squared-error, ``tf.nn.dropout`` / ``tf.layers.dropout`` after a dense layer into a
@@ -22,7 +22,7 @@ ACT_IDS = {None: 0, "Relu": 1, "Sigmoid": 2, "Tanh": 3}
 
 
 class UnsupportedGraph(ValueError):
-    """The graph is valid but outside the family the compiled B200 plan covers."""
+    """The graph is valid but outside the family the compiled H100 plan covers."""
 
 
 @dataclass

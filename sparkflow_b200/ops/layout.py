@@ -1,10 +1,10 @@
 """Flat parameter layout shared by the master, the replicas and the push/pull kernels.
 
 The reference ships parameters as a python list of per-variable numpy arrays in
-``tf.trainable_variables()`` order (/root/reference/sparkflow/ml_util.py:9-28).  On the GPU all
+``tf.trainable_variables()`` order (lifeomic/sparkflow/sparkflow/ml_util.py:9-28).  On the GPU all
 variables live in ONE flat fp32 buffer (params, gradients and every optimizer slot use the same
 offsets) so that a push is a single multi-tensor kernel launch, plus ONE bf16 "publish" buffer that
-holds, for every matrix, the two K-major operand layouts the tcgen05 GEMMs consume:
+holds, for every matrix, the two K-major operand layouts the wgmma GEMMs consume:
 
 * ``W``   [in, ld]  row-major  – B operand of dgrad  (dx = dy . W^T)
 * ``W^T`` [out, ld] row-major  – B operand of forward (y = x . W)

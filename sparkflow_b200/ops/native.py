@@ -1,6 +1,6 @@
 """Loader for the in-tree native extensions.
 
-``_C``    – sm_100a kernels + C++ step-plan runtime (needs a B200 at run time, imports anywhere)
+``_C``    – sm_90a kernels + C++ step-plan runtime (needs an H100 at run time, imports anywhere)
 ``_host`` – CPU-only native helpers (TF bundle codec, crc32c, carrier codec, CSV reader)
 
 On a GPU box the CUDA path is THE path: if ``_C.so`` is missing we fail loudly instead of silently
@@ -66,7 +66,7 @@ WAIT_CODES = {0x100: "gemm: TMA producer waiting for a free smem stage", 0x200: 
 
 
 def cuda_ext() -> ModuleType:
-    """The sm_100a kernel/runtime module (``sparkflow_b200._C``).  On a CUDA machine the first call per device
+    """The sm_90a kernel/runtime module (``sparkflow_b200._C``).  On a CUDA machine the first call per device
     also installs the host-visible error word that bounded device waits write before trapping."""
     mod = _load("_C")
     try:
@@ -95,6 +95,13 @@ def describe_device_error() -> str:
 def host_ext() -> ModuleType:
     """The CPU-only native helper module (``sparkflow_b200._host``)."""
     return _load("_host")
+
+
+def num_sms() -> int:
+    """SMs of the current CUDA device (132, an H100 SXM, when no device is visible)."""
+    import torch
+
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count if torch.cuda.is_available() else 132
 
 
 def ptr(t) -> int:

@@ -1,8 +1,8 @@
 """The ten optimizers of the reference's factory, as flat multi-tensor update rules.
 
 Reference: ``build_optimizer`` maps ten names to ``tf.train.*Optimizer`` classes
-(/root/reference/sparkflow/tensorflow_async.py:17-42) and the parameter server applies **one
-optimizer step per pushed gradient** (/root/reference/sparkflow/HogwildSparkModel.py:194,232).
+(lifeomic/sparkflow/sparkflow/tensorflow_async.py:17-42) and the parameter server applies **one
+optimizer step per pushed gradient** (lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:194,232).
 
 Here every optimizer is a :class:`OptimizerSpec` (name + normalised hyper-parameters).  The update
 math exists twice with identical semantics (TF-1.x ``training_ops`` formulas):

@@ -1,13 +1,13 @@
-"""B200 engine: master parameter state + per-GPU worker that executes compiled step plans.
+"""H100 engine: master parameter state + per-GPU worker that executes compiled step plans.
 
-Mapping of the reference's runtime (SURVEY.md sections 1, 3.1, 5.1) onto one B200 box:
+Mapping of the reference's runtime (SURVEY.md sections 1, 3.1, 5.1) onto one H100 box:
 
 * parameter-server process (Flask, HogwildSparkModel.py:175-244)  ->  :class:`MasterState`, one
   cudaMalloc'ed segment on the driver GPU holding the flat fp32 params, the optimizer slots, the bf16
   publish buffer and a 256-byte control block (RW lock word, version, step counters).  The segment
   is exported with CUDA IPC so every worker process addresses it over NVLink.
 * Spark partition worker (``handle_model``, HogwildSparkModel.py:38-100)  ->  :class:`DeviceWorker`:
-  one process per GPU.  A training step is a *compiled plan* – pull, input cast, tcgen05 GEMMs with
+  one process per GPU.  A training step is a *compiled plan* – pull, input cast, wgmma GEMMs with
   fused epilogues, loss kernel, wgrad/dgrad GEMMs, fused push – captured once into a CUDA graph and
   replayed, so a step costs one graph launch on the host.
 * ``GET /parameters`` -> ``pull`` kernel (or TMA reads of the master's publish buffer straight from
@@ -337,7 +337,7 @@ class DeviceWorker:
             # snapshot pull: the copy is latency bound, so give every shard as many CTAs as it has tiles (all CTAs of the
             # kernel must be co-resident for the per-shard version agreement: at most one CTA per SM in total)
             tiles_per_shard = max(1, -(-m.n_tiles // m.n))
-            self.sync_cps = max(1, min(tiles_per_shard, 148 // m.n, int(os.environ.get("SPARKFLOW_PULL_CTAS_PER_SHARD", "16"))))
+            self.sync_cps = max(1, min(tiles_per_shard, native.num_sms() // m.n, int(os.environ.get("SPARKFLOW_PULL_CTAS_PER_SHARD", "16"))))
             init = torch.zeros(8, 8, dtype=torch.int64)
             init[:, 1] = 0xFFFFFFFF
             self.sync_sp = torch.from_numpy(init.numpy().astype("uint32").view("int32").copy()).to(dev)

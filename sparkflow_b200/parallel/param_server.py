@@ -1,6 +1,6 @@
 """Host parameter server: the CPU / gloo twin of the fused GPU push/pull path.
 
-Reference behaviour that is preserved (/root/reference/sparkflow/HogwildSparkModel.py:175-244):
+Reference behaviour that is preserved (lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:175-244):
   * the master holds the weights AND all optimizer state; workers only ever send raw gradients;
   * ONE optimizer step per push, gradients are never summed across workers;
   * ``acquire_lock=False`` (Hogwild): pulls and updates race freely; ``True``: writer-priority RW lock;

@@ -1,4 +1,4 @@
-"""LayerPlan -> native step plan (list of sm_100a kernel launches, later a CUDA graph).
+"""LayerPlan -> native step plan (list of sm_90a kernel launches, later a CUDA graph).
 
 Supported layer grammar (anything else is reported as UnsupportedGraph and handled by the generic engine):
 
@@ -95,7 +95,7 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
 def _split_k(tiles: int, kblocks: int) -> int:
     if kblocks < 16:
         return 1
-    return max(1, min(148 // max(tiles, 1), kblocks // 4))
+    return max(1, min(native.num_sms() // max(tiles, 1), kblocks // 4))
 
 
 def _emit_mega(plan, C, items: List[List[Any]], keep: List[Any]) -> None:
@@ -241,7 +241,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     elif do_pull:
         add_pull_op()
     first_is_dense = layers[first_trainable].kind == "dense"
-    # weight gradients read the row-major activation / dz buffers directly (MN-major tcgen05 operands): no transposed copy
+    # weight gradients read the row-major activation / dz buffers directly (MN-major wgmma operands): no transposed copy
     # of any activation, gradient or im2col matrix is ever written.  (The opt-in megakernel only has K-major tiles.)
     use_mn = bool(train and use_mn_possible(worker, layers, train))
     if inputs is not None:

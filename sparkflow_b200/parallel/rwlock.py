@@ -1,6 +1,6 @@
 """Writer-priority readers/writer lock (host side).
 
-Same contract as the reference's lock (/root/reference/sparkflow/RWLock.py:10-65): many readers XOR
+Same contract as the reference's lock (lifeomic/sparkflow/sparkflow/RWLock.py:10-65): many readers XOR
 one writer; readers are held back while a writer holds the lock *or is waiting for it*, so updates
 cannot starve.  Used by the host parameter server when ``acquire_lock=True``; the GPU path uses the
 device-side twin in ``csrc/optim_push.cu`` (same state machine on one 32-bit word).

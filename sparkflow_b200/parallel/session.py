@@ -12,7 +12,7 @@ single process, CPU             worker threads + in-process ParameterServer (Spa
 =============================  =================================================================
 
 The reference's fixed costs are gone: no server process spawn, no 8 s sleep
-(/root/reference/sparkflow/HogwildSparkModel.py:118,135) – ``open`` returns once the master is ready.
+(lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:118,135) – ``open`` returns once the master is ready.
 """
 from __future__ import annotations
 
@@ -75,12 +75,12 @@ class TrainingSession:
 
                 check_grammar(compile_graph(self.ir, tf_input, tf_label))
                 self.engine_kind = "b200"
-                self.engine_reason = "graph compiled to the native sm_100a plan"
+                self.engine_reason = "graph compiled to the native sm_90a plan"
             except UnsupportedGraph as exc:
                 if engine == "b200":
                     raise
                 self.engine_reason = f"graph outside the compiled plan family: {exc}"
-                warnings.warn(f"sparkflow_b200: graph is outside the compiled sm_100a plan family ({exc}); "
+                warnings.warn(f"sparkflow_b200: graph is outside the compiled sm_90a plan family ({exc}); "
                               "running the generic PyTorch interpreter engine on the GPU instead", RuntimeWarning)
         elif engine == "b200":
             raise RuntimeError("engine='b200' requested but no CUDA device is available")

@@ -1,7 +1,7 @@
 """Sharded parameter server: the master state is partitioned over ALL GPUs of the box.
 
 The reference has ONE parameter server on the Spark driver: every ``GET /parameters`` and ``POST /update`` terminates
-there (/root/reference/sparkflow/HogwildSparkModel.py:206-244).  On a B200 box that star topology wastes 7/8 of the
+there (lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:206-244).  On an H100 box that star topology wastes 7/8 of the
 NVLink ports and serialises every optimizer step on one GPU.  Here (SURVEY.md section 5.1, "sharded master"):
 
 * the flat state (one ``(p, slot0, slot1, slot2)`` tuple per parameter) is split by *push tile* (32 x 64 elements of one

@@ -6,7 +6,7 @@ Every GPU of the job allocates a segment with the SAME layout through the CUDA v
 the multicast alias (``multimem.st`` in the kernels) is replicated by the switch into every GPU's segment.
 
 This replaces the reference's transport rendezvous (``master_url`` + Flask port + 8 s sleep,
-/root/reference/sparkflow/HogwildSparkModel.py:118-135,145-166): there is no server address, only mapped memory.
+lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:118-135,145-166): there is no server address, only mapped memory.
 
 Two process models:
 

@@ -1,6 +1,6 @@
 """The per-partition training loop (engine-agnostic) and the two engines that execute its steps.
 
-Loop semantics are the reference's ``handle_model`` (/root/reference/sparkflow/HogwildSparkModel.py:38-100):
+Loop semantics are the reference's ``handle_model`` (lifeomic/sparkflow/sparkflow/HogwildSparkModel.py:38-100):
 
 * per outer iteration: pull, optional shuffle, then ONE of
   A. ``mini_stochastic_iters >= 1`` – that many random minibatches (without replacement inside a batch),
@@ -13,7 +13,7 @@ Loop semantics are the reference's ``handle_model`` (/root/reference/sparkflow/H
 Engines:
 * :class:`TorchEngine` – GraphProgram (autograd) + a host transport (threads or gloo). CPU path, and the
   generic path for graphs the compiled plan does not cover.
-* :class:`B200Engine`  – DeviceWorker: compiled sm_100a step plans, pinned-host partitions fed through
+* :class:`B200Engine`  – DeviceWorker: compiled sm_90a step plans, pinned-host partitions fed through
   a side stream, fused NVLink push/pull.
 """
 from __future__ import annotations
@@ -200,7 +200,7 @@ class B200Engine(Engine):
 
     def load_partition(self, features, labels):
         """``SPARKFLOW_PARTITION=pinned`` (default): the partition stays in pinned host memory and every step copies its
-        minibatch host->device.  ``resident``: the partition is uploaded to HBM once (180 GB per B200 hold any Spark
+        minibatch host->device.  ``resident``: the partition is uploaded to HBM once (80 GB per H100 hold any Spark
         partition the reference could train on); shuffles are a device index permutation and every step gathers its rows
         on the device - no PCIe traffic in the training loop.  ``auto``: resident when it fits in a quarter of free HBM."""
         self.X = torch.as_tensor(np.ascontiguousarray(features, dtype=np.float32)).pin_memory()
@@ -342,9 +342,8 @@ class B200Engine(Engine):
         in the loop.  ``SPARKFLOW_H2D=dma`` (default): copy-engine H2D of every minibatch on a side stream, SLOTS-deep,
         event hand-off to the step graph.  ``SPARKFLOW_H2D=fetch``: every step's CUDA graph fetches the NEXT minibatch
         from the pinned partition itself (zero-copy SM loads + cast on a side branch), so a step costs the host one
-        ``cudaGraphLaunch`` and nothing sits between two graphs.  Measured on this pod (profiles/r1_e2e_h2d_modes.md):
-        fetch removes the cast from the critical path (step 55 vs 57 us) but SM reads of cold host pages run at
-        ~20 GB/s vs 40 GB/s for the DMA engine, so dma is the faster end-to-end choice here."""
+        ``cudaGraphLaunch`` and nothing sits between two graphs.  Fetch takes the cast off the critical path, but SM
+        reads of cold host pages are slower than the DMA engine, which is why dma is the default."""
         w = self.w
         if not w.use_graphs or len(starts) == 0:
             for s0 in starts:

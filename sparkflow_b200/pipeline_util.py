@@ -1,6 +1,6 @@
 """Persistence of pure-python pipeline stages through a ``StopWordsRemover`` *carrier*.
 
-Format parity with /root/reference/sparkflow/pipeline_util.py:16-127: a stage is ``dill``-pickled,
+Format parity with lifeomic/sparkflow/sparkflow/pipeline_util.py:16-127: a stage is ``dill``-pickled,
 zlib-compressed, written as ONE string of decimal byte values each followed by ``','``, and stored as
 ``stopWords = [payload, GUID]`` of a ``StopWordsRemover`` that carries the python object's uid; loading
 recognises carriers by the GUID in the last stop word.  The byte<->decimal codec is native

@@ -1,7 +1,7 @@
 """Which Spark do the API classes build on?
 
-The reference *is* a ``pyspark.ml`` Estimator / Model (/root/reference/sparkflow/tensorflow_async.py:51,102) and persists
-through the JVM ``JavaMLWriter`` (/root/reference/sparkflow/pipeline_util.py:85-127).  When a genuine PySpark is importable
+The reference *is* a ``pyspark.ml`` Estimator / Model (lifeomic/sparkflow/sparkflow/tensorflow_async.py:51,102) and persists
+through the JVM ``JavaMLWriter`` (lifeomic/sparkflow/sparkflow/pipeline_util.py:85-127).  When a genuine PySpark is importable
 ``SparkAsyncDL`` / ``SparkAsyncDLModel`` / ``PysparkReaderWriter`` derive from ITS classes - they sit in a real
 ``Pipeline``, take real DataFrames and save through ``JavaMLWriter``; otherwise (this image: no pyspark, no JVM) they
 derive from the dependency-free stand-ins under ``sparkflow_b200.spark`` with the same behaviour and on-disk layout.
@@ -48,7 +48,7 @@ if not REAL_PYSPARK:
 
 
 def collect_partitions(rdd):
-    """The rows of every partition of ``rdd`` on the driver: the B200 engine trains on the GPUs of the driver's box, the
+    """The rows of every partition of ``rdd`` on the driver: the H100 engine trains on the GPUs of the driver's box, the
     partitions are its workers' shards (reference: ``rdd.foreachPartition(handle_model)``, HogwildSparkModel.py:259)."""
     if hasattr(rdd, "partitions") and callable(rdd.partitions):
         return [list(p) for p in rdd.partitions()]          # stand-in RDD

@@ -1,12 +1,12 @@
 """``SparkAsyncDL`` (Estimator) and ``SparkAsyncDLModel`` (Model).
 
-Public API parity with /root/reference/sparkflow/tensorflow_async.py: the same 21 Params with the same
+Public API parity with lifeomic/sparkflow/sparkflow/tensorflow_async.py: the same 21 Params with the same
 defaults (:176-182), ``@keyword_only`` constructor/``setParams``, the same getters (including the
 historically misspelt ``getAqcuireLock``, :245), ``build_optimizer`` with its quirks (options replace
 ``tfLearningRate``; unknown names fall back to SGD, :32-42), ``_fit`` -> ``HogwildSparkModel.train`` ->
 weights JSON -> ``SparkAsyncDLModel`` and ``_transform`` = per-partition ``predict_func``.
 
-Params are declared from a table instead of one statement each; the engine underneath is the B200
+Params are declared from a table instead of one statement each; the engine underneath is the H100
 parameter-server runtime instead of Flask + TF sessions.
 """
 from __future__ import annotations

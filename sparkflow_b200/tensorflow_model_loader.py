@@ -1,6 +1,6 @@
 """Load a pre-trained TensorFlow checkpoint (``<path>.meta`` + V2 bundle) as a ``SparkAsyncDLModel``.
 
-API parity with /root/reference/sparkflow/tensorflow_model_loader.py:8-45, implemented without
+API parity with lifeomic/sparkflow/sparkflow/tensorflow_model_loader.py:8-45, implemented without
 TensorFlow: the binary MetaGraphDef is decoded by ``graph.pbwire`` and the ``.index`` / ``.data``
 bundle by the native TF-bundle reader (``io.bundle``).
 """

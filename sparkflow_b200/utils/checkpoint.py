@@ -3,7 +3,7 @@
 The reference never checkpoints during training: the master lives only in the Flask process' memory
 (SURVEY.md section 5).  Here the master's parameters AND optimizer slots can be written as a TF checkpoint with
 the names TF itself would use (``<var>``, ``<var>/Adam``, ``<var>/Adam_1``, ``beta1_power``, ``beta2_power`` –
-compare the keys of /root/reference/tests/test_model/to_load.index), so a snapshot is loadable by
+compare the keys of lifeomic/sparkflow/tests/test_model/to_load.index), so a snapshot is loadable by
 ``load_tensorflow_model`` (and by TensorFlow), and training can resume from it with identical optimizer state.
 """
 from __future__ import annotations

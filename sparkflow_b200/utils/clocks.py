@@ -1,4 +1,4 @@
-"""nvidia-smi clock / throttle sampler used while a timed region runs (B200_PROFILING.md recipe)."""
+"""nvidia-smi clock / throttle sampler used while a timed region runs (read-only queries)."""
 from __future__ import annotations
 
 import shutil

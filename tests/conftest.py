@@ -12,7 +12,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `pytest -m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU of compute capability 9.0 (H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -65,7 +65,7 @@ def pytest_terminal_summary(terminalreporter, exitstatus, config):
 @pytest.fixture(scope="session")
 def tf_checkpoint(tmp_path_factory):
     """A self-generated TF-V2 checkpoint of the reference fixture's architecture (2-10 tanh-10 tanh-1 sigmoid, Adam
-    slots, beta powers: the key set of /root/reference/tests/test_model/to_load.index) written by this package's own
+    slots, beta powers: the key set of tests/golden/test_model/to_load.index) written by this package's own
     bundle writer - the suite does not depend on the reference tree being mounted."""
     import numpy as np
 

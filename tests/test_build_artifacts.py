@@ -1,7 +1,7 @@
 """No-GPU checks on the built kernel library (`cuobjdump` on sparkflow_b200/_C.so): the hot kernels must not keep their
 working set in local memory (round 2 found the optimizer tile code spilling its whole tile state because one fallback loop
 indexed a register array with a runtime bound: 34 % of the push kernel's stall samples were `STL`), and the GEMMs must be
-tcgen05 / TMA kernels."""
+wgmma / TMA kernels."""
 import os
 import re
 import shutil
@@ -35,11 +35,11 @@ def test_hot_kernels_have_no_stack_frame():
     assert all(use[k][0] * 256 * 2 <= 65536 for k in use if k.startswith("sf::push_kernel")), {k: v for k, v in use.items() if "push_kernel" in k}
 
 
-def test_gemm_kernels_are_tcgen05_tma_kernels():
+def test_gemm_kernels_are_wgmma_tma_kernels():
     fn = subprocess.run(["cuobjdump", "-sass", "-fun", "_ZN2sf14sf_gemm_kernelILi32ELb0EEEv14CUtensorMap_stS1_14SfGemmEpilogueiiii", SO],
                         stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout
     if "Function" not in fn:
         pytest.skip("cuobjdump -fun did not find the mangled name (toolkit version)")
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR", "UTCATOMSWS", "SYNCS", "ACQBULK"):
+    for mnemonic in ("HGMMA", "WARPGROUP", "UTMALDG", "SYNCS"):
         assert mnemonic in fn, f"{mnemonic} missing from sf_gemm_kernel<32, false>"
-    assert "HMMA." not in fn.replace("UTCHMMA", "")          # no legacy mma.sync path
+    assert "HMMA." not in fn                                  # no legacy mma.sync path

@@ -1,4 +1,4 @@
-"""End-to-end numerics of the compiled B200 step (pull -> fwd -> loss -> bwd -> push) against the
+"""End-to-end numerics of the compiled H100 step (pull -> fwd -> loss -> bwd -> push) against the
 PyTorch-autograd oracle running the reference semantics on the CPU."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""The reference's integration suite (/root/reference/tests/dl_runner.py:97-312) re-expressed against
+"""The reference's integration suite (tests/dl_runner.py:97-312 of the reference project) re-expressed against
 this framework, written the way a sparkflow user would write it: through the ``sparkflow`` /
 ``pyspark`` / ``tensorflow`` import paths (provided by ``sparkflow_b200.compat.install()`` when the real
 packages are absent).  Assertions are the reference's statistical smoke checks (errors < N of 10)."""

@@ -23,14 +23,13 @@ from sparkflow_b200.ops.layout import ParamLayout
 from sparkflow_b200.ops.optimizers import NUM_SLOTS, OPT_IDS, OptimizerSpec, apply_update, init_slots
 from sparkflow_b200.parallel.rwlock import RWLock
 
-FIXTURE = "/root/reference/tests/test_model/to_load"
-HAVE_FIXTURE = os.path.exists(FIXTURE + ".meta")
+# the reference project's TF-1.7 checkpoint of its test model (graph .meta, V2 bundle, checkpoint state file)
+FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "test_model", "to_load")
 
 
 # ---------------------------------------------------------------------------------------------
 # protobuf codec
 # ---------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not HAVE_FIXTURE, reason="reference fixture not mounted")
 def test_pbwire_decodes_real_tf_metagraph():
     mg = pbwire.decode("MetaGraphDef", open(FIXTURE + ".meta", "rb").read())
     assert len(mg["graphDef"]["node"]) == 264 and mg["metaInfoDef"]["tensorflowVersion"] == "1.7.0"
@@ -293,7 +292,6 @@ def test_param_layout_tables():
     assert lay.tile_map().shape == (25 * 4 + 4 + 8 + 1, 3)
 
 
-@pytest.mark.skipif(not HAVE_FIXTURE, reason="reference fixture not mounted")
 def test_bundle_reader_and_writer_are_byte_exact(tmp_path):
     from sparkflow_b200.io.bundle import read_bundle, read_checkpoint_state, write_bundle
 

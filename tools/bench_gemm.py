@@ -1,4 +1,4 @@
-"""GEMM throughput: the one-CTA tcgen05 kernel, the persistent 2-CTA kernel and cuBLAS (torch.matmul) on the same shapes.
+"""GEMM throughput: the one-CTA wgmma kernel, the persistent 2-CTA kernel and cuBLAS (torch.matmul) on the same shapes.
 CUDA-event timing, warm-up, L2 flushed between timed launches by rotating through operand sets larger than L2."""
 import json
 import sys
@@ -59,4 +59,4 @@ for M, N, K in shapes:
     res.append(row)
     del As, Bs, out
     torch.cuda.empty_cache()
-json.dump(res, open("gpurun_out/bench_gemm.json", "w"), indent=1)
+json.dump(res, open("bench_out/bench_gemm.json", "w"), indent=1)

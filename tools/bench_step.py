@@ -1,4 +1,4 @@
-"""Device-side microbenchmarks: tcgen05 GEMM vs torch.matmul, and the compiled training step."""
+"""Device-side microbenchmarks: wgmma GEMM vs torch.matmul, and the compiled training step."""
 import json
 import sys
 import time
@@ -105,5 +105,5 @@ if __name__ == "__main__":
         out["step"].append(bench_step(*cfg))
         print(json.dumps(out["step"][-1]), flush=True)
     import os
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(out, open("gpurun_out/bench_step.json", "w"), indent=1)
+    os.makedirs("bench_out", exist_ok=True)
+    json.dump(out, open("bench_out/bench_step.json", "w"), indent=1)

@@ -1,10 +1,10 @@
 """In-tree build of the native extensions.
 
-* ``sparkflow_b200/_C.so``    – sm_100a kernels (csrc/kernels.cu) + host runtime (csrc/runtime.cpp)
+* ``sparkflow_b200/_C.so``    – sm_90a kernels (csrc/kernels.cu) + host runtime (csrc/runtime.cpp)
 * ``sparkflow_b200/_host.so`` – CPU-only native helpers (TF bundle codec, crc32c, carrier codec, CSV)
 
-nvcc cross-compiles for sm_100a without a GPU; the resulting ``.so`` files are git-ignored but travel
-to the GPU box with the gpurun snapshot.  Objects are cached by source hash under ``build/``.
+nvcc cross-compiles for sm_90a without a GPU; the resulting ``.so`` files are git-ignored.  Objects are cached by
+source hash under ``build/``.
 """
 from __future__ import annotations
 
@@ -24,7 +24,7 @@ PKG = ROOT / "sparkflow_b200"
 
 NVCC = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 CXX = os.environ.get("CXX") or shutil.which("g++") or "g++"
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _includes() -> list[str]:
@@ -87,7 +87,7 @@ def build(verbose_ptxas: bool = False, only: str | None = None) -> dict[str, Pat
         if only in (None, "host") and (CSRC / "hostlib.cpp").exists():
             jobs["hostlib"] = ex.submit(_compile_cxx, "hostlib", [CSRC / "hostlib.cpp"])
         objs = {k: f.result() for k, f in jobs.items()}
-    # keep only the objects just used: stale ones would otherwise travel with every gpurun snapshot
+    # keep only the objects just used: stale ones would otherwise pile up under build/
     for k, keep in objs.items():
         for old in BUILD.glob(f"{k}.*.o"):
             if old != keep:

@@ -37,5 +37,5 @@ out = dict(slots=eng.SLOTS, no_h2d=os.environ.get("SPARKFLOW_DRV_NO_H2D", "0"), 
            h2d_late_frac=float(np.mean(h2d_late > 0)), h2d_late_us_p90=float(np.percentile(h2d_late, 90)),
            first_rows=[[round(float(v), 1) for v in r] for r in np.c_[step, ready - start[0], start - start[0], end - start[0]][:20]])
 print(json.dumps(out))
-json.dump(out, open("gpurun_out/e2e_probe_%s_%s.json" % (eng.SLOTS, out["no_h2d"]), "w"))
+json.dump(out, open("bench_out/e2e_probe_%s_%s.json" % (eng.SLOTS, out["no_h2d"]), "w"))
 sess.close()

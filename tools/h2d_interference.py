@@ -76,5 +76,5 @@ for name, fn in (("dma_alone", dma), ("zero_copy32_alone", zc(32)), ("zero_copy9
     out[name] = dict(side_us_each=s0.elapsed_time(s1) * 1e3 / 200, GBs=nbytes / (s0.elapsed_time(s1) * 1e-3 / 200) / 1e9)
 assert torch.equal(dst[(199) % 4].cpu(), host[199 % 64])
 print(json.dumps(out, indent=1))
-json.dump(out, open("gpurun_out/h2d_interference.json", "w"), indent=1)
+json.dump(out, open("bench_out/h2d_interference.json", "w"), indent=1)
 sess.close()

@@ -1,6 +1,6 @@
 """Top stall sites of a kernel from an .ncu-rep captured with --import-source on (SASS view of the source page).
 
-    python tools/ncu_hotspots.py gpurun_out/prof_gemm_pair8192.ncu-rep [N]
+    python tools/ncu_hotspots.py bench_out/prof_gemm_pair8192.ncu-rep [N]
 """
 import csv
 import subprocess

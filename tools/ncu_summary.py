@@ -1,7 +1,7 @@
 """Summarise an .ncu-rep (captured with `ncu --set full --clock-control none --import-source on`) as a markdown
-table: one row per captured kernel with the metrics the B200 profiling recipe asks for.
+table: one row per captured kernel with the metrics the H100 profiling recipe asks for.
 
-    python tools/ncu_summary.py gpurun_out/prof_step.ncu-rep > profiles/r1_ncu_step.md
+    python tools/ncu_summary.py bench_out/prof_step.ncu-rep > profiles/r1_ncu_step.md
 """
 import csv
 import subprocess

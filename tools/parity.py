@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Convergence parity: the bf16 sm_100a engine vs the fp32 oracle, same init, same minibatch sequence.
+"""Convergence parity: the bf16 sm_90a engine vs the fp32 oracle, same init, same minibatch sequence.
 
 The reference computes in fp32 (TF-1.x CPU kernels); the engine runs its GEMMs in bf16 with fp32 accumulation and
 keeps fp32 master weights / optimizer state.  This tool trains the same model both ways on LEARNABLE synthetic data
 (10 Gaussian blobs in 784-D for the classifiers, low-rank data for the autoencoders) for >= 500 steps, one optimizer step
 per push, and records the two loss curves, the final losses / accuracies and the weight distance.
 
-    python tools/parity.py --steps 600 --out gpurun_out/parity.json        (needs a B200)
+    python tools/parity.py --steps 600 --out bench_out/parity.json        (needs an H100)
 """
 from __future__ import annotations
 
@@ -94,7 +94,7 @@ def main():
     ap.add_argument("--steps", type=int, default=600)
     ap.add_argument("--batch", type=int, default=300)
     ap.add_argument("--models", default="simple_dnn,autoencoder,cnn")
-    ap.add_argument("--out", default="gpurun_out/parity.json")
+    ap.add_argument("--out", default="bench_out/parity.json")
     args = ap.parse_args()
     res = []
     for m in args.models.split(","):

@@ -1,6 +1,6 @@
-"""Launch the tcgen05 GEMM a few times for an `ncu --set full` capture (one GPU, short).
+"""Launch the wgmma GEMM a few times for an `ncu --set full` capture (one GPU, short).
 
-    ncu --set full --clock-control none --import-source on -k regex:sf_gemm_kernel -s 4 -c 2 -o gpurun_out/prof_gemm \
+    ncu --set full --clock-control none --import-source on -k regex:sf_gemm_kernel -s 4 -c 2 -o bench_out/prof_gemm \
         python tools/profile_gemm.py 4096 4096 4096
 """
 import sys

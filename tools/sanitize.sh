@@ -5,10 +5,10 @@
 # on the lock-mode and single-kernel tests.
 TOOL=${1:-memcheck}
 EXPR=${2:-"cast_transpose or softmax or mse or argmax or gemm_plain or push_matches or pull_copies or fetch"}
-mkdir -p gpurun_out
+mkdir -p bench_out
 SPARKFLOW_NO_PDL=1 timeout ${SANITIZE_TIMEOUT:-600} compute-sanitizer --tool "$TOOL" --error-exitcode 9 --print-limit 20 \
-  --log-file gpurun_out/sanitize_$TOOL.log python -m pytest tests/test_gpu_kernels.py -m gpu -x -q -k "$EXPR" -p no:cacheprovider
+  --log-file bench_out/sanitize_$TOOL.log python -m pytest tests/test_gpu_kernels.py -m gpu -x -q -k "$EXPR" -p no:cacheprovider
 RC=$?
 echo "compute-sanitizer $TOOL exit code: $RC"
-tail -5 gpurun_out/sanitize_$TOOL.log
+tail -5 bench_out/sanitize_$TOOL.log
 exit $RC

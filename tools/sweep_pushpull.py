@@ -133,8 +133,8 @@ def main():
             out.append(merged)
             print(json.dumps(merged), flush=True)
     if ctx.is_master:
-        os.makedirs("gpurun_out", exist_ok=True)
-        json.dump(out, open("gpurun_out/sweep_pushpull.json", "w"), indent=1)
+        os.makedirs("bench_out", exist_ok=True)
+        json.dump(out, open("bench_out/sweep_pushpull.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

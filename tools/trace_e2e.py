@@ -79,5 +79,5 @@ import os
 out["slots"] = eng.SLOTS
 out["block"] = os.environ.get("SPARKFLOW_DRIVER_BLOCK", "0")
 print(json.dumps(out))
-json.dump(out, open("gpurun_out/trace_e2e%s.json" % ("_lock" if lock else ""), "w"))
+json.dump(out, open("bench_out/trace_e2e%s.json" % ("_lock" if lock else ""), "w"))
 sess.close()

@@ -64,5 +64,5 @@ print("--- gemm phases (block 0 of each gemm): 101 = MMA thread [role start, fir
 for r in rows:
     if r["kid"] >= 100 and r["block"] == 0:
         print(r)
-json.dump(dict(summary=summ, rows=rows), open("gpurun_out/trace_step_%s%s.json" % (model, "_lock" if lock else ""), "w"))
+json.dump(dict(summary=summ, rows=rows), open("bench_out/trace_step_%s%s.json" % (model, "_lock" if lock else ""), "w"))
 sess.close()
