@@ -388,10 +388,11 @@ sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   float* s_bias = reinterpret_cast<float*>(smem + S::kStages * S::kStageBytes + S::kBarBytes);
 
   TraceScope trace;
-  // A GEMM that carries the fused read-your-writes wait may spin for a while: do NOT let its successors pre-launch behind
-  // it (they would sit resident on SMs - one CTA per SM at this shared-memory size - that the shard applier whose
-  // acknowledgement this kernel waits for needs for its own CTAs).
-  if (ep.ryw == nullptr) pdl_launch_dependents();
+  // When a successor may launch (PDL trigger): a GEMM that carries the fused read-your-writes wait never triggers (its
+  // successors launch when it completes) - they must not sit on SMs that the shard applier whose acknowledgement it
+  // waits for needs for its own CTAs.  A grid of several waves triggers at entry: its successor's CTAs only get SMs as
+  // this grid drains.  A one-wave grid triggers after its main loop, see there.
+  if (ep.ryw == nullptr && !ep.one_wave) pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * BN;
@@ -472,6 +473,10 @@ sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     float acc[BN / 2];
     mma_mainloop<BN, MN, S::kStages, S::kStageBytes, S::kABytes>(acc, stage_base, full_bar, empty_bar, 0, num_kb, ct >> 7,
                                                                  (ct & 127) == 0, 0x200);
+    // One-wave grid: the successor launches once every CTA is past its main loop, so its launch and prologue overlap
+    // this epilogue.  A trigger at entry would let a chain of small GEMMs pre-launch in a cascade, and those waiting
+    // CTAs (one per SM at this register / shared-memory size, 149 for the push) hold SMs the GEMMs ahead of them need.
+    if (ep.ryw == nullptr && ep.one_wave) pdl_launch_dependents();
     // every stage has been consumed by both warpgroups: the ring holds the staged accumulator tile from here on
     float* stg = reinterpret_cast<float*>(stage_base);
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -591,6 +596,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   int lim = g->N;
   if (g->ep.out_bf16 && g->ep.ld_bf16 > lim) lim = g->ep.ld_bf16;
   g->ep.n_store_limit = lim;
+  g->ep.one_wave = static_cast<long long>((g->N + g->bn - 1) / g->bn) * ((g->M + sf::kBM - 1) / sf::kBM) * g->split_k <= sf_num_sms();
   return 0;
 }
 

@@ -570,7 +570,6 @@ __global__ void __launch_bounds__(256, 1)
 pull_kernel(const SfPullArgs a, uint32_t* local_sync) {
   __shared__ uint32_t s_epoch;
   TraceScope trace;
-  pdl_launch_dependents();
   pdl_wait();
   trace.mark();
   const int tid = threadIdx.x;
@@ -608,6 +607,9 @@ pull_kernel(const SfPullArgs a, uint32_t* local_sync) {
     }
     __syncthreads();
   }
+  // successors may pre-launch only once the waits above are over: while this kernel spins on the applier or on a writer's
+  // lock, their CTAs (one per SM at GEMM shared-memory sizes) would hold the SMs the kernel it waits for needs
+  pdl_launch_dependents();
   const uint32_t cur = dbuf ? s_cur : 0u;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t gid = static_cast<size_t>(blockIdx.x) * blockDim.x + tid;

@@ -567,11 +567,18 @@ class StepDriver {
       if (e.free_) cudaEventDestroy(e.free_);
     }
   }
-  int add_plan(py::object plan, uintptr_t x_stage, uintptr_t y_stage, uintptr_t loss_out, int batch) {
+  // `prep` (optional, captured): prepares the step's operands from what was just staged; replayed on the copy stream
+  // after the staging copies and before the step's ready event, so it overlaps the steps still in flight
+  int add_plan(py::object plan, uintptr_t x_stage, uintptr_t y_stage, uintptr_t loss_out, int batch, py::object prep) {
     Entry e;
     e.keep = plan;
     e.plan = plan.cast<Plan*>();
     if (!e.plan->captured()) throw std::runtime_error("StepDriver: plan must be captured first");
+    if (!prep.is_none()) {
+      e.keep_prep = prep;
+      e.prep = prep.cast<Plan*>();
+      if (!e.prep->captured()) throw std::runtime_error("StepDriver: prep plan must be captured first");
+    }
     e.x_stage = P<char>(x_stage);
     e.y_stage = P<char>(y_stage);
     e.loss_out = P<float>(loss_out);
@@ -612,6 +619,7 @@ class StepDriver {
       if (e.y_stage && y_host_ && !no_h2d_)
         ck(cudaMemcpyAsync(e.y_stage, y_host_ + static_cast<size_t>(sp[k]) * y_row_, static_cast<size_t>(e.batch) * y_row_,
                            cudaMemcpyHostToDevice, copy_), "cudaMemcpyAsync(y)");
+      if (e.prep) e.prep->replay(reinterpret_cast<uintptr_t>(copy_));
       const auto t2 = clk::now();
       ck(cudaEventRecord(e.ready, copy_), "cudaEventRecord(ready)");
       ck(cudaStreamWaitEvent(compute_, e.ready, 0), "cudaStreamWaitEvent");
@@ -715,6 +723,7 @@ class StepDriver {
       // copy overlaps the steps still in flight and the step graph only waits on an event that has usually fired already
       ck(cudaMemcpyAsync(e.x_stage, perm + sp[k], static_cast<size_t>(e.batch) * sizeof(int32_t), cudaMemcpyDeviceToDevice, copy_),
          "cudaMemcpyAsync(minibatch row ids)");
+      if (e.prep) e.prep->replay(reinterpret_cast<uintptr_t>(copy_));
       ck(cudaEventRecord(e.ready, copy_), "cudaEventRecord(ready)");
       ck(cudaStreamWaitEvent(compute_, e.ready, 0), "cudaStreamWaitEvent");
       const auto t2 = clk::now();
@@ -797,8 +806,9 @@ class StepDriver {
   struct Entry {
     long long pending = -1;
     unsigned long long launched = 0;      // zero-copy mode: graph launches so far (the completion word counts them)
-    py::object keep;
+    py::object keep, keep_prep;
     Plan* plan = nullptr;
+    Plan* prep = nullptr;
     char* x_stage = nullptr;
     char* y_stage = nullptr;
     float* loss_out = nullptr;
@@ -1156,7 +1166,8 @@ PYBIND11_MODULE(_C, m) {
 
   py::class_<StepDriver>(m, "StepDriver")
       .def(py::init<uintptr_t, uintptr_t, uintptr_t, size_t, uintptr_t, size_t, uintptr_t, int>())
-      .def("add_plan", &StepDriver::add_plan)
+      .def("add_plan", &StepDriver::add_plan, py::arg("plan"), py::arg("x_stage"), py::arg("y_stage"), py::arg("loss_out"),
+           py::arg("batch"), py::arg("prep") = py::none())
       .def("run", &StepDriver::run)
       .def("steps", &StepDriver::steps)
       .def("flush", &StepDriver::flush)

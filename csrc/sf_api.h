@@ -60,6 +60,7 @@ struct SfGemmEpilogue {
   int aux_act;                    // SfAct whose derivative is taken at aux
   int accumulate;                 // atomicAdd into out_f32
   int n_store_limit;              // filled by sf_gemm_prepare
+  int one_wave;                   // filled by sf_gemm_prepare: the grid fits on the SMs at once (PDL trigger placement)
   int a_evict_first;
   // fused loss (last dense layer): the epilogue turns the activation into dL/dz in registers, so
   // out_bf16 / outT_bf16 / colsum receive dz, dz^T and the bias gradient directly.

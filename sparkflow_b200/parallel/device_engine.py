@@ -250,7 +250,8 @@ class StepBuffers:
     y_stage: Optional[torch.Tensor]
     loss_out: torch.Tensor
     result: Optional[torch.Tensor] = None
-    idx: Optional[torch.Tensor] = None     # resident mode: device int32 [B] row ids gathered by the step itself
+    idx: Optional[torch.Tensor] = None     # resident mode: device int32 [B] row ids gathered by the prep plan
+    prep: Any = None                       # staged plans: the plan that prepares the step's operands (run before the step)
 
 
 class DeviceWorker:
@@ -477,16 +478,19 @@ class DeviceWorker:
         self.stream.synchronize()
 
     def input_set(self, B: int, slot: int) -> Dict[str, Any]:
+        from .plan_builder import use_mn_possible
+
         key = (B, slot)
         if key not in self._input_sets:
             lp, D = self.plan, self.plan.input_dim
             ldB = round_up(B, 8)
             first = next(l for l in lp.layers if l.kind in ("dense", "conv"))
             dev = self.device
+            need_t = first.kind == "dense" and not use_mn_possible(self, lp.layers, True)     # K-major first wgrad
             self._input_sets[key] = dict(
                 x32=torch.zeros(B, D, dtype=torch.float32, device=dev),
                 a0=torch.zeros(B, round_up(D, 8), dtype=torch.bfloat16, device=dev),
-                a0T=torch.zeros(D, ldB, dtype=torch.bfloat16, device=dev) if first.kind == "dense" else None,
+                a0T=torch.zeros(D, ldB, dtype=torch.bfloat16, device=dev) if need_t else None,
                 y=None if lp.target_is_input or not lp.label_dim else torch.zeros(B, lp.label_dim, dtype=torch.float32, device=dev))
         return self._input_sets[key]
 
@@ -517,17 +521,26 @@ class DeviceWorker:
         self.copy_stream.wait_stream(cur)
 
     def build_plan(self, B: int, slot: int = 0, with_pull: bool = True, with_push: bool = True, fetch_slots: int = 0,
-                   resident: Optional[Tuple[torch.Tensor, Optional[torch.Tensor]]] = None):
+                   resident: Optional[Tuple[torch.Tensor, Optional[torch.Tensor]]] = None, staged: bool = False):
         """Compile the training step for batch size ``B`` reading from staging-buffer set ``slot``.  With
         ``fetch_slots`` = S > 0 the plan is a zero-copy one: it consumes input set ``slot`` and its graph fetches
-        the next minibatch into input set ``(slot + 1) % S``."""
+        the next minibatch into input set ``(slot + 1) % S``.
+
+        ``staged`` (implied by ``resident``): the step consumes input set ``slot`` and ``bufs.prep`` is the plan that
+        prepares it - cast of the rows copied into ``bufs.x_stage``, or, with ``resident`` = (X, Y) device tensors, the
+        gather of the rows whose ids are in ``bufs.idx``.  Running it before the step (on the stream that stages the
+        minibatch) takes the cast / gather off the step graph, which then starts with the pull.  Otherwise the step
+        casts ``bufs.x_stage`` itself."""
         from . import plan_builder
 
-        key = (B, slot, with_pull, with_push, fetch_slots, None if resident is None else resident[0].data_ptr())
-        if key not in self._plans and resident is not None:
-            built = plan_builder.build(self, B, train=True, with_pull=with_pull, with_push=with_push, resident=dict(x=resident[0], y=resident[1]))
+        staged = staged or resident is not None
+        key = (B, slot, with_pull, with_push, fetch_slots, staged, None if resident is None else resident[0].data_ptr())
+        if key not in self._plans and staged:
+            ins = self.input_set(B, slot)
+            built = plan_builder.build(self, B, train=True, with_pull=with_pull, with_push=with_push, inputs=ins)
+            prep, idx = plan_builder.build_prep(self, B, ins, None if resident is None else dict(x=resident[0], y=resident[1]))
             self._plans[key] = built.plan
-            self._bufs[key] = StepBuffers(built.x_stage, built.y_stage, built.loss_out, built.result, built.idx)
+            self._bufs[key] = StepBuffers(built.x_stage, built.y_stage, built.loss_out, built.result, idx, prep)
             self._keep.append(built.keep)
             self.launches_per_step = len(built.plan)
             self._last_names = list(built.plan.names())
@@ -640,6 +653,16 @@ class DeviceWorker:
         return plan_publish_needs(self.plan)
 
     # ------------------------------------------------------------------------------------------
+    def run_prep(self, bufs: StepBuffers, stream) -> None:
+        """Prepare a staged step's operands on ``stream`` (a CUDA graph once captured)."""
+        st = stream.cuda_stream
+        if not self.use_graphs:
+            bufs.prep.run(st)
+            return
+        if not bufs.prep.captured():
+            bufs.prep.capture(st)
+        bufs.prep.replay(st)
+
     def run_plan(self, plan) -> None:
         """Launch one step on the worker stream (CUDA graph after the first eager execution)."""
         st = self.stream.cuda_stream

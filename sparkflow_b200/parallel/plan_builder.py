@@ -12,8 +12,9 @@ Data-flow conventions (all activations bf16, all accumulation fp32):
 * conv is im2col (patches + patches^T) followed by the same GEMM; NHWC activations are exactly the
   row-major GEMM output, so no layout conversion exists anywhere.
 * backward: ``dgrad`` GEMMs run on the main branch of the graph, ``wgrad`` GEMMs (which only feed the push)
-  on a side branch; bias gradients come out of epilogues / the pool-backward kernel; every gradient lands in
-  the flat fp32 buffer the push kernel consumes.
+  alternate between two side branches, except the first layer's, which the push waits for: it runs on the main
+  branch; bias gradients come out of epilogues / the pool-backward kernel; every gradient lands in the flat fp32
+  buffer the push kernel consumes.
 """
 from __future__ import annotations
 
@@ -37,7 +38,6 @@ class BuiltPlan:
     loss_out: torch.Tensor
     result: Optional[torch.Tensor] = None
     keep: List[Any] = field(default_factory=list)
-    idx: Optional[torch.Tensor] = None       # resident mode: int32 [B] row ids of the minibatch this plan trains on
     debug: Optional[Dict[int, Dict[str, Any]]] = None     # per layer index: intermediate buffers (tests / tools)
 
 
@@ -141,17 +141,41 @@ def add_fetch_ops(plan, fetch: Dict[str, Any], B: int, D: int) -> None:
     plan.add_cast_transpose(P(t["x32"]), D, 0, P(t["a0"]), t["a0"].shape[1], P(t["a0T"]), 0 if t["a0T"] is None else t["a0T"].shape[1], B, D)
 
 
+def build_prep(worker, B: int, inputs: Dict[str, Any], resident: Optional[Dict[str, Any]] = None):
+    """Plan that prepares input set ``inputs`` (see ``build``) for one training step, run before the step's graph on the
+    stream that stages the minibatch.  DMA staging: cast (+ transpose) of the fp32 rows already copied into ``x32``.
+    ``resident``: dict(x, y) device tensors holding the whole partition in HBM: gather + cast of the rows whose ids are in
+    the returned ``idx`` buffer, and a row gather of the labels (or, for autoencoders, of the fp32 target rows).
+    Returns (plan, idx or None)."""
+    C, lp = worker.C, worker.plan
+    P = native.ptr
+    D = lp.input_dim
+    a0, a0T, x32, y = inputs["a0"], inputs["a0T"], inputs["x32"], inputs["y"]
+    ldT = a0T.shape[1] if a0T is not None else 0
+    plan = C.Plan()
+    if resident is None:
+        plan.add_cast_transpose(P(x32), D, 0, P(a0), a0.shape[1], P(a0T), ldT, B, D)
+        return plan, None
+    idx = torch.zeros(B, dtype=torch.int32, device=worker.device)
+    xr, yr = resident["x"], resident["y"]
+    plan.add_cast_transpose(P(xr), xr.shape[1], P(idx), P(a0), a0.shape[1], P(a0T), ldT, B, D)
+    if lp.target_is_input:
+        plan.add_gather_rows(P(xr), xr.shape[1], P(idx), P(x32), D, B, D)
+    if y is not None:
+        plan.add_gather_rows(P(yr), yr.shape[1], P(idx), P(y), y.shape[1], B, y.shape[1])
+    return plan, idx
+
+
 def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = True, upto: Optional[int] = None,
           post: Optional[str] = None, with_loss: bool = False, inputs: Optional[Dict[str, Any]] = None,
-          fetch: Optional[Dict[str, Any]] = None, resident: Optional[Dict[str, Any]] = None) -> BuiltPlan:
+          fetch: Optional[Dict[str, Any]] = None) -> BuiltPlan:
     """``train``: full step (fwd + loss + bwd + push).  Otherwise forward up to dense index ``upto``
     (None = last) producing an fp32 result (+ArgMax), or forward + loss only when ``with_loss``.
 
-    ``inputs`` (zero-copy mode): dict(x32, a0, a0T, y) already holding this step's minibatch (fp32 staging, bf16
-    operands, labels) - no H2D staging and no cast kernel on the critical path; ``fetch``: dict(args, target) of the
-    fetch node that fills the NEXT slot's input set from the pinned host partition on a side branch of this graph.
-    ``resident``: dict(x, y) device tensors holding the whole partition in HBM - the step gathers its minibatch rows
-    (ids in the returned ``idx`` buffer) itself: gather fused into the cast kernel, label rows by a row-gather kernel."""
+    ``inputs``: dict(x32, a0, a0T, y) already holding this step's minibatch (fp32 rows, bf16 operands, labels) when the
+    graph starts - filled by ``build_prep``'s plan or by a fetch node - so the graph has no cast kernel and starts with
+    the pull; ``fetch``: dict(args, target) of the fetch node that fills the NEXT slot's input set from the pinned host
+    partition on a side branch of this graph."""
     C, dev, lay, lp = worker.C, worker.device, worker.layout, worker.plan
     check_grammar(lp)
     P = native.ptr
@@ -166,13 +190,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     ldB = round_up(B, 8)
     D = lp.input_dim
     need_labels = (train or with_loss) and not lp.target_is_input
-    idx_stage = None
     if inputs is not None:
         x_stage, y_stage = inputs["x32"], inputs["y"]
-    elif resident is not None:
-        idx_stage = zeros(B, dtype=torch.int32)
-        x_stage = zeros(B, D, dtype=f32) if lp.target_is_input else None      # fp32 target rows (autoencoders)
-        y_stage = zeros(B, lp.label_dim, dtype=f32) if need_labels else None
     else:
         x_stage = zeros(B, D, dtype=f32)
         y_stage = zeros(B, lp.label_dim, dtype=f32) if need_labels else None
@@ -233,7 +252,11 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         add_fetch_ops(plan, fetch, B, D)
         plan.branch(0)
     # ---------------- pull || input cast ----------------
-    if do_pull and branches:
+    # with `inputs` the operands are ready when the graph starts: the pull heads the main branch and the first GEMM
+    # follows it over a programmatic edge (a join would be a full-completion edge).  The sharded snapshot pull keeps the
+    # join: it waits for the shard appliers and lets its successors pre-launch before that wait.
+    overlap_pull = do_pull and branches and (inputs is None or sharded)
+    if overlap_pull:
         plan.fork(1)
         plan.branch(1)
         add_pull_op()
@@ -249,16 +272,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     else:
         a0 = zeros(B, round_up(D, 8))
         a0T = zeros(D, ldB) if (train and first_is_dense and not use_mn) else None
-        if resident is not None:
-            xr, yr = resident["x"], resident["y"]
-            plan.add_cast_transpose(P(xr), xr.shape[1], P(idx_stage), P(a0), a0.shape[1], P(a0T), ldB if a0T is not None else 0, B, D)
-            if x_stage is not None:
-                plan.add_gather_rows(P(xr), xr.shape[1], P(idx_stage), P(x_stage), D, B, D)
-            if y_stage is not None:
-                plan.add_gather_rows(P(yr), yr.shape[1], P(idx_stage), P(y_stage), y_stage.shape[1], B, y_stage.shape[1])
-        else:
-            plan.add_cast_transpose(P(x_stage), D, 0, P(a0), a0.shape[1], P(a0T), ldB if a0T is not None else 0, B, D)
-    if do_pull and branches:
+        plan.add_cast_transpose(P(x_stage), D, 0, P(a0), a0.shape[1], P(a0T), ldB if a0T is not None else 0, B, D)
+    if overlap_pull:
         plan.join(1)
 
     # ---------------- forward ----------------
@@ -272,7 +287,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     produced: Dict[int, int] = {}             # output buffer address -> index of the GEMM that writes it
 
     def emit(g, name: str, d: Dict[str, Any], on_side: bool = False) -> None:
-        """Add a GEMM to the plan: its own launch (optionally on the wgrad branch), or a ticket range of the megakernel."""
+        """Add a GEMM to the plan: its own launch (optionally on a wgrad branch), or a ticket range of the megakernel."""
         gemms.append(g)
         if use_mega:
             deps = sorted({produced[p] for p in (d.get("a"), d.get("b"), d.get("aux")) if p in produced})
@@ -284,6 +299,12 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             side(lambda: plan.add_gemm(g, name))
         else:
             plan.add_gemm(g, name)
+
+    def wgrad_on_side(i: int) -> bool:
+        """The first trainable layer's wgrad is the last GEMM of the step and the only one the push still waits for: it
+        runs on the main branch right after the dgrad that produces its operand, and the push follows it over a
+        programmatic edge.  Sharded steps keep it on a side branch, beside the post of the bias-gradient tail."""
+        return i != first_trainable or sharded
 
     out_f32 = None
     dz_last = dzT_last = None
@@ -412,11 +433,16 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                          dz_last.shape[1], P(dzT_last), ldt_last, db, B, n_out)
 
     # ---------------- backward ----------------
+    n_side = [0]
+
     def side(fn):
-        """run `fn` (which adds ops) on the wgrad branch"""
+        """run `fn` (which adds ops) on a wgrad branch: branches 2 and 1 alternate, so no wgrad queues behind the previous
+        one (branch 3 belongs to the fetch node)"""
         if branches:
-            plan.fork(2)
-            plan.branch(2)
+            b = 2 - n_side[0] % 2
+            n_side[0] += 1
+            plan.fork(b)
+            plan.branch(b)
         fn()
         plan.branch(0)
 
@@ -440,7 +466,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             else:
                 wd.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
             wg = C.Gemm(wd)
-            emit(wg, f"wgrad{i}", wd, on_side=True)
+            emit(wg, f"wgrad{i}", wd, on_side=wgrad_on_side(i))
             if i == first_trainable:
                 break
             prev = layers[i - 1]
@@ -504,7 +530,10 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 cw.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
             wg = C.Gemm(cw)
             gemms.append(wg)
-            side(lambda wg=wg, i=i: plan.add_gemm(wg, f"wgrad{i}"))
+            if wgrad_on_side(i):
+                side(lambda wg=wg, i=i: plan.add_gemm(wg, f"wgrad{i}"))
+            else:
+                plan.add_gemm(wg, f"wgrad{i}")
             if i == first_trainable:
                 break
             h, w, cin = r["in_shape"]
@@ -522,8 +551,9 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         plan.add_post_flags(worker._post_flags_args(loss_out, phase=1))
     if use_mega:
         _emit_mega(plan, C, mega_items, keep)
-    elif branches:
-        plan.join(2)
+    else:
+        for b in (2, 1)[:n_side[0]]:
+            plan.join(b)
     if fetch is not None:
         plan.join(3)
     if with_push:
@@ -535,4 +565,4 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         else:
             plan.add_push(dict(worker._push_args(loss_out), **extra), P(worker.sync_push), 0)
     keep.append(gemms)
-    return BuiltPlan(plan, x_stage, y_stage, loss_out, None, keep, idx_stage, rec)
+    return BuiltPlan(plan, x_stage, y_stage, loss_out, None, keep, rec)

@@ -258,6 +258,7 @@ class B200Engine(Engine):
                 host.copy_(torch.as_tensor(np.asarray(rows, dtype=np.int64)))
                 self.h2d_bytes += B * 8
                 bufs.idx.copy_(self.perm_d[host.to(w.device, non_blocking=True)], non_blocking=True)
+        w.run_prep(bufs, w.stream)
         w.run_plan(plan)
         self._slot_free[slot].record(w.stream)
         self._pending[slot] = (self.step_idx % self.LOSS_RING, bufs.loss_out)
@@ -277,7 +278,7 @@ class B200Engine(Engine):
         if self.resident:
             return self._train_resident(rows, pull, slot)
         B = (rows.stop - rows.start) if isinstance(rows, slice) else len(rows)
-        plan, bufs = w.build_plan(B, slot, with_pull=pull)
+        plan, bufs = w.build_plan(B, slot, with_pull=pull, staged=True)
         if self._primed[slot]:
             self._slot_free[slot].synchronize()            # host gather buffer + staging are reusable
             self._harvest(slot)
@@ -288,6 +289,7 @@ class B200Engine(Engine):
             if bufs.y_stage is not None and hy is not None:
                 bufs.y_stage.copy_(hy, non_blocking=True)
                 self.h2d_bytes += hy.numel() * 4
+            w.run_prep(bufs, w.copy_stream)
             self._slot_ready[slot].record(w.copy_stream)
         w.stream.wait_event(self._slot_ready[slot])
         w.run_plan(plan)
@@ -365,7 +367,7 @@ class B200Engine(Engine):
                                               0 if self.Y is None else self.Y.shape[1] * 4, self.loss_ring.data_ptr(), self.LOSS_RING)
             drv_ids = []
             for slot in range(self.SLOTS):
-                plan, bufs = w.build_plan(batch, slot, with_pull=pull)
+                plan, bufs = w.build_plan(batch, slot, with_pull=pull, staged=True)
                 if not plan.captured():
                     # the first use of a plan runs it eagerly (a REAL step on the next scheduled minibatch) and
                     # captures the graph; step counts therefore stay exactly iters x batches
@@ -375,7 +377,7 @@ class B200Engine(Engine):
                     self.train(slice(starts[0], starts[0] + batch), pull, slot=slot)
                     starts = starts[1:]
                 drv_ids.append(self._driver.add_plan(plan, bufs.x_stage.data_ptr(), 0 if bufs.y_stage is None else bufs.y_stage.data_ptr(),
-                                                     bufs.loss_out.data_ptr(), batch))
+                                                     bufs.loss_out.data_ptr(), batch, self._captured_prep(bufs)))
             self._driver_plans[key] = drv_ids
         if not starts:
             return
@@ -390,6 +392,12 @@ class B200Engine(Engine):
         self._driver_last = (self._driver.steps() - 1) % self.LOSS_RING
         self.step_idx += n
 
+    def _captured_prep(self, bufs):
+        """The StepDriver replays a staged step's prep plan on the copy stream, after the minibatch copy."""
+        if not bufs.prep.captured():
+            bufs.prep.capture(self.w.copy_stream.cuda_stream)
+        return bufs.prep
+
     def _train_contiguous_resident(self, starts: List[int], batch: int, pull: bool) -> None:
         w = self.w
         key = (batch, pull, self.Xd.data_ptr())
@@ -400,7 +408,7 @@ class B200Engine(Engine):
                 plan, bufs = w.build_plan(batch, slot, with_pull=pull, resident=(self.Xd, self.Yd))
                 if not plan.captured():
                     plan.capture(w.stream.cuda_stream)
-                d.add_plan(plan, bufs.idx.data_ptr(), 0, bufs.loss_out.data_ptr(), batch)
+                d.add_plan(plan, bufs.idx.data_ptr(), 0, bufs.loss_out.data_ptr(), batch, self._captured_prep(bufs))
             drv = self._resident_driver[key] = d
         w.stream.synchronize()
         for slot in range(self.SLOTS):
