@@ -1,7 +1,6 @@
 // Unity translation unit for all device code (one copy of the sf::g_sf_error_code symbol).
 #include "gemm_sm90.cu"
 #include "gemm_pair_sm90.cu"
-#include "mega_sm90.cu"
 #include "elementwise.cu"
 #include "optim_push.cu"
 #include "conv.cu"
@@ -32,8 +31,8 @@ extern "C" int sf_preload_kernels() {
   SF_SMEM_ATTR(sf::sf_gemm_kernel<128>, sf::GemmSmem<128>::kBytes); SF_SMEM_ATTR(sf::sf_gemm_kernel<256>, sf::GemmSmem<256>::kBytes);
   SF_SMEM_ATTR((sf::sf_gemm_kernel<64, true>), sf::GemmSmem<64>::kBytes); SF_SMEM_ATTR((sf::sf_gemm_kernel<128, true>), sf::GemmSmem<128>::kBytes);
   SF_PRELOAD((sf::sf_gemm_kernel<64, true>)); SF_PRELOAD((sf::sf_gemm_kernel<128, true>));
-  SF_SMEM_ATTR(sf::sf_mega_kernel, sf::GemmSmem<32>::kBytes); SF_SMEM_ATTR(sf::sf_gemm_pair_kernel, sf::kPairSmemBytes);
-  SF_PRELOAD(sf::sf_gemm_kernel<32>); SF_PRELOAD(sf::sf_gemm_kernel<64>); SF_PRELOAD(sf::sf_gemm_kernel<128>); SF_PRELOAD(sf::sf_gemm_kernel<256>); SF_PRELOAD(sf::sf_mega_kernel); SF_PRELOAD(sf::sf_gemm_pair_kernel);
+  SF_SMEM_ATTR(sf::sf_gemm_pair_kernel, sf::kPairSmemBytes);
+  SF_PRELOAD(sf::sf_gemm_kernel<32>); SF_PRELOAD(sf::sf_gemm_kernel<64>); SF_PRELOAD(sf::sf_gemm_kernel<128>); SF_PRELOAD(sf::sf_gemm_kernel<256>); SF_PRELOAD(sf::sf_gemm_pair_kernel);
   SF_PRELOAD(sf::hostcopy_kernel); SF_PRELOAD(sf::gather_rows_f32_kernel); SF_PRELOAD(sf::fetch_kernel); SF_PRELOAD(sf::cast_transpose_kernel<false>); SF_PRELOAD(sf::cast_transpose_kernel<true>);
   SF_PRELOAD(sf::softmax_xent_kernel); SF_PRELOAD(sf::mse_kernel); SF_PRELOAD(sf::argmax_rows_kernel);
   SF_PRELOAD(sf::im2col_kernel); SF_PRELOAD(sf::col2im_kernel); SF_PRELOAD(sf::maxpool_fwd_kernel); SF_PRELOAD(sf::maxpool_bwd_kernel);

@@ -116,60 +116,6 @@ struct Gemm {
 };
 
 // ---------------------------------------------------------------------------
-// Mega: an ordered, dependency-annotated list of 128x32-tile GEMMs executed by ONE persistent launch
-// (csrc/mega_sm90.cu).  Built from prepared Gemm objects; owns the device copies of their descriptors.
-// ---------------------------------------------------------------------------
-struct Mega {
-  std::vector<std::shared_ptr<Gemm>> keep;
-  SfMegaArgs args{};
-  SfMegaGemm* d_gemms = nullptr;
-  unsigned int* d_ctr = nullptr;
-  int grid = 0;
-  Mega(std::vector<std::shared_ptr<Gemm>> gemms, const std::vector<std::vector<int>>& deps, int grid_) : keep(std::move(gemms)), grid(grid_) {
-    const int n = static_cast<int>(keep.size());
-    if (n < 1 || n > SF_MEGA_MAX_GEMMS) throw std::runtime_error("mega: between 1 and 16 GEMMs");
-    if (static_cast<int>(deps.size()) != n) throw std::runtime_error("mega: one dependency list per GEMM");
-    std::vector<SfMegaGemm> host(n);
-    int ticket = 0;
-    for (int i = 0; i < n; ++i) {
-      const SfGemm& g = keep[i]->g;
-      if (g.bn != 32 || g.split_k != 1 || g.pair != 0) throw std::runtime_error("mega: every GEMM must be a 128x32-tile, un-split, one-CTA GEMM");
-      std::memset(&host[i], 0, sizeof(SfMegaGemm));
-      host[i].tmA = g.tmA;
-      host[i].tmB = g.tmB;
-      host[i].ep = g.ep;
-      host[i].M = g.M; host[i].N = g.N; host[i].K = g.K;
-      host[i].tiles_m = (g.M + 127) / 128;
-      host[i].tiles_n = (g.N + 31) / 32;
-      host[i].tile_begin = ticket;
-      ticket += host[i].tiles_m * host[i].tiles_n;
-      if (deps[i].size() > SF_MEGA_MAX_DEPS) throw std::runtime_error("mega: too many dependencies");
-      host[i].n_deps = static_cast<int>(deps[i].size());
-      for (size_t d = 0; d < deps[i].size(); ++d) {
-        if (deps[i][d] < 0 || deps[i][d] >= i) throw std::runtime_error("mega: dependencies must point at earlier GEMMs (topological order)");
-        host[i].deps[d] = deps[i][d];
-      }
-    }
-    ck(cudaMalloc(reinterpret_cast<void**>(&d_gemms), sizeof(SfMegaGemm) * n), "cudaMalloc(mega gemms)");
-    ck(cudaMalloc(reinterpret_cast<void**>(&d_ctr), sizeof(unsigned int) * (2 + SF_MEGA_MAX_GEMMS)), "cudaMalloc(mega counters)");
-    ck(cudaMemcpy(d_gemms, host.data(), sizeof(SfMegaGemm) * n, cudaMemcpyHostToDevice), "cudaMemcpy(mega gemms)");
-    ck(cudaMemset(d_ctr, 0, sizeof(unsigned int) * (2 + SF_MEGA_MAX_GEMMS)), "cudaMemset(mega counters)");
-    args.gemms = d_gemms;
-    args.n_gemms = n;
-    args.total_tiles = ticket;
-    args.ctr = d_ctr;
-  }
-  ~Mega() {
-    if (d_gemms) cudaFree(d_gemms);
-    if (d_ctr) cudaFree(d_ctr);
-  }
-  Mega(const Mega&) = delete;
-  Mega& operator=(const Mega&) = delete;
-  void launch(uintptr_t stream) const { ck_rc(sf_mega_launch(&args, grid, S(stream)), "sf_mega_launch"); }
-  int total_tiles() const { return args.total_tiles; }
-};
-
-// ---------------------------------------------------------------------------
 // push / pull argument parsing
 // ---------------------------------------------------------------------------
 SfHyper parse_hyper(const py::dict& d) {
@@ -438,9 +384,6 @@ class Plan {
   }
   void add_gemm(std::shared_ptr<Gemm> g, const std::string& name) {
     add(name, [g](cudaStream_t st) { return sf_gemm_launch(&g->g, st); });
-  }
-  void add_mega(std::shared_ptr<Mega> m, const std::string& name) {
-    add(name, [m](cudaStream_t st) { return sf_mega_launch(&m->args, m->grid, st); });
   }
   size_t size() const {
     size_t n = 0;
@@ -1007,11 +950,6 @@ PYBIND11_MODULE(_C, m) {
   m.attr("PUSH_TILE_R") = 32;
   m.attr("PUSH_TILE_C") = 64;
 
-  py::class_<Mega, std::shared_ptr<Mega>>(m, "Mega")
-      .def(py::init<std::vector<std::shared_ptr<Gemm>>, const std::vector<std::vector<int>>&, int>(), py::arg("gemms"), py::arg("deps"),
-           py::arg("grid") = 0)
-      .def("launch", &Mega::launch)
-      .def_property_readonly("total_tiles", &Mega::total_tiles);
   py::class_<Gemm, std::shared_ptr<Gemm>>(m, "Gemm")
       .def(py::init<const py::dict&>())
       .def("launch", &Gemm::launch)
@@ -1035,7 +973,6 @@ PYBIND11_MODULE(_C, m) {
       .def("join", &Plan::join)
       .def("graph_nodes", &Plan::graph_nodes)
       .def("add_gemm", &Plan::add_gemm, py::arg("gemm"), py::arg("name") = "gemm")
-      .def("add_mega", &Plan::add_mega, py::arg("mega"), py::arg("name") = "mega")
       .def("add_cast_transpose",
            [](Plan& p, uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, uintptr_t outT,
               int ld_t, int rows, int cols) {

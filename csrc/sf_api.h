@@ -106,35 +106,10 @@ struct SfGemm {
   SfGemmEpilogue ep;
 };
 
-// ---------------------------------------------------------------------------
-// Whole-chain GEMM kernel ("megakernel", csrc/mega_sm90.cu): ONE persistent launch executes an ordered list of
-// 128 x 32-tile GEMMs (the forward / dgrad / wgrad chain of a dense network).  CTAs draw tile tickets from an atomic
-// counter; a tile of GEMM g starts once every tile of the GEMMs it depends on has been published (per-GEMM done
-// counters, release / acquire at gpu scope + a generic->async proxy fence before the TMA loads).
-// ---------------------------------------------------------------------------
-#define SF_MEGA_MAX_GEMMS 16
-#define SF_MEGA_MAX_DEPS 4
-struct alignas(64) SfMegaGemm {
-  CUtensorMap tmA, tmB;
-  SfGemmEpilogue ep;
-  int M, N, K;
-  int tiles_m, tiles_n;
-  int tile_begin;                 // first ticket of this GEMM
-  int n_deps;
-  int deps[SF_MEGA_MAX_DEPS];     // indices of the GEMMs whose outputs this one reads
-};
-struct SfMegaArgs {
-  const SfMegaGemm* gemms;        // device array
-  int n_gemms;
-  int total_tiles;
-  unsigned int* ctr;              // device: [0] ticket, [1] CTAs exited, [2 + g] tiles of GEMM g done
-};
-
 #ifdef __cplusplus
 extern "C" {
 #endif
 
-int sf_mega_launch(const SfMegaArgs* a, int grid, cudaStream_t st);
 int sf_gemm_prepare(SfGemm* g);
 int sf_gemm_launch(const SfGemm* g, cudaStream_t st);
 int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st);

@@ -142,16 +142,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32
 }
 
 // ---------------------------------------------------------------------------
-// Proxy fences
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_global() {
-  asm volatile("fence.proxy.async.global;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------
 // TMA
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {

@@ -291,7 +291,6 @@ class DeviceWorker:
         self.use_graphs = use_graphs and os.environ.get("SPARKFLOW_NO_GRAPHS") != "1"
         self.use_branches = os.environ.get("SPARKFLOW_NO_BRANCHES") != "1"
         self.fuse_loss = os.environ.get("SPARKFLOW_NO_FUSED_LOSS") != "1"
-        self.use_mega = os.environ.get("SPARKFLOW_MEGAKERNEL") == "1"       # opt-in: whole GEMM chain as one launch
         self.C.set_pdl(0 if os.environ.get("SPARKFLOW_NO_PDL") == "1" else 1)
         self.stream = torch.cuda.Stream(device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
@@ -486,7 +485,7 @@ class DeviceWorker:
             ldB = round_up(B, 8)
             first = next(l for l in lp.layers if l.kind in ("dense", "conv"))
             dev = self.device
-            need_t = first.kind == "dense" and not use_mn_possible(self, lp.layers, True)     # K-major first wgrad
+            need_t = first.kind == "dense" and not use_mn_possible(True)     # K-major first wgrad
             self._input_sets[key] = dict(
                 x32=torch.zeros(B, D, dtype=torch.float32, device=dev),
                 a0=torch.zeros(B, round_up(D, 8), dtype=torch.bfloat16, device=dev),

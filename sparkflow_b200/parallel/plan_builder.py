@@ -98,38 +98,10 @@ def _split_k(tiles: int, kblocks: int) -> int:
     return max(1, min(native.num_sms() // max(tiles, 1), kblocks // 4))
 
 
-def _emit_mega(plan, C, items: List[List[Any]], keep: List[Any]) -> None:
-    """Turn the recorded GEMM chain into ONE megakernel op (or, when a GEMM is not a plain 128x32-tile one, back into
-    individual launches).  Within a layer the dgrad goes before the wgrad in ticket order: it is on the critical path."""
-    order = list(range(len(items)))
-    k = 0
-    while k + 1 < len(order):
-        a, b = items[order[k]], items[order[k + 1]]
-        if a[1].startswith("wgrad") and b[1].startswith("dgrad") and order[k] not in b[2]:
-            order[k], order[k + 1] = order[k + 1], order[k]
-            k += 2
-        else:
-            k += 1
-    pos = {old: new for new, old in enumerate(order)}
-    gemms = [items[o][0] for o in order]
-    deps = [sorted(pos[d] for d in items[o][2]) for o in order]
-    ok = all(g.bn == 32 and g.split_k == 1 and g.pair == 0 for g in gemms) and len(gemms) <= 16 and all(len(d) <= 4 for d in deps)
-    if not ok:
-        for o in range(len(items)):
-            plan.add_gemm(items[o][0], items[o][1])
-        return
-    mega = C.Mega(gemms, deps, int(os.environ.get("SPARKFLOW_MEGA_CTAS", "0")))
-    keep.append(mega)
-    plan.add_mega(mega, "mega[" + ",".join(items[o][1] for o in order) + "]")
-
-
-def use_mn_possible(worker, layers, train: bool) -> bool:
-    """MN-major weight gradients (no transposed activation copies) are used unless switched off or the opt-in dense
-    megakernel (K-major tiles only) is active; forward-only plans never need transposes."""
-    if not train:
-        return True
-    return bool(os.environ.get("SPARKFLOW_WGRAD_MN", "1") == "1"
-                and not (getattr(worker, "use_mega", False) and all(l.kind == "dense" for l in layers)))
+def use_mn_possible(train: bool) -> bool:
+    """MN-major weight gradients (no transposed activation copies) are used unless switched off; forward-only plans never
+    need transposes."""
+    return not train or os.environ.get("SPARKFLOW_WGRAD_MN", "1") == "1"
 
 
 def add_fetch_ops(plan, fetch: Dict[str, Any], B: int, D: int) -> None:
@@ -218,7 +190,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         fuse_ryw = bool(train and getattr(worker, "fuse_ryw", False))
         if fuse_ryw:
             do_pull = False
-    fused_conv = fused_first_conv(lp) if use_mn_possible(worker, lp.layers, train) else None
+    fused_conv = fused_first_conv(lp) if use_mn_possible(train) else None
     if fused_conv is not None:
         fuse_ryw = False             # the first weight reader is the direct conv kernel: keep the stand-alone wait
         if sharded:
@@ -265,8 +237,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         add_pull_op()
     first_is_dense = layers[first_trainable].kind == "dense"
     # weight gradients read the row-major activation / dz buffers directly (MN-major wgmma operands): no transposed copy
-    # of any activation, gradient or im2col matrix is ever written.  (The opt-in megakernel only has K-major tiles.)
-    use_mn = bool(train and use_mn_possible(worker, layers, train))
+    # of any activation, gradient or im2col matrix is ever written.
+    use_mn = bool(train and use_mn_possible(train))
     if inputs is not None:
         a0, a0T = inputs["a0"], inputs["a0T"]
     else:
@@ -281,21 +253,11 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     cur: Dict[str, Any] = dict(kind="flat", buf=a0, bufT=a0T, feat=D, ld=a0.shape[1])
     rec: Dict[int, Dict[str, Any]] = {}        # per-layer tensors needed by backward
     gemms: List[Any] = []
-    # opt-in (SPARKFLOW_MEGAKERNEL=1): dense-only training steps run their whole GEMM chain as ONE persistent launch
-    use_mega = bool(train and getattr(worker, "use_mega", False) and not sharded and all(l.kind == "dense" for l in layers))
-    mega_items: List[List[Any]] = []          # [gemm, name, deps (indices into mega_items)]
-    produced: Dict[int, int] = {}             # output buffer address -> index of the GEMM that writes it
 
-    def emit(g, name: str, d: Dict[str, Any], on_side: bool = False) -> None:
-        """Add a GEMM to the plan: its own launch (optionally on a wgrad branch), or a ticket range of the megakernel."""
+    def emit(g, name: str, on_side: bool = False) -> None:
+        """Add a GEMM to the plan as its own launch, optionally on a wgrad branch."""
         gemms.append(g)
-        if use_mega:
-            deps = sorted({produced[p] for p in (d.get("a"), d.get("b"), d.get("aux")) if p in produced})
-            mega_items.append([g, name, deps])
-            for k in ("out_bf16", "outT_bf16"):
-                if d.get(k):
-                    produced[d[k]] = len(mega_items) - 1
-        elif on_side:
+        if on_side:
             side(lambda: plan.add_gemm(g, name))
         else:
             plan.add_gemm(g, name)
@@ -392,14 +354,14 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 out_f32 = zeros(B, ks.cols, dtype=f32)
                 d.update(out_f32=P(out_f32), ld_f32=ks.cols)
             g = C.Gemm(d)
-            emit(g, f"fwd{i}" + ("+loss" if fuse_loss else ""), d)
+            emit(g, f"fwd{i}" + ("+loss" if fuse_loss else ""))
             rec[i]["N"] = ks.cols
             break
         nxt = zeros(B, round_up(ks.cols, 8))
         nxtT = zeros(ks.cols, ldB) if (train and not use_mn) else None
         d.update(out_bf16=P(nxt), ld_bf16=nxt.shape[1], outT_bf16=P(nxtT), ld_t=ldB if nxtT is not None else 0)
         g = C.Gemm(d)
-        emit(g, f"fwd{i}", d)
+        emit(g, f"fwd{i}")
         cur = dict(kind="flat", buf=nxt, bufT=nxtT, feat=ks.cols, ld=nxt.shape[1])
 
     result = None
@@ -466,7 +428,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             else:
                 wd.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
             wg = C.Gemm(wd)
-            emit(wg, f"wgrad{i}", wd, on_side=wgrad_on_side(i))
+            emit(wg, f"wgrad{i}", on_side=wgrad_on_side(i))
             if i == first_trainable:
                 break
             prev = layers[i - 1]
@@ -478,7 +440,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                           ld_bf16=ndz.shape[1], outT_bf16=P(ndzT), ld_t=ldB if ndzT is not None else 0,
                           colsum=P(worker.grads) + pb.offset * 4 if pb else 0)
                 dg = C.Gemm(dd)
-                emit(dg, f"dgrad{i}", dd)
+                emit(dg, f"dgrad{i}")
                 g_dz, g_dzT = ndz, ndzT
             else:                                  # flatten over a pooled image: gradient wrt the pooled tensor
                 g_img = zeros(B, ks.rows)
@@ -549,11 +511,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         # forward the 1-D tail (bias gradients, all complete by now on the main branch) beside the last wgrad, so the post
         # after the join is a bare flag store: no store of its own to order, no system fence on the critical path
         plan.add_post_flags(worker._post_flags_args(loss_out, phase=1))
-    if use_mega:
-        _emit_mega(plan, C, mega_items, keep)
-    else:
-        for b in (2, 1)[:n_side[0]]:
-            plan.join(b)
+    for b in (2, 1)[:n_side[0]]:
+        plan.join(b)
     if fetch is not None:
         plan.join(3)
     if with_push:

@@ -267,34 +267,6 @@ def test_train_contiguous_native_loop_tracks_oracle(mode, served, monkeypatch):
     master.close()
 
 
-@pytest.mark.parametrize("name", ["simple_dnn", "autoencoder", "test_mlp"])
-def test_megakernel_chain_matches_per_gemm_launches(name, monkeypatch):
-    """SPARKFLOW_MEGAKERNEL=1: the forward / dgrad / wgrad GEMMs of a dense step run as ONE persistent launch with in-kernel
-    dependency counters; weights after a few steps must match the one-launch-per-GEMM plan."""
-    spec = OptimizerSpec.from_tf_kwargs("adam", dict(learning_rate=0.001))
-    results = []
-    for mega in ("0", "1"):
-        monkeypatch.setenv("SPARKFLOW_MEGAKERNEL", mega)
-        ir, master, worker, w0, (tf_in, tf_lab, d, c, kind) = _setup(name, spec, True)
-        assert worker.use_mega == (mega == "1")
-        X, Y = _data(256, d, c, kind)
-        eng = B200Engine(worker)
-        eng.load_partition(X, Y)
-        for r in [slice(0, 64), slice(64, 128), slice(128, 192), slice(192, 256)] * 2:
-            eng.train(r, pull=True)
-        eng.finish()
-        plan, _ = worker.build_plan(64, 0)
-        names = plan.names()
-        assert any(n.startswith("mega[") for n in names) == (mega == "1"), names
-        results.append((master.weights(), eng.last_loss(), master.counters()))
-        master.close()
-    (w_a, l_a, c_a), (w_b, l_b, c_b) = results
-    assert c_a["pushes"] == c_b["pushes"] == 8
-    assert abs(l_a - l_b) < 1e-3 * max(1.0, abs(l_a))
-    for a, b, v in zip(w_a, w_b, ir.trainable):
-        np.testing.assert_allclose(a, b, rtol=2e-3, atol=2e-5, err_msg=v.name)
-
-
 def test_fused_dropout_mask_statistics_and_gradients():
     """K13: tf.nn.dropout after a dense layer runs inside the compiled plan (Philox mask in the GEMM epilogue).  The mask
     is recovered from the stored activation; forward statistics and every gradient are checked against PyTorch given
