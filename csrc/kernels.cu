@@ -37,6 +37,7 @@ extern "C" int sf_preload_kernels() {
   SF_PRELOAD(sf::softmax_xent_kernel); SF_PRELOAD(sf::mse_kernel); SF_PRELOAD(sf::argmax_rows_kernel);
   SF_PRELOAD(sf::im2col_kernel); SF_PRELOAD(sf::col2im_kernel); SF_PRELOAD(sf::maxpool_fwd_kernel); SF_PRELOAD(sf::maxpool_bwd_kernel);
   SF_PRELOAD(sf::im2col_vec8_kernel); SF_PRELOAD(sf::col2im_vec8_kernel);
+  SF_PRELOAD(sf::maxpool_gen_fwd_kernel); SF_PRELOAD(sf::maxpool_gen_bwd_kernel); SF_PRELOAD(sf::act_bwd_bias_kernel);
   SF_PRELOAD((sf::conv_first_fwd_kernel<5, 5, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<5, 5, 1>));
   SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 1>));
   SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 3>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 3>));

@@ -1015,18 +1015,27 @@ PYBIND11_MODULE(_C, m) {
              });
            })
       .def("add_im2col",
-           [](Plan& p, uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t) {
+           [](Plan& p, uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, int sh,
+              int sw, int pad_top, int pad_left, int out_h, int out_w) {
              p.add("im2col", [=](cudaStream_t st) {
-               return sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, P<__nv_bfloat16>(out), ld_out,
-                                     P<__nv_bfloat16>(outT), ld_t, st);
+               return sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                                     P<__nv_bfloat16>(out), ld_out, P<__nv_bfloat16>(outT), ld_t, st);
              });
-           })
+           },
+           py::arg("in"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("out"), py::arg("ld_out"),
+           py::arg("outT"), py::arg("ld_t"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0,
+           py::arg("out_h") = 0, py::arg("out_w") = 0)
       .def("add_col2im",
-           [](Plan& p, uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din) {
+           [](Plan& p, uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din, int sh, int sw, int pad_top,
+              int pad_left, int out_h, int out_w) {
              p.add("col2im", [=](cudaStream_t st) {
-               return sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, P<__nv_bfloat16>(din), st);
+               return sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                                     P<__nv_bfloat16>(din), st);
              });
-           })
+           },
+           py::arg("dcols"), py::arg("ld_cols"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"),
+           py::arg("din"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0, py::arg("out_h") = 0,
+           py::arg("out_w") = 0)
       .def("add_maxpool_fwd",
            [](Plan& p, uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintptr_t argmax, uintptr_t outT, int ld_t) {
              p.add("maxpool_fwd", [=](cudaStream_t st) {
@@ -1043,22 +1052,53 @@ PYBIND11_MODULE(_C, m) {
                                       ld_t, P<float>(dbias), st);
              });
            })
+      .def("add_maxpool_gen_fwd",
+           [](Plan& p, uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
+              int out_w, uintptr_t out, uintptr_t argmax) {
+             p.add("maxpool_gen_fwd", [=](cudaStream_t st) {
+               return sf_maxpool_fwd(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                                     P<__nv_bfloat16>(out), P<uint8_t>(argmax), st);
+             });
+           })
+      .def("add_maxpool_gen_bwd",
+           [](Plan& p, uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
+              int pad_left, int out_h, int out_w, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+             p.add("maxpool_gen_bwd", [=](cudaStream_t st) {
+               return sf_maxpool_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top,
+                                     pad_left, out_h, out_w, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz,
+                                     P<float>(dbias), st);
+             });
+           })
+      .def("add_act_bwd_bias",
+           [](Plan& p, uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+             p.add("act_bwd_bias", [=](cudaStream_t st) {
+               return sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act,
+                                      P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
+             });
+           })
       .def("add_conv_first_fwd",
            [](Plan& p, uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act,
-              uintptr_t pooled, uintptr_t argmax) {
+              uintptr_t pooled, uintptr_t argmax, int pad_top, int pad_left, int out_h, int out_w) {
              p.add("conv_first_fwd", [=](cudaStream_t st) {
                return sf_conv_first_fwd(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(wT), ld_w, P<const float>(bias),
-                                        act, P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), st);
+                                        act, P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), pad_top, pad_left, out_h, out_w, st);
              });
-           })
+           },
+           py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"), py::arg("wT"),
+           py::arg("ld_w"), py::arg("bias"), py::arg("act"), py::arg("pooled"), py::arg("argmax"), py::arg("pad_top") = 0,
+           py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0)
       .def("add_conv_first_wgrad",
            [](Plan& p, uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t g_pool, uintptr_t pooled, uintptr_t argmax,
-              int act, uintptr_t dW, uintptr_t db) {
+              int act, uintptr_t dW, uintptr_t db, int pad_top, int pad_left, int out_h, int out_w) {
              p.add("conv_first_wgrad", [=](cudaStream_t st) {
                return sf_conv_first_wgrad(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(g_pool),
-                                          P<const __nv_bfloat16>(pooled), P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), st);
+                                          P<const __nv_bfloat16>(pooled), P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), pad_top,
+                                          pad_left, out_h, out_w, st);
              });
-           })
+           },
+           py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"),
+           py::arg("g_pool"), py::arg("pooled"), py::arg("argmax"), py::arg("act"), py::arg("dW"), py::arg("db"), py::arg("pad_top") = 0,
+           py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0)
       .def("add_push",
            [](Plan& p, const py::dict& d, uintptr_t local_sync, int grid) {
              const SfPushArgs a = parse_push(d);
@@ -1160,12 +1200,29 @@ PYBIND11_MODULE(_C, m) {
   m.def("lock_op", [](uintptr_t ctrl, int op, uintptr_t stream) {
     ck_rc(sf_lock_test(P<uint32_t>(ctrl), op, S(stream)), "lock_op");
   });
-  m.def("im2col", [](uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, uintptr_t stream) {
-    ck_rc(sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, P<__nv_bfloat16>(out), ld_out, P<__nv_bfloat16>(outT), ld_t, S(stream)), "im2col");
-  });
-  m.def("col2im", [](uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din, uintptr_t stream) {
-    ck_rc(sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, P<__nv_bfloat16>(din), S(stream)), "col2im");
-  });
+  // conv geometry (stride, pad_top / pad_left, output size) trails the stream argument; the defaults are VALID stride 1
+  m.def(
+      "im2col",
+      [](uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, uintptr_t stream, int sh,
+         int sw, int pad_top, int pad_left, int out_h, int out_w) {
+        ck_rc(sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w, P<__nv_bfloat16>(out),
+                             ld_out, P<__nv_bfloat16>(outT), ld_t, S(stream)),
+              "im2col");
+      },
+      py::arg("in"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("out"), py::arg("ld_out"),
+      py::arg("outT"), py::arg("ld_t"), py::arg("stream"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0,
+      py::arg("out_h") = 0, py::arg("out_w") = 0);
+  m.def(
+      "col2im",
+      [](uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din, uintptr_t stream, int sh, int sw, int pad_top,
+         int pad_left, int out_h, int out_w) {
+        ck_rc(sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                             P<__nv_bfloat16>(din), S(stream)),
+              "col2im");
+      },
+      py::arg("dcols"), py::arg("ld_cols"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("din"),
+      py::arg("stream"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0, py::arg("out_h") = 0,
+      py::arg("out_w") = 0);
   m.def("maxpool_fwd", [](uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintptr_t argmax, uintptr_t outT, int ld_t, uintptr_t stream) {
     ck_rc(sf_maxpool2_fwd(P<const __nv_bfloat16>(in), n, h, w, c, P<__nv_bfloat16>(out), P<uint8_t>(argmax), P<__nv_bfloat16>(outT), ld_t, S(stream)), "maxpool_fwd");
   });
@@ -1174,16 +1231,47 @@ PYBIND11_MODULE(_C, m) {
     ck_rc(sf_maxpool2_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, P<const __nv_bfloat16>(act_out), act,
                           P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), S(stream)), "maxpool_bwd");
   });
-  m.def("conv_first_fwd", [](uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act,
-                             uintptr_t pooled, uintptr_t argmax, uintptr_t stream) {
-    ck_rc(sf_conv_first_fwd(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(wT), ld_w, P<const float>(bias), act,
-                            P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), S(stream)), "conv_first_fwd");
+  m.def("maxpool_gen_fwd", [](uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
+                              int out_w, uintptr_t out, uintptr_t argmax, uintptr_t stream) {
+    ck_rc(sf_maxpool_fwd(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w, P<__nv_bfloat16>(out),
+                         P<uint8_t>(argmax), S(stream)),
+          "maxpool_gen_fwd");
   });
-  m.def("conv_first_wgrad", [](uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t g_pool, uintptr_t pooled,
-                               uintptr_t argmax, int act, uintptr_t dW, uintptr_t db, uintptr_t stream) {
-    ck_rc(sf_conv_first_wgrad(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(g_pool), P<const __nv_bfloat16>(pooled),
-                              P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), S(stream)), "conv_first_wgrad");
+  m.def("maxpool_gen_bwd", [](uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
+                              int pad_left, int out_h, int out_w, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias,
+                              uintptr_t stream) {
+    ck_rc(sf_maxpool_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                         P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), S(stream)),
+          "maxpool_gen_bwd");
   });
+  m.def("act_bwd_bias", [](uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias,
+                           uintptr_t stream) {
+    ck_rc(sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz,
+                          P<float>(dbias), S(stream)),
+          "act_bwd_bias");
+  });
+  m.def(
+      "conv_first_fwd",
+      [](uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act, uintptr_t pooled,
+         uintptr_t argmax, uintptr_t stream, int pad_top, int pad_left, int out_h, int out_w) {
+        ck_rc(sf_conv_first_fwd(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(wT), ld_w, P<const float>(bias), act,
+                                P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), pad_top, pad_left, out_h, out_w, S(stream)),
+              "conv_first_fwd");
+      },
+      py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"), py::arg("wT"),
+      py::arg("ld_w"), py::arg("bias"), py::arg("act"), py::arg("pooled"), py::arg("argmax"), py::arg("stream"), py::arg("pad_top") = 0,
+      py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0);
+  m.def(
+      "conv_first_wgrad",
+      [](uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t g_pool, uintptr_t pooled, uintptr_t argmax, int act,
+         uintptr_t dW, uintptr_t db, uintptr_t stream, int pad_top, int pad_left, int out_h, int out_w) {
+        ck_rc(sf_conv_first_wgrad(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(g_pool), P<const __nv_bfloat16>(pooled),
+                                  P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), pad_top, pad_left, out_h, out_w, S(stream)),
+              "conv_first_wgrad");
+      },
+      py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"), py::arg("g_pool"),
+      py::arg("pooled"), py::arg("argmax"), py::arg("act"), py::arg("dW"), py::arg("db"), py::arg("stream"), py::arg("pad_top") = 0,
+      py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0);
   m.def("gemm_pick_bn", &sf_gemm_pick_bn);
   m.def("set_pdl", &sf_set_pdl);
   m.def("trace_enable", [](uintptr_t buf, unsigned int cap) { ck_rc(sf_trace_enable(P<void>(buf), cap), "trace_enable"); });

@@ -164,23 +164,38 @@ int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target
 int sf_argmax_rows(const float* in, int ld, float* out, int rows, int cols, cudaStream_t st);
 int sf_fill_zero(void* p, size_t bytes, cudaStream_t st);
 
-// conv building blocks (NHWC, VALID, stride 1) and 2x2/s2 max-pool (conv.cu)
-int sf_im2col_nhwc(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw,
-                   __nv_bfloat16* out, int ld_out, __nv_bfloat16* outT, int ld_t, cudaStream_t st);
-int sf_col2im_nhwc(const __nv_bfloat16* dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw,
-                   __nv_bfloat16* din, cudaStream_t st);
+// conv building blocks (NHWC; stride (sh, sw), pad_top / pad_left zero rows / columns in front of the image, output
+// out_h x out_w; out_h / out_w <= 0 = the VALID size) and max-pools (conv.cu)
+int sf_im2col_nhwc(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left,
+                   int out_h, int out_w, __nv_bfloat16* out, int ld_out, __nv_bfloat16* outT, int ld_t, cudaStream_t st);
+int sf_col2im_nhwc(const __nv_bfloat16* dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, int sh, int sw,
+                   int pad_top, int pad_left, int out_h, int out_w, __nv_bfloat16* din, cudaStream_t st);
+// 2x2 / stride-2 / unpadded max-pool (the fast path)
 int sf_maxpool2_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, __nv_bfloat16* out,
                     uint8_t* argmax, __nv_bfloat16* outT, int ld_t, cudaStream_t st);
 int sf_maxpool2_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c,
                     const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz, int ld_dz,
                     __nv_bfloat16* dzT, int ld_t, float* dbias, cudaStream_t st);
+// general max-pool: kh x kw <= 4x4 window, any stride, VALID or SAME (argmax = dy * kw + dx of the winner); the backward
+// pass is fused with act'(a) of the pooled conv output and the bias gradient and writes row-major dz [M, ld_dz]
+int sf_maxpool_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left,
+                   int out_h, int out_w, __nv_bfloat16* out, uint8_t* argmax, cudaStream_t st);
+int sf_maxpool_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw,
+                   int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz,
+                   int ld_dz, float* dbias, cudaStream_t st);
+// activation gradient of a conv with no pool after it: dz = g * act'(a) [rows, ld_dz], dbias += column sums
+int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz,
+                    int ld_dz, float* dbias, cudaStream_t st);
 
 // first convolution of a network (K = kh * kw * cin <= 64, cout in {8, 16, 32, 64}) fused with bias, activation and the
-// 2x2 max-pool that follows it: direct CUDA-core kernels, one CTA per image, nothing but the pooled tensor is written
+// 2x2 max-pool that follows it: direct CUDA-core kernels, one CTA per image, nothing but the pooled tensor is written.
+// Stride 1; out_h / out_w <= 0 = VALID, otherwise the conv output size with pad_top / pad_left zero rows / columns in front
 int sf_conv_first_fwd(const __nv_bfloat16* x, int n, int h, int w, int cin, int kh, int kw, int cout, const __nv_bfloat16* wT,
-                      int ld_w, const float* bias, int act, __nv_bfloat16* pooled, uint8_t* argmax, cudaStream_t st);
+                      int ld_w, const float* bias, int act, __nv_bfloat16* pooled, uint8_t* argmax, int pad_top, int pad_left,
+                      int out_h, int out_w, cudaStream_t st);
 int sf_conv_first_wgrad(const __nv_bfloat16* x, int n, int h, int w, int cin, int kh, int kw, int cout, const __nv_bfloat16* g_pool,
-                        const __nv_bfloat16* pooled, const uint8_t* argmax, int act, float* dW, float* db, cudaStream_t st);
+                        const __nv_bfloat16* pooled, const uint8_t* argmax, int act, float* dW, float* db, int pad_top, int pad_left,
+                        int out_h, int out_w, cudaStream_t st);
 
 // ---------------------------------------------------------------------------
 // Fused push: optimizer step on the (possibly remote) master shard + bf16 publish (optim_push.cu)

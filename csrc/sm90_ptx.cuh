@@ -44,7 +44,8 @@ __device__ unsigned int g_trace_cap = 0;
 __device__ unsigned int g_trace_n = 0;
 
 enum KernelId { KID_GEMM = 1, KID_CAST = 2, KID_SOFTMAX = 3, KID_MSE = 4, KID_ARGMAX = 5, KID_PUSH = 6, KID_PULL = 7,
-                KID_IM2COL = 8, KID_COL2IM = 9, KID_POOL_FWD = 10, KID_POOL_BWD = 11 };
+                KID_IM2COL = 8, KID_COL2IM = 9, KID_POOL_FWD = 10, KID_POOL_BWD = 11, KID_POOL_GEN_FWD = 12, KID_POOL_GEN_BWD = 13,
+                KID_ACT_BWD = 14 };
 
 __device__ __forceinline__ unsigned long long trace_now() {
   unsigned long long t;

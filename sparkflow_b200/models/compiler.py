@@ -9,7 +9,11 @@ Softmax).  Graphs outside this family (custom losses, exotic ops) are reported a
 generic interpreter engine instead (loudly: a RuntimeWarning names the reason).
 
 Covers every model the reference ships (SURVEY.md section 2.3): simple_dnn, cnn_example,
-autoencoder_example, the test MLPs / auto-encoder and the checkpoint fixture.
+autoencoder_example, the test MLPs / auto-encoder and the checkpoint fixture, and the usual TF-1.x CNN geometry beyond
+them: NHWC ``Conv2D`` with VALID or SAME padding and any stride, ``MaxPool`` with a window of up to 4x4, any stride and
+VALID or SAME padding (e.g. the "Deep MNIST" network).  Output sizes and pads follow TensorFlow: VALID
+``out = (in - k) // s + 1``; SAME ``out = ceil(in / s)`` with ``pad_total = max((out - 1) * s + k - in, 0)`` split as
+``top = pad_total // 2`` and the extra row / column at the bottom / right.
 """
 from __future__ import annotations
 
@@ -33,7 +37,10 @@ class Layer:
     act: Optional[str] = None                   # Relu | Sigmoid | Tanh | None
     in_shape: Tuple[int, ...] = ()              # per-sample shape (no batch dim)
     out_shape: Tuple[int, ...] = ()
-    ksize: Tuple[int, int] = (0, 0)
+    ksize: Tuple[int, int] = (0, 0)            # conv: filter taps; pool: window
+    strides: Tuple[int, int] = (1, 1)           # conv / pool: (sh, sw)
+    pads: Tuple[int, int, int, int] = (0, 0, 0, 0)   # conv / pool: (top, bottom, left, right), from the padding mode
+    padding: str = "VALID"                      # conv / pool: TF padding mode (VALID | SAME)
     tensors: Dict[str, str] = field(default_factory=dict)   # stage -> tensor name (linear / bias / act / dropout)
     dropout_keep: float = 0.0                   # dense: keep probability of a tf.nn.dropout applied to the layer's output (0 = none)
 
@@ -79,6 +86,21 @@ class LayerPlan:
 
 
 _PASS = ("Identity", "StopGradient", "PlaceholderWithDefault")
+MAX_POOL_WINDOW = 4
+
+
+def _padding(node: Node) -> str:
+    p = node.attrs.get("padding", "VALID")
+    return p.decode() if isinstance(p, bytes) else str(p)
+
+
+def conv_geometry(size: int, k: int, s: int, padding: str) -> Tuple[int, int, int]:
+    """TensorFlow's output size and (before, after) padding of one spatial dimension."""
+    if padding == "SAME":
+        out = -(-size // s)
+        total = max((out - 1) * s + k - size, 0)
+        return out, total // 2, total - total // 2
+    return (size - k) // s + 1, 0, 0
 
 
 def _var_of(ir: GraphIR, ref: Tuple[str, int]) -> Optional[str]:
@@ -296,9 +318,11 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
         if pending_drop:
             raise UnsupportedGraph(f"dropout on top of '{node.op}' ({node.name}): the compiled plan fuses dropout into dense layers only")
         if node.op == "Conv2D":
-            if node.attrs.get("padding", "VALID") != "VALID" or list(node.attrs.get("strides", [1, 1, 1, 1])) != [1, 1, 1, 1] \
+            strides = [int(v) for v in node.attrs.get("strides", [1, 1, 1, 1])]
+            if _padding(node) not in ("VALID", "SAME") or len(strides) != 4 or strides[0] != 1 or strides[3] != 1 or min(strides) < 1 \
                     or node.attrs.get("data_format", "NHWC") != "NHWC" or list(node.attrs.get("dilations", [1, 1, 1, 1])) != [1, 1, 1, 1]:
-                raise UnsupportedGraph("only NHWC / VALID / stride-1 Conv2D is covered by the compiled plan")
+                raise UnsupportedGraph("only NHWC / undilated Conv2D with VALID or SAME padding and strides [1, sh, sw, 1] is covered "
+                                       "by the compiled plan")
             kvar = _var_of(ir, node.inputs[1])
             if kvar is None:
                 raise UnsupportedGraph(f"Conv2D '{node.name}' filter is not a variable")
@@ -310,17 +334,21 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
                 tensors["act"] = pending_act[1]
             layers_rev.append(Layer("conv", kernel=kvar, bias=pending_bias[0] if pending_bias else None,
                                     act=pending_act[0] if pending_act else None, in_shape=(-1, -1, cin), out_shape=(-1, -1, cout),
-                                    ksize=(kh, kw), tensors=tensors))
+                                    ksize=(kh, kw), strides=(strides[1], strides[2]), padding=_padding(node), tensors=tensors))
             pending_act = pending_bias = None
             cur = node.inputs[0]
             continue
         if pending_act or pending_bias:
             raise UnsupportedGraph(f"bias/activation stacked on unsupported op '{node.op}' ({node.name})")
         if node.op == "MaxPool":
-            if list(node.attrs.get("ksize")) != [1, 2, 2, 1] or list(node.attrs.get("strides")) != [1, 2, 2, 1] \
-                    or node.attrs.get("padding", "VALID") != "VALID":
-                raise UnsupportedGraph("only 2x2 / stride-2 / VALID MaxPool is covered by the compiled plan")
-            layers_rev.append(Layer("pool", ksize=(2, 2), tensors={"act": tname}))
+            ks = [int(v) for v in node.attrs.get("ksize", [])]
+            st = [int(v) for v in node.attrs.get("strides", [])]
+            if len(ks) != 4 or len(st) != 4 or ks[0] != 1 or ks[3] != 1 or st[0] != 1 or st[3] != 1 or min(ks) < 1 or min(st) < 1 \
+                    or max(ks[1], ks[2]) > MAX_POOL_WINDOW or _padding(node) not in ("VALID", "SAME") \
+                    or node.attrs.get("data_format", "NHWC") != "NHWC":
+                raise UnsupportedGraph(f"only NHWC MaxPool with a window of at most {MAX_POOL_WINDOW}x{MAX_POOL_WINDOW}, strides "
+                                       "[1, sh, sw, 1] and VALID or SAME padding is covered by the compiled plan")
+            layers_rev.append(Layer("pool", ksize=(ks[1], ks[2]), strides=(st[1], st[2]), padding=_padding(node), tensors={"act": tname}))
             cur = node.inputs[0]
             continue
         if node.op == "Reshape":
@@ -356,15 +384,17 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
         elif l.kind == "dense":
             if len(shape) != 1 or shape[0] != l.in_shape[0]:
                 raise UnsupportedGraph(f"dense layer '{l.kernel}' expects {l.in_shape} features but receives {shape}")
-        elif l.kind == "conv":
-            if len(shape) != 3 or shape[2] != l.in_shape[2]:
-                raise UnsupportedGraph(f"conv layer '{l.kernel}' expects NHWC input, got per-sample shape {shape}")
-            l.in_shape = shape
-            l.out_shape = (shape[0] - l.ksize[0] + 1, shape[1] - l.ksize[1] + 1, l.out_shape[2])
-        elif l.kind == "pool":
+        elif l.kind in ("conv", "pool"):
             if len(shape) != 3:
-                raise UnsupportedGraph("MaxPool on non-image tensor")
-            l.in_shape, l.out_shape = shape, (shape[0] // 2, shape[1] // 2, shape[2])
+                raise UnsupportedGraph(f"{l.kind} layer on a non-image tensor (per-sample shape {shape})")
+            if l.kind == "conv" and shape[2] != l.in_shape[2]:
+                raise UnsupportedGraph(f"conv layer '{l.kernel}' expects NHWC input, got per-sample shape {shape}")
+            oh, pt, pb = conv_geometry(shape[0], l.ksize[0], l.strides[0], l.padding)
+            ow, pl, pr = conv_geometry(shape[1], l.ksize[1], l.strides[1], l.padding)
+            if oh < 1 or ow < 1:
+                raise UnsupportedGraph(f"{l.kind} layer: a {l.ksize[0]}x{l.ksize[1]} window does not fit its {shape[0]}x{shape[1]} input")
+            l.in_shape, l.pads = shape, (pt, pb, pl, pr)
+            l.out_shape = (oh, ow, l.out_shape[2] if l.kind == "conv" else shape[2])
         shape = l.out_shape
 
     if not any(l.kind in ("dense", "conv") for l in layers):

@@ -8,6 +8,9 @@ Each function mirrors a model definition of the reference:
   * :func:`test_mlp` / :func:`test_autoencoder` – tests/dl_runner.py:45-73
   * :func:`fixture_mlp`       – the graph stored in tests/test_model/to_load.meta (2-10-10-1)
   * :func:`autoencoder_small` / :func:`wide_dnn` – BASELINE.json configs 4 and 5
+  * :func:`cnn_same`          – TensorFlow's "Deep MNIST" network (SAME-padded convs and pools)
+  * :func:`cnn_strided`       – strided / SAME convs, a conv feeding a conv, an overlapping 3x3/2 pool, a conv feeding
+    the flatten
 """
 from __future__ import annotations
 
@@ -33,6 +36,34 @@ def cnn():
     c1 = tf.layers.max_pooling2d(tf.layers.conv2d(img, 32, 5, activation=tf.nn.relu), 2, 2)
     c2 = tf.layers.max_pooling2d(tf.layers.conv2d(c1, 64, 3, activation=tf.nn.relu), 2, 2)
     logits = tf.layers.dense(tf.layers.flatten(c2), 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def cnn_same():
+    """conv 5x5x32 SAME relu -> pool 2x2/2 SAME -> conv 5x5x64 SAME relu -> pool 2x2/2 SAME -> dense 1024 relu -> dense 10"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    c1 = tf.layers.max_pooling2d(tf.layers.conv2d(img, 32, 5, padding="same", activation=tf.nn.relu), 2, 2, padding="same")
+    c2 = tf.layers.max_pooling2d(tf.layers.conv2d(c1, 64, 5, padding="same", activation=tf.nn.relu), 2, 2, padding="same")
+    h = tf.layers.dense(tf.layers.flatten(c2), 1024, activation=tf.nn.relu)
+    logits = tf.layers.dense(h, 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def cnn_strided():
+    """28x28x1 -> conv 3x3x16 SAME relu -> conv 3x3x32 SAME stride 2 tanh -> pool 3x3/2 SAME -> conv 3x3x32 VALID stride 2 relu
+    -> flatten 288 -> dense 10"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    c1 = tf.layers.conv2d(img, 16, 3, padding="same", activation=tf.nn.relu)
+    c2 = tf.layers.conv2d(c1, 32, 3, strides=2, padding="same", activation=tf.nn.tanh)
+    p2 = tf.layers.max_pooling2d(c2, 3, 2, padding="same")
+    c3 = tf.layers.conv2d(p2, 32, 3, strides=2, padding="valid", activation=tf.nn.relu)
+    logits = tf.layers.dense(tf.layers.flatten(c3), 10)
     tf.argmax(logits, 1, name="out")
     return tf.losses.softmax_cross_entropy(y, logits)
 
@@ -94,6 +125,8 @@ def fixture_mlp():
 MODELS: Dict[str, Callable] = {
     "simple_dnn": simple_dnn,
     "cnn": cnn,
+    "cnn_same": cnn_same,
+    "cnn_strided": cnn_strided,
     "autoencoder": autoencoder,
     "autoencoder_small": autoencoder_small,
     "wide_dnn": wide_dnn,

@@ -2,19 +2,24 @@
 
 Supported layer grammar (anything else is reported as UnsupportedGraph and handled by the generic engine):
 
-    input -> [reshape] -> (conv pool)* -> [flatten] -> dense+ -> loss
+    input -> [reshape] -> (conv [maxpool])* -> [flatten] -> dense+ -> loss
+
+conv: NHWC, VALID or SAME padding, stride (sh, sw); maxpool: window up to 4x4, stride (sh, sw), VALID or SAME (TF geometry,
+see models/compiler.py).  A conv without a pool after it feeds the next conv or the flatten directly.
 
 Data-flow conventions (all activations bf16, all accumulation fp32):
 
 * dense layer i consumes ``a_i`` [B, ld] (A operand) and the published ``W_i^T`` [out, ld] (B operand);
   its epilogue adds bias, applies the activation and writes ``a_{i+1}`` plus ``a_{i+1}^T`` (the K-major
   operand of the next layer's wgrad).  The last dense layer's epilogue also computes the loss and dL/dz.
-* conv is im2col (patches + patches^T) followed by the same GEMM; NHWC activations are exactly the
-  row-major GEMM output, so no layout conversion exists anywhere.
+* conv is im2col (patches + patches^T; out-of-image taps of a padded conv read zero) followed by the same GEMM; NHWC
+  activations are exactly the row-major GEMM output, so no layout conversion exists anywhere.
+* max-pool: 2x2 / stride 2 without padding runs on the dedicated kernels (SAME on even sizes included), every other
+  geometry on the general window kernels.
 * backward: ``dgrad`` GEMMs run on the main branch of the graph, ``wgrad`` GEMMs (which only feed the push)
   alternate between two side branches, except the first layer's, which the push waits for: it runs on the main
-  branch; bias gradients come out of epilogues / the pool-backward kernel; every gradient lands in the flat fp32
-  buffer the push kernel consumes.
+  branch; bias gradients come out of epilogues / the pool-backward kernel (or, for a conv with no pool after it, the
+  activation-gradient kernel); every gradient lands in the flat fp32 buffer the push kernel consumes.
 """
 from __future__ import annotations
 
@@ -41,6 +46,23 @@ class BuiltPlan:
     debug: Optional[Dict[int, Dict[str, Any]]] = None     # per layer index: intermediate buffers (tests / tools)
 
 
+def pool_fast_path(l: Layer) -> bool:
+    """A 2x2 / stride-2 max-pool with zero effective padding runs on the dedicated 2x2 kernels."""
+    return l.ksize == (2, 2) and l.strides == (2, 2) and not any(l.pads)
+
+
+def _kmajor_geometry_ok(layers: List[Layer]) -> bool:
+    """The K-major weight-gradient path (SPARKFLOW_WGRAD_MN=0) needs transposed copies that only the VALID stride-1 conv
+    followed by the 2x2 / stride-2 pool kernels write."""
+    for i, l in enumerate(layers):
+        if l.kind == "conv":
+            if l.strides != (1, 1) or any(l.pads) or i + 1 >= len(layers) or layers[i + 1].kind != "pool":
+                return False
+        elif l.kind == "pool" and not pool_fast_path(l):
+            return False
+    return True
+
+
 def check_grammar(lp: LayerPlan) -> None:
     """Raise UnsupportedGraph unless the layer sequence matches the grammar above."""
     kinds = [l.kind for l in lp.layers]
@@ -48,9 +70,11 @@ def check_grammar(lp: LayerPlan) -> None:
     if i < len(kinds) and kinds[i] == "reshape":
         i += 1
     saw_conv = False
-    while i + 1 < len(kinds) and kinds[i] == "conv" and kinds[i + 1] == "pool":
+    while i < len(kinds) and kinds[i] == "conv":
         saw_conv = True
-        i += 2
+        i += 1
+        if i < len(kinds) and kinds[i] == "pool":
+            i += 1
     if i < len(kinds) and kinds[i] == "reshape":
         i += 1
     n_dense = 0
@@ -59,7 +83,7 @@ def check_grammar(lp: LayerPlan) -> None:
         i += 1
     if i != len(kinds) or n_dense == 0:
         raise UnsupportedGraph(f"layer sequence {kinds} is outside the compiled plan grammar "
-                               "(input -> [reshape] -> (conv pool)* -> [flatten] -> dense+)")
+                               "(input -> [reshape] -> (conv [maxpool])* -> [flatten] -> dense+)")
     for l in lp.layers:
         if l.kind == "conv":
             if l.out_shape[2] % 8:
@@ -68,12 +92,16 @@ def check_grammar(lp: LayerPlan) -> None:
                 raise UnsupportedGraph(f"conv activation {l.act}")
     if saw_conv and lp.input_dim % 8:
         raise UnsupportedGraph("image inputs need a feature count that is a multiple of 8")
+    if saw_conv and not use_mn_possible(True) and not _kmajor_geometry_ok(lp.layers):
+        raise UnsupportedGraph("SPARKFLOW_WGRAD_MN=0 (K-major weight gradients) covers only VALID stride-1 convs each followed by a "
+                               "2x2 / stride-2 max-pool")
 
 
 def fused_first_conv(lp: LayerPlan) -> Optional[int]:
-    """Index of the network's first trainable layer when it is a small convolution directly followed by the 2x2 max-pool
-    (K = kh * kw * cin <= 64, 8..64 output channels): that pair runs as ONE direct CUDA-core kernel forward and ONE
-    backward (csrc/conv.cu: conv_first_fwd / conv_first_wgrad) instead of im2col + a K-padded GEMM + a pooling pass."""
+    """Index of the network's first trainable layer when it is a small stride-1 convolution directly followed by a 2x2 /
+    stride-2 max-pool without padding (K = kh * kw * cin <= 64, 8..64 output channels, the zero-padded image within 64 KiB
+    of fp32): that pair runs as ONE direct CUDA-core kernel forward and ONE backward (csrc/conv.cu: conv_first_fwd /
+    conv_first_wgrad) instead of im2col + a K-padded GEMM + a pooling pass."""
     if os.environ.get("SPARKFLOW_FUSED_CONV1", "1") == "0":
         return None
     layers = lp.layers
@@ -82,12 +110,14 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
         return None
     i = trainable[0]
     l = layers[i]
-    if l.kind != "conv" or i + 1 >= len(layers) or layers[i + 1].kind != "pool":
+    if l.kind != "conv" or i + 1 >= len(layers) or layers[i + 1].kind != "pool" or not pool_fast_path(layers[i + 1]):
+        return None
+    if l.strides != (1, 1):
         return None
     cin, cout = l.in_shape[2], l.out_shape[2]
     if l.ksize[0] * l.ksize[1] * cin > 64 or cout not in (8, 16, 32, 64) or l.act not in (None, "Relu", "Sigmoid", "Tanh"):
         return None
-    if l.in_shape[0] * l.in_shape[1] * cin * 4 > 64 * 1024:
+    if (l.out_shape[0] + l.ksize[0] - 1) * (l.out_shape[1] + l.ksize[1] - 1) * cin * 4 > 64 * 1024:
         return None
     return i
 
@@ -294,7 +324,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             pooled = zeros(B, ph * pw * cout)
             argmax = zeros(B, ph * pw * cout, dtype=torch.uint8)
             plan.add_conv_first_fwd(P(cur["buf"]), B, h, w, cin, kh, kw, cout, P(wsrc) + ks.wt_off * 2, ks.wt_ld,
-                                    worker._bias_ptr(bs) if bs else 0, ACT_IDS[l.act], P(pooled), P(argmax))
+                                    worker._bias_ptr(bs) if bs else 0, ACT_IDS[l.act], P(pooled), P(argmax), l.pads[0], l.pads[2], oh, ow)
             rec[i] = dict(fused=True, x=cur["buf"], in_shape=(h, w, cin), pooled=pooled, argmax=argmax)
             cur = dict(kind="img", buf=pooled, shape=(ph, pw, cout), flatT=None, fused_pool=i)
             continue
@@ -309,7 +339,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             ldK, ldM = round_up(K, 8), round_up(M, 8)
             patches = zeros(M, ldK)
             patchesT = zeros(K, ldM) if (train and not use_mn) else None
-            plan.add_im2col(P(cur["buf"]), B, h, w, cin, kh, kw, P(patches), ldK, P(patchesT), ldM if patchesT is not None else 0)
+            plan.add_im2col(P(cur["buf"]), B, h, w, cin, kh, kw, P(patches), ldK, P(patchesT), ldM if patchesT is not None else 0,
+                            l.strides[0], l.strides[1], l.pads[0], l.pads[2], oh, ow)
             ks, bs = lay.by_name(l.kernel), (lay.by_name(l.bias) if l.bias else None)
             act_out = zeros(M, cout)
             g = C.Gemm(dict(a=P(patches), lda=ldK, b=P(wsrc) + ks.wt_off * 2, ldb=ks.wt_ld, M=M, N=cout, K=K,
@@ -322,12 +353,17 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             continue
         if l.kind == "pool":
             h, w, c = cur["shape"]
-            oh, ow = h // 2, w // 2
+            oh, ow = l.out_shape[0], l.out_shape[1]
             pooled = zeros(B, oh * ow * c)
             argmax = zeros(B, oh * ow * c, dtype=torch.uint8)
-            nxt_dense = (i + 2 < len(layers) and layers[i + 1].kind == "reshape" and layers[i + 2].kind == "dense")
-            flatT = zeros(oh * ow * c, ldB) if (train and nxt_dense and not use_mn) else None
-            plan.add_maxpool_fwd(P(cur["buf"]), B, h, w, c, P(pooled), P(argmax), P(flatT), ldB if flatT is not None else 0)
+            flatT = None
+            if pool_fast_path(l):
+                nxt_dense = (i + 2 < len(layers) and layers[i + 1].kind == "reshape" and layers[i + 2].kind == "dense")
+                flatT = zeros(oh * ow * c, ldB) if (train and nxt_dense and not use_mn) else None
+                plan.add_maxpool_fwd(P(cur["buf"]), B, h, w, c, P(pooled), P(argmax), P(flatT), ldB if flatT is not None else 0)
+            else:
+                plan.add_maxpool_gen_fwd(P(cur["buf"]), B, h, w, c, l.ksize[0], l.ksize[1], l.strides[0], l.strides[1], l.pads[0], l.pads[2],
+                                         oh, ow, P(pooled), P(argmax))
             rec[i] = dict(argmax=argmax, in_shape=(h, w, c), conv=cur.get("conv"), pooled=pooled)
             cur = dict(kind="img", buf=pooled, shape=(oh, ow, c), flatT=flatT)
             continue
@@ -442,7 +478,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 dg = C.Gemm(dd)
                 emit(dg, f"dgrad{i}")
                 g_dz, g_dzT = ndz, ndzT
-            else:                                  # flatten over a pooled image: gradient wrt the pooled tensor
+            else:                                  # flatten over an image: gradient wrt the pooled tensor / the conv activation
                 g_img = zeros(B, ks.rows)
                 dg = C.Gemm(dict(a=P(g_dz), lda=g_dz.shape[1], b=P(wsrc) + ks.w_off * 2, ldb=ks.w_ld, M=B, N=ks.rows, K=ks.cols,
                                  out_bf16=P(g_img), ld_bf16=ks.rows))
@@ -459,7 +495,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             h, w, cin = cr["in_shape"]
             plan.add_conv_first_wgrad(P(cr["x"]), B, h, w, cin, conv_l.ksize[0], conv_l.ksize[1], ks.cols, P(g_img), P(cr["pooled"]),
                                       P(cr["argmax"]), ACT_IDS[conv_l.act], P(worker.grads) + ks.offset * 4,
-                                      P(worker.grads) + cb.offset * 4 if cb else 0)
+                                      P(worker.grads) + cb.offset * 4 if cb else 0, conv_l.pads[0], conv_l.pads[2], conv_l.out_shape[0],
+                                      conv_l.out_shape[1])
             break                                  # it is the first trainable layer: nothing below needs a gradient
         if l.kind == "pool":
             r = rec[i]
@@ -470,13 +507,26 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             need_dz = ci != first_trainable or use_mn   # conv dgrad (and the MN-major wgrad) read the row-major dz
             dzc = zeros(cr["M"], c) if need_dz else None
             dzcT = None if use_mn else zeros(c, cr["ldM"])
-            plan.add_maxpool_bwd(P(g_img), P(r["argmax"]), B, h, w, c, P(cr["act_out"]), ACT_IDS[conv_l.act], P(dzc), c if need_dz else 0,
-                                 P(dzcT), cr["ldM"] if dzcT is not None else 0, P(worker.grads) + cb.offset * 4 if cb else 0)
+            if pool_fast_path(l):
+                plan.add_maxpool_bwd(P(g_img), P(r["argmax"]), B, h, w, c, P(cr["act_out"]), ACT_IDS[conv_l.act], P(dzc), c if need_dz else 0,
+                                     P(dzcT), cr["ldM"] if dzcT is not None else 0, P(worker.grads) + cb.offset * 4 if cb else 0)
+            else:                                   # check_grammar keeps general pools off the K-major path: dz is row-major only
+                plan.add_maxpool_gen_bwd(P(g_img), P(r["argmax"]), B, h, w, c, l.ksize[0], l.ksize[1], l.strides[0], l.strides[1], l.pads[0],
+                                         l.pads[2], l.out_shape[0], l.out_shape[1], P(cr["act_out"]), ACT_IDS[conv_l.act], P(dzc), c,
+                                         P(worker.grads) + cb.offset * 4 if cb else 0)
             rec[ci]["dz"], rec[ci]["dzT"] = dzc, dzcT
             continue
         if l.kind == "conv":
             ks = lay.by_name(l.kernel)
             r = rec[i]
+            if i + 1 >= len(layers) or layers[i + 1].kind != "pool":
+                # no pool after this conv: g_img is the gradient wrt its activation output (col2im of the next conv or the
+                # flatten dgrad); dz = g * act'(a) and the bias gradient come from one kernel
+                cb = lay.by_name(l.bias) if l.bias else None
+                dzc = zeros(r["M"], ks.cols)
+                plan.add_act_bwd_bias(P(g_img), ks.cols, r["M"], ks.cols, P(r["act_out"]), ACT_IDS[l.act], P(dzc), ks.cols,
+                                      P(worker.grads) + cb.offset * 4 if cb else 0)
+                r["dz"], r["dzT"] = dzc, None
             kblocks = (r["M"] + 63) // 64
             tiles = ((r["K"] + 127) // 128) * max(1, (ks.cols + 63) // 64)
             if use_mn:
@@ -505,7 +555,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             gemms.append(dg)
             plan.add_gemm(dg, f"dgrad{i}")
             g_img = zeros(B, h * w * cin)
-            plan.add_col2im(P(dpatch), r["ldK"], B, h, w, cin, l.ksize[0], l.ksize[1], P(g_img))
+            plan.add_col2im(P(dpatch), r["ldK"], B, h, w, cin, l.ksize[0], l.ksize[1], P(g_img), l.strides[0], l.strides[1], l.pads[0],
+                            l.pads[2], l.out_shape[0], l.out_shape[1])
             continue
     if sharded and with_push:
         # forward the 1-D tail (bias gradients, all complete by now on the main branch) beside the last wgrad, so the post
