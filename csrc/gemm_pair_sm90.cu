@@ -112,7 +112,7 @@ sf_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       if (ct < kPairBN) s_bias[ct] = (ep.bias != nullptr && n0 + ct < N) ? ep.bias[n0 + ct] : 0.f;
       stage_acc<kPairBN>(stg, acc, ct);
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      epilogue_tile<kPairBN, false>(ep, stg, s_bias, m0, n0, M, N, ct);
+      epilogue_tile<kPairBN, kEpiPair>(ep, stg, s_bias, m0, n0, M, N, ct);
     }
   }
 

@@ -16,6 +16,9 @@
 //   * column sums (bias gradient) via an in-register transpose-reduce + one red per column,
 //   * fp32 store or atomic accumulate (split-K / straight into the flat gradient buffer that the
 //     push kernel consumes).
+// The generic kernel (sf_gemm_kernel) tests each of these at run time.  The training GEMMs run specialized variants
+// (sf_gemm_epi_kernel, one per SfEpi kind) that contain only their own epilogue code, a fifth to a half of the generic
+// kernel's; the DGRAD / LOSS variants also fetch their act'(aux) / label rows before the main loop.
 //
 // The B operand may live in *peer* GPU memory: the tensor map simply carries the peer-mapped
 // address, and the TMA engine pulls weight tiles over NVLink while the MMA pipeline runs
@@ -104,20 +107,39 @@ __device__ __forceinline__ void colsum_step(float (&r)[32], int lane) {
   }
 }
 
+// Epilogue feature sets.  EPI is an SfEpi value, or kEpiPair: the generic set without the loss heads (the cluster-pair
+// kernel never runs a loss).  The generic sets test every feature at run time; a specialized variant compiles in only
+// its own features, and sf_gemm_prepare selects it only when the features it leaves out are absent and the ones it
+// keeps unconditionally (the bf16 / fp32 output, the aux operand) are present.
+constexpr int kEpiPair = -1;
+template <int EPI>
+struct EpiFeatures {
+  static constexpr bool kGeneric = EPI == SF_EPI_GENERIC || EPI == kEpiPair;
+  static constexpr bool kAct = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS;
+  static constexpr bool kLoss = EPI == SF_EPI_GENERIC || EPI == SF_EPI_LOSS;
+  static constexpr bool kAux = kGeneric || EPI == SF_EPI_DGRAD;
+  static constexpr bool kColsum = kGeneric || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD;
+  static constexpr bool kF32 = kGeneric || EPI == SF_EPI_WGRAD;
+  static constexpr bool kBf16 = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD;
+  // the thread's act'(aux) chunk / label row are fetched before the main loop (epi_prefetch)
+  static constexpr bool kPrefetch = EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD;
+};
+
 // One 32-column chunk of a thread's output row: everything between the accumulator (v, already in registers) and
 // global memory.  `aux_pref` / `tgt_pref` are the act'(a) operand / label row of this chunk when the caller fetched
-// them before the accumulator wait (nullptr: read here).  kLoss compiles the fused softmax-CE / MSE heads in.
-template <bool kLoss>
+// them before the accumulator wait (nullptr: read here).
+template <int EPI>
 __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32_t (&v)[32], const float* s_bias32, int row, bool row_ok,
                                           int col0, int M, int N, int lane, const uint4* aux_pref, const float* tgt_pref,
                                           unsigned long long* tq = nullptr) {
+    using F = EpiFeatures<EPI>;
     float f[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]) * ep.alpha + s_bias32[j];
     if (tq != nullptr) tq[0] = trace_now();
-    act_fwd32(f, ep.act);
+    if (F::kAct) act_fwd32(f, ep.act);
     if (tq != nullptr) tq[1] = trace_now();
-    if (ep.drop_keep > 0.f && ep.drop_keep < 1.f) {
+    if (F::kGeneric && ep.drop_keep > 0.f && ep.drop_keep < 1.f) {
       // fused dropout: keep with probability drop_keep, scale the survivors by 1 / drop_keep
       const float inv_keep = __fdividef(1.f, ep.drop_keep);
       const uint32_t thr = static_cast<uint32_t>(fminf(ep.drop_keep * 4294967296.f, 4294967040.f));
@@ -133,7 +155,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
       }
     }
     if (tq != nullptr) tq[2] = trace_now();
-    if (kLoss && ep.loss_mode == SF_LOSS_SOFTMAX_XENT) {
+    if (F::kLoss && ep.loss_mode == SF_LOSS_SOFTMAX_XENT) {
       // whole row lives in this thread (host guarantees N <= 32): softmax + CE + gradient in registers
       const float* yv = tgt_pref;                         // N <= 32: the single chunk was prefetched
       const int nvalid = row_ok ? (N - col0 < 32 ? N - col0 : 32) : 0;
@@ -159,7 +181,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) lrow += __shfl_xor_sync(0xffffffffu, lrow, o);
       if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow);
-    } else if (kLoss && ep.loss_mode == SF_LOSS_MSE) {
+    } else if (F::kLoss && ep.loss_mode == SF_LOSS_MSE) {
       const float scale = 2.f / (static_cast<float>(M) * static_cast<float>(N));
       const float* tp = ep.target + static_cast<size_t>(row_ok ? row : 0) * ep.ld_target + col0;
       float lrow = 0.f;
@@ -181,7 +203,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
       if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow * 0.5f * scale);
     }
     if (tq != nullptr) tq[3] = trace_now();
-    if (ep.aux != nullptr && row_ok) {
+    if (F::kAux && (!F::kGeneric || ep.aux != nullptr) && row_ok) {
       const __nv_bfloat16* ap = ep.aux + static_cast<size_t>(row) * ep.ld_aux + col0;
       float a32[32];
 #pragma unroll
@@ -196,7 +218,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
           a32[g * 8 + 2 * t + 1] = a2.y;
         }
       }
-      act_bwd32(f, a32, ep.aux_act, ep.aux_keep);
+      act_bwd32(f, a32, ep.aux_act, F::kGeneric ? ep.aux_keep : 0.f);
     }
     if (tq != nullptr) tq[4] = trace_now();
     // padded columns / rows contribute exact zeros everywhere below
@@ -204,7 +226,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
     for (int j = 0; j < 32; ++j)
       if (col0 + j >= N || !row_ok) f[j] = 0.f;
 
-    if (ep.colsum != nullptr) {
+    if (F::kColsum && ep.colsum != nullptr) {
       // transpose-reduce over the 32 rows held by this warp: 31 shuffles, lane j ends up with
       // the sum of column col0 + j.
       float r[32];
@@ -220,9 +242,9 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
     }
 
     if (tq != nullptr) tq[5] = trace_now();          // tracer: math done, stores follow
-    if ((ep.out_f32 != nullptr || ep.route != nullptr) && row_ok) {
+    if (F::kF32 && (!F::kGeneric || ep.out_f32 != nullptr || ep.route != nullptr) && row_ok) {
       float* op;
-      if (ep.route != nullptr) {
+      if (F::kGeneric && ep.route != nullptr) {
         // push fused into the wgrad epilogue: this 32-column chunk lies inside ONE 32 x 64 push tile; its gradient goes
         // straight into this worker's mailbox on the GPU that owns the tile (NVLink peer stores / reds)
         const int tile = ep.route_tile0 + (row >> 5) * ep.route_tiles_c + (col0 >> 6);
@@ -250,7 +272,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
       }
     }
     if (tq != nullptr) tq[6] = trace_now();
-    if (ep.out_bf16 != nullptr && row_ok) {
+    if (F::kBf16 && (!F::kGeneric || ep.out_bf16 != nullptr) && row_ok) {
       __nv_bfloat16* op = ep.out_bf16 + static_cast<size_t>(row) * ep.ld_bf16 + col0;
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
@@ -265,7 +287,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
       }
     }
     if (tq != nullptr) tq[7] = trace_now();
-    if (ep.outT_bf16 != nullptr && row_ok) {
+    if (F::kGeneric && ep.outT_bf16 != nullptr && row_ok) {
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (col0 + j < N)
@@ -342,11 +364,36 @@ __device__ __forceinline__ void stage_acc(float* stg, const float (&acc)[BN / 2]
   for (int j = 0; j < BN / 2; ++j) stg[(r0 + 8 * ((j >> 1) & 1)) * (BN + 1) + 8 * (j >> 2) + c0 + (j & 1)] = acc[j];
 }
 
+// The act'(aux) chunk (DGRAD) or label row (LOSS) that consumer thread ct's epilogue reads, fetched before the main loop
+// so that the load's latency hides under it.  Earlier launches wrote both, and everything upstream of this grid is
+// complete once pdl_wait has returned.  BN <= 64: a thread owns at most one chunk (c = q / 4, see epilogue_tile).
+template <int BN, int EPI>
+__device__ __forceinline__ void epi_prefetch(const SfGemmEpilogue& ep, uint4 (&aux)[4], float (&tgt)[32], int m0, int n0, int M, int N,
+                                             int ct) {
+  static_assert(BN <= 64, "one 32-column chunk per consumer thread");
+  const int q = ct >> 5, lane = ct & 31;
+  const int row = m0 + (q & 3) * 32 + lane;
+  const int col0 = n0 + (q >> 2) * 32;
+  const bool live = row < M && (q >> 2) < BN / 32 && col0 < ep.n_store_limit;
+  if constexpr (EPI == SF_EPI_DGRAD) {
+    const __nv_bfloat16* ap = ep.aux + static_cast<size_t>(live ? row : 0) * ep.ld_aux + col0;
+#pragma unroll
+    for (int g = 0; g < 4; ++g)
+      aux[g] = (live && col0 + g * 8 < ep.ld_aux) ? *reinterpret_cast<const uint4*>(ap + g * 8) : make_uint4(0u, 0u, 0u, 0u);
+  } else {
+    const float* tp = ep.target + static_cast<size_t>(live ? row : 0) * ep.ld_target + col0;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) tgt[j] = (live && col0 + j < N) ? tp[j] : 0.f;
+  }
+}
+
 // Epilogue of one 128 x BN tile from the staged accumulator, by the 256 consumer threads: warp q owns rows
-// 32 * (q % 4) .. + 32 (one row per lane) and every other 32-column chunk starting at chunk q / 4.
-template <int BN, bool kLoss>
+// 32 * (q % 4) .. + 32 (one row per lane) and every other 32-column chunk starting at chunk q / 4.  aux_pref / tgt_pref:
+// the thread's chunk fetched by epi_prefetch (variants with EpiFeatures::kPrefetch only).
+template <int BN, int EPI>
 __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const float* stg, const float* s_bias, int m0, int n0, int M,
-                                              int N, int ct) {
+                                              int N, int ct, const uint4* aux_pref = nullptr, const float* tgt_pref = nullptr) {
+  using F = EpiFeatures<EPI>;
   const int q = ct >> 5, lane = ct & 31;
   const int r = (q & 3) * 32 + lane;
   const int row = m0 + r;
@@ -359,13 +406,17 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
     uint32_t v[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(srow[c * 32 + j]);
-    float tgt[32];
-    if (kLoss && ep.loss_mode != SF_LOSS_NONE) {
-      const float* tp = ep.target + static_cast<size_t>(row_ok ? row : 0) * ep.ld_target + col0;
+    if constexpr (F::kPrefetch) {
+      epi_chunk<EPI>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, aux_pref, tgt_pref);
+    } else {
+      float tgt[32];
+      if (F::kLoss && ep.loss_mode != SF_LOSS_NONE) {
+        const float* tp = ep.target + static_cast<size_t>(row_ok ? row : 0) * ep.ld_target + col0;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) tgt[j] = (row_ok && col0 + j < N) ? tp[j] : 0.f;
+        for (int j = 0; j < 32; ++j) tgt[j] = (row_ok && col0 + j < N) ? tp[j] : 0.f;
+      }
+      epi_chunk<EPI>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, nullptr, F::kLoss ? tgt : nullptr);
     }
-    epi_chunk<kLoss>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, nullptr, kLoss ? tgt : nullptr);
   }
 }
 
@@ -373,11 +424,12 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 // run the wgmma main loop for 64 rows of the tile and then, together, the epilogue.
 // MN: both operands MN-major (D = a^T . b with a [K, M], b [K, N] row-major): the stage buffers have the same size, but a
 // stage is filled with {64 MN elements, 64 K rows} boxes and described to the tensor core as MN-major.
-template <int BN, bool MN = false>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+// EPI: epilogue feature set (SfEpi); only the generic kernel handles the fused read-your-writes wait.
+template <int BN, bool MN, int EPI>
+__device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorMap& tmB, const SfGemmEpilogue& ep, int M, int N,
+                                         int K, int kblocks_per_split) {
   static_assert(!MN || BN % 64 == 0, "MN-major B needs whole 64-element swizzle atoms");
+  using F = EpiFeatures<EPI>;
   using S = GemmSmem<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
@@ -392,7 +444,7 @@ sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // successors launch when it completes) - they must not sit on SMs that the shard applier whose acknowledgement it
   // waits for needs for its own CTAs.  A grid of several waves triggers at entry: its successor's CTAs only get SMs as
   // this grid drains.  A one-wave grid triggers after its main loop, see there.
-  if (ep.ryw == nullptr && !ep.one_wave) pdl_launch_dependents();
+  if ((!F::kGeneric || ep.ryw == nullptr) && !ep.one_wave) pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * BN;
@@ -419,7 +471,7 @@ sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      if (ep.ryw != nullptr) {
+      if (F::kGeneric && ep.ryw != nullptr) {
         // pull fused into this GEMM: read-your-writes wait before the first weight tile is fetched (local spin)
         const SfRyw& w = *ep.ryw;
         const uint32_t posted = *w.my_posted;
@@ -470,22 +522,47 @@ sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   } else {
     // ===================== wgmma main loop + epilogue =====================
     const int ct = threadIdx.x - 128;
+    uint4 aux_pref[4];
+    float tgt_pref[32];
+    if constexpr (F::kPrefetch) epi_prefetch<BN, EPI>(ep, aux_pref, tgt_pref, m0, n0, M, N, ct);
     float acc[BN / 2];
     mma_mainloop<BN, MN, S::kStages, S::kStageBytes, S::kABytes>(acc, stage_base, full_bar, empty_bar, 0, num_kb, ct >> 7,
                                                                  (ct & 127) == 0, 0x200);
     // One-wave grid: the successor launches once every CTA is past its main loop, so its launch and prologue overlap
     // this epilogue.  A trigger at entry would let a chain of small GEMMs pre-launch in a cascade, and those waiting
     // CTAs (one per SM at this register / shared-memory size, 149 for the push) hold SMs the GEMMs ahead of them need.
-    if (ep.ryw == nullptr && ep.one_wave) pdl_launch_dependents();
+    if ((!F::kGeneric || ep.ryw == nullptr) && ep.one_wave) pdl_launch_dependents();
     // every stage has been consumed by both warpgroups: the ring holds the staged accumulator tile from here on
     float* stg = reinterpret_cast<float*>(stage_base);
     asm volatile("bar.sync 1, 256;" ::: "memory");
     stage_acc<BN>(stg, acc, ct);
     asm volatile("bar.sync 1, 256;" ::: "memory");
     asm volatile("bar.sync 2, 352;" ::: "memory");      // bias tile in shared memory
-    epilogue_tile<BN, true>(ep, stg, s_bias, m0, n0, M, N, ct);
+    if constexpr (F::kPrefetch) {
+      epilogue_tile<BN, EPI>(ep, stg, s_bias, m0, n0, M, N, ct, aux_pref, tgt_pref);
+    } else {
+      epilogue_tile<BN, EPI>(ep, stg, s_bias, m0, n0, M, N, ct);
+    }
   }
   trace.end(KID_GEMM);
+}
+
+// The generic kernel: every epilogue feature, each behind a runtime test.
+template <int BN, bool MN = false>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  gemm_cta<BN, MN, SF_EPI_GENERIC>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+
+// A specialized epilogue variant (EPI != SF_EPI_GENERIC): a fraction of the generic kernel's code, which matters because
+// the epilogue runs once per launch on a cold instruction cache.
+template <int BN, bool MN, int EPI>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  static_assert(EPI != SF_EPI_GENERIC, "the generic epilogue is sf_gemm_kernel");
+  gemm_cta<BN, MN, EPI>(tmA, tmB, ep, M, N, K, kblocks_per_split);
 }
 
 // ---------------------------------------------------------------------------
@@ -551,6 +628,24 @@ extern "C" int sf_gemm_pick_bn(int M, int N) {
   return 32;
 }
 
+// The specialized epilogue variant that computes exactly what the generic kernel would for this GEMM, or SF_EPI_GENERIC.
+// Variants exist only at the tile shapes the dense training plans use: K-major BN 32 / 64, MN-major (WGRAD) BN 64 / 128.
+static int pick_epi(const SfGemm* g) {
+  const SfGemmEpilogue& e = g->ep;
+  const bool dropout = e.drop_keep > 0.f && e.drop_keep < 1.f;
+  const bool aux_dropout = e.aux_keep > 0.f && e.aux_keep < 1.f;
+  if (g->pair || dropout || e.route != nullptr || e.ryw != nullptr || e.outT_bf16 != nullptr) return SF_EPI_GENERIC;
+  if (g->mn_major) {
+    const bool wgrad = (g->bn == 64 || g->bn == 128) && e.out_f32 != nullptr && e.out_bf16 == nullptr && e.aux == nullptr &&
+                       e.colsum == nullptr && e.act == SF_ACT_NONE && e.loss_mode == SF_LOSS_NONE;
+    return wgrad ? SF_EPI_WGRAD : SF_EPI_GENERIC;
+  }
+  if ((g->bn != 32 && g->bn != 64) || e.out_bf16 == nullptr || e.out_f32 != nullptr) return SF_EPI_GENERIC;
+  if (e.loss_mode != SF_LOSS_NONE) return e.aux == nullptr ? SF_EPI_LOSS : SF_EPI_GENERIC;
+  if (e.aux != nullptr) return (!aux_dropout && e.act == SF_ACT_NONE) ? SF_EPI_DGRAD : SF_EPI_GENERIC;
+  return e.colsum == nullptr ? SF_EPI_FWD : SF_EPI_GENERIC;
+}
+
 extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return -2;
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
@@ -597,27 +692,47 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->ep.out_bf16 && g->ep.ld_bf16 > lim) lim = g->ep.ld_bf16;
   g->ep.n_store_limit = lim;
   g->ep.one_wave = static_cast<long long>((g->N + g->bn - 1) / g->bn) * ((g->M + sf::kBM - 1) / sf::kBM) * g->split_k <= sf_num_sms();
+  g->epi = g->epi == SF_EPI_GENERIC ? SF_EPI_GENERIC : pick_epi(g);
   return 0;
 }
 
-template <int BN, bool MN = false>
+template <int BN, bool MN = false, int EPI = SF_EPI_GENERIC>
 static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
   using S = sf::GemmSmem<BN>;
+  auto kernel = [] {
+    if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
+    else return sf::sf_gemm_epi_kernel<BN, MN, EPI>;
+  }();
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(sf::sf_gemm_kernel<BN, MN>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, S::kBytes);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kBytes);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   dim3 grid((g->N + BN - 1) / BN, (g->M + sf::kBM - 1) / sf::kBM, g->split_k);
-  return sf::launch(sf::sf_gemm_kernel<BN, MN>, grid, dim3(sf::kGemmThreads), S::kBytes, st, g->tmA, g->tmB, g->ep,
+  return sf::launch(kernel, grid, dim3(sf::kGemmThreads), S::kBytes, st, g->tmA, g->tmB, g->ep,
                     g->M, g->N, g->K, g->kblocks_per_split);
+}
+
+// K-major epilogue variants exist at BN 32 and 64 (pick_epi)
+template <int EPI>
+static cudaError_t launch_kmajor_variant(const SfGemm* g, cudaStream_t st) {
+  return g->bn == 32 ? launch_bn<32, false, EPI>(g, st) : launch_bn<64, false, EPI>(g, st);
 }
 
 extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
   if (g->pair) return sf_gemm_pair_launch(g, st);
   cudaError_t e;
+  switch (g->epi) {
+    case SF_EPI_GENERIC: break;
+    case SF_EPI_FWD: return static_cast<int>(launch_kmajor_variant<SF_EPI_FWD>(g, st));
+    case SF_EPI_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_LOSS>(g, st));
+    case SF_EPI_DGRAD: return static_cast<int>(launch_kmajor_variant<SF_EPI_DGRAD>(g, st));
+    case SF_EPI_WGRAD:
+      e = g->bn == 64 ? launch_bn<64, true, SF_EPI_WGRAD>(g, st) : launch_bn<128, true, SF_EPI_WGRAD>(g, st);
+      return static_cast<int>(e);
+    default: return -3;
+  }
   if (g->mn_major) {
     switch (g->bn) {
       case 64: e = launch_bn<64, true>(g, st); break;

@@ -31,6 +31,18 @@ extern "C" int sf_preload_kernels() {
   SF_SMEM_ATTR(sf::sf_gemm_kernel<128>, sf::GemmSmem<128>::kBytes); SF_SMEM_ATTR(sf::sf_gemm_kernel<256>, sf::GemmSmem<256>::kBytes);
   SF_SMEM_ATTR((sf::sf_gemm_kernel<64, true>), sf::GemmSmem<64>::kBytes); SF_SMEM_ATTR((sf::sf_gemm_kernel<128, true>), sf::GemmSmem<128>::kBytes);
   SF_PRELOAD((sf::sf_gemm_kernel<64, true>)); SF_PRELOAD((sf::sf_gemm_kernel<128, true>));
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<32, false, SF_EPI_FWD>), sf::GemmSmem<32>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<64, false, SF_EPI_FWD>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<32, false, SF_EPI_LOSS>), sf::GemmSmem<32>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<64, false, SF_EPI_LOSS>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<32, false, SF_EPI_DGRAD>), sf::GemmSmem<32>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<64, false, SF_EPI_DGRAD>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<64, true, SF_EPI_WGRAD>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_kernel<128, true, SF_EPI_WGRAD>), sf::GemmSmem<128>::kBytes);
+  SF_PRELOAD((sf::sf_gemm_epi_kernel<32, false, SF_EPI_FWD>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<64, false, SF_EPI_FWD>));
+  SF_PRELOAD((sf::sf_gemm_epi_kernel<32, false, SF_EPI_LOSS>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<64, false, SF_EPI_LOSS>));
+  SF_PRELOAD((sf::sf_gemm_epi_kernel<32, false, SF_EPI_DGRAD>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<64, false, SF_EPI_DGRAD>));
+  SF_PRELOAD((sf::sf_gemm_epi_kernel<64, true, SF_EPI_WGRAD>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<128, true, SF_EPI_WGRAD>));
   SF_SMEM_ATTR(sf::sf_gemm_pair_kernel, sf::kPairSmemBytes);
   SF_PRELOAD(sf::sf_gemm_kernel<32>); SF_PRELOAD(sf::sf_gemm_kernel<64>); SF_PRELOAD(sf::sf_gemm_kernel<128>); SF_PRELOAD(sf::sf_gemm_kernel<256>); SF_PRELOAD(sf::sf_gemm_pair_kernel);
   SF_PRELOAD(sf::hostcopy_kernel); SF_PRELOAD(sf::gather_rows_f32_kernel); SF_PRELOAD(sf::fetch_kernel); SF_PRELOAD(sf::cast_transpose_kernel<false>); SF_PRELOAD(sf::cast_transpose_kernel<true>);

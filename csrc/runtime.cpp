@@ -71,6 +71,7 @@ struct Gemm {
     g.pair = getd<int>(d, "pair", -1);
     g.mn_major = getd<int>(d, "mn_major", 0);
     g.pair_ctas = getd<int>(d, "pair_ctas", 0);
+    g.epi = getd<int>(d, "epi", -1);
     g.ep.out_f32 = P<float>(getd<uintptr_t>(d, "out_f32", 0));
     g.ep.ld_f32 = getd<int>(d, "ld_f32", g.N);
     g.ep.out_bf16 = P<__nv_bfloat16>(getd<uintptr_t>(d, "out_bf16", 0));
@@ -109,6 +110,7 @@ struct Gemm {
   int bn() const { return g.bn; }
   int split_k() const { return g.split_k; }
   int pair() const { return g.pair; }
+  int epi() const { return g.epi; }
   py::tuple grid() const {
     return py::make_tuple((g.N + g.bn - 1) / g.bn, (g.M + 127) / 128, g.split_k);
   }
@@ -956,6 +958,7 @@ PYBIND11_MODULE(_C, m) {
       .def_property_readonly("bn", &Gemm::bn)
       .def_property_readonly("split_k", &Gemm::split_k)
       .def_property_readonly("pair", &Gemm::pair)
+      .def_property_readonly("epi", &Gemm::epi)
       .def("mn_major", &Gemm::mn_major)
       .def_property_readonly("grid", &Gemm::grid);
 

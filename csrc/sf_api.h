@@ -88,6 +88,14 @@ struct SfGemmEpilogue {
 
 enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2 };
 
+// Epilogue variant of the one-CTA GEMM kernel.  The generic kernel carries every epilogue feature behind runtime tests;
+// each specialized variant compiles in only the features of one kind of training GEMM (sf_gemm_prepare picks it):
+//   FWD   bias + activation -> bf16
+//   LOSS  bias (+ activation) + softmax-CE / MSE head -> dz bf16, loss, optional column sum
+//   DGRAD act'(aux) -> bf16, optional column sum
+//   WGRAD fp32 store or atomic accumulate (MN-major operands)
+enum SfEpi { SF_EPI_GENERIC = 0, SF_EPI_FWD = 1, SF_EPI_LOSS = 2, SF_EPI_DGRAD = 3, SF_EPI_WGRAD = 4 };
+
 
 struct SfGemm {
   CUtensorMap tmA, tmB;           // filled by sf_gemm_prepare
@@ -103,6 +111,7 @@ struct SfGemm {
                                   // stored, no transposed copies); 0: both K-major (a [M, lda], b [N, ldb])
   int pair;                       // in: -1 = auto, 0 = one-CTA kernel, 1 = force the persistent cluster-pair kernel; out: 0 / 1
   int pair_ctas;                  // CTAs of the persistent cluster-pair kernel (0 = one per SM)
+  int epi;                        // in: -1 = auto, SF_EPI_GENERIC = force the generic kernel; out: the SfEpi variant launched
   SfGemmEpilogue ep;
 };
 
