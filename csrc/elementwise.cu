@@ -211,110 +211,6 @@ argmax_rows_kernel(const float* __restrict__ in, int ld, float* __restrict__ out
 
 }  // namespace sf
 
-namespace sf {
-// Zero-copy host->device fetch: the SMs load straight from pinned, device-mapped host memory (PCIe reads issued by
-// ordinary ld.global), 4 x 16 B in flight per thread.  Used where a copy-engine DMA would sit on a critical path.
-__global__ void __launch_bounds__(256)
-hostcopy_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, size_t n16) {
-  TraceScope trace;
-  pdl_launch_dependents();
-  pdl_wait();
-  trace.mark();
-  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-  size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  for (; i + 3 * stride < n16; i += 4 * stride) {
-    const uint4 v0 = ld_stream_u4(src + i), v1 = ld_stream_u4(src + i + stride), v2 = ld_stream_u4(src + i + 2 * stride),
-                v3 = ld_stream_u4(src + i + 3 * stride);
-    dst[i] = v0; dst[i + stride] = v1; dst[i + 2 * stride] = v2; dst[i + 3 * stride] = v3;
-  }
-  for (; i < n16; i += stride) dst[i] = ld_stream_u4(src + i);
-  trace.end(KID_CAST);
-}
-}  // namespace sf
-
-namespace sf {
-// In-graph minibatch fetch (see SfFetchArgs): the minibatch is ONE contiguous run of the pinned partition, so it is
-// streamed linearly (16-byte loads, 8 in flight per thread, a few CTAs) into an fp32 staging buffer; the cast /
-// transpose to the GEMM operand layouts is a second, device-local kernel on the same graph branch.  (A tiled access
-// pattern from many CTAs touches hundreds of host pages at once and collapses to ~8 GB/s behind an IOMMU; the linear
-// stream runs at the PCIe rate.)  The last CTA bumps the fetch sequence number.
-__device__ __forceinline__ void fetch_linear(const float* __restrict__ src, float* __restrict__ dst, long long n, int tid_global, int nthreads) {
-  const bool vec = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
-  long long done = 0;
-  if (vec) {
-    const long long n4 = n / 4;
-    const float4* s4 = reinterpret_cast<const float4*>(src);
-    float4* d4 = reinterpret_cast<float4*>(dst);
-    long long i = tid_global;
-    for (; i + 7ll * nthreads < n4; i += 8ll * nthreads) {
-      float4 v[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) v[k] = ld_stream_f4(s4 + i + static_cast<long long>(k) * nthreads);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) d4[i + static_cast<long long>(k) * nthreads] = v[k];
-    }
-    for (; i < n4; i += nthreads) d4[i] = ld_stream_f4(s4 + i);
-    done = n4 * 4;
-  }
-  for (long long i = done + tid_global; i < n; i += nthreads) dst[i] = src[i];
-}
-
-__global__ void __launch_bounds__(256)
-fetch_kernel(const SfFetchArgs a) {
-  __shared__ long long s_start;
-  TraceScope trace;
-  pdl_launch_dependents();
-  pdl_wait();
-  trace.mark();
-  const int tid = threadIdx.x;
-  const SfFetchDesc d = *a.desc;
-  if (tid == 0) {
-    const unsigned int q = *a.counter;
-    s_start = *reinterpret_cast<const volatile long long*>(a.sched + (q & a.ring_mask));     // zero-copy read of the schedule
-  }
-  __syncthreads();
-  const long long start = s_start;
-  const int gtid = blockIdx.x * blockDim.x + tid, nthr = gridDim.x * blockDim.x;
-  const float* x = d.x_host + start * d.x_ld;
-  if (d.x_ld == a.cols) {
-    fetch_linear(x, a.x_out, static_cast<long long>(a.rows) * a.cols, gtid, nthr);
-  } else {
-    for (int r = 0; r < a.rows; ++r) fetch_linear(x + r * d.x_ld, a.x_out + static_cast<long long>(r) * a.cols, a.cols, gtid, nthr);
-  }
-  if (a.y_out != nullptr) {
-    const float* y = d.y_host + start * d.y_ld;
-    if (d.y_ld == a.y_cols) {
-      fetch_linear(y, a.y_out, static_cast<long long>(a.rows) * a.y_cols, gtid, nthr);
-    } else {
-      for (int r = 0; r < a.rows; ++r) fetch_linear(y + r * d.y_ld, a.y_out + static_cast<long long>(r) * a.y_cols, a.y_cols, gtid, nthr);
-    }
-  }
-  __syncthreads();
-  if (tid == 0) {
-    __threadfence();
-    const unsigned int prev = atomicAdd(a.sync, 1u);
-    if (prev == gridDim.x - 1) {
-      *a.sync = 0;
-      *a.counter = *a.counter + 1;
-    }
-  }
-  trace.end(KID_CAST);
-}
-}  // namespace sf
-
-extern "C" int sf_fetch_launch(const SfFetchArgs* a, int grid, cudaStream_t st) {
-  if (grid <= 0) grid = 8;
-  if (!a->desc || !a->sched || !a->counter || !a->sync || !a->x_out) return -8;
-  return static_cast<int>(sf::launch(sf::fetch_kernel, dim3(grid), dim3(256), 0, st, *a));
-}
-
-extern "C" int sf_hostcopy(const void* src_host, void* dst, size_t bytes, int grid, cudaStream_t st) {
-  if (bytes % 16) return -7;
-  if (grid <= 0) grid = 32;
-  return static_cast<int>(sf::launch(sf::hostcopy_kernel, dim3(grid), dim3(256), 0, st, static_cast<const uint4*>(src_host),
-                                     static_cast<uint4*>(dst), bytes / 16));
-}
-
 extern "C" int sf_cast_transpose(const float* in, int ld_in, __nv_bfloat16* out, int ld_out,
                                  __nv_bfloat16* outT, int ld_t, int rows, int cols, cudaStream_t st) {
   const int span_c = (out && ld_out > cols) ? ld_out : cols;

@@ -213,25 +213,6 @@ SfPostArgs parse_post(const py::dict& d) {
   return a;
 }
 
-SfFetchArgs parse_fetch(const py::dict& d) {
-  SfFetchArgs a;
-  std::memset(&a, 0, sizeof(a));
-  a.desc = P<const SfFetchDesc>(getd<uintptr_t>(d, "desc", 0));
-  a.sched = P<const long long>(getd<uintptr_t>(d, "sched", 0));
-  a.ring_mask = getd<unsigned int>(d, "ring_mask", 0);
-  a.counter = P<unsigned int>(getd<uintptr_t>(d, "counter", 0));
-  a.sync = P<unsigned int>(getd<uintptr_t>(d, "sync", 0));
-  a.x_out = P<float>(getd<uintptr_t>(d, "x_out", 0));
-  a.y_out = P<float>(getd<uintptr_t>(d, "y_out", 0));
-  a.rows = getd<int>(d, "rows", 0);
-  a.cols = getd<int>(d, "cols", 0);
-  a.y_cols = getd<int>(d, "y_cols", 0);
-  if (!a.desc || !a.sched || !a.counter || !a.sync || !a.x_out || a.rows <= 0 || a.cols <= 0)
-    throw std::runtime_error("fetch: desc/sched/counter/sync/x_out/rows/cols are required");
-  return a;
-}
-
-
 void fill_bounds(const py::dict& d, int n_shards, int* bounds) {
   auto b = getd<std::vector<int>>(d, "bounds", {});
   if (static_cast<int>(b.size()) != n_shards + 1) throw std::runtime_error("sharded: bounds must have n_shards + 1 entries");
@@ -358,9 +339,9 @@ SfPullArgs parse_pull(const py::dict& d) {
 class Plan {
  public:
   using Op = std::function<int(cudaStream_t)>;
-  static constexpr int kMaxBranches = 4;
+  static constexpr int kMaxBranches = 3;
   Plan() {
-    for (int i = 0; i < kMaxBranches; ++i) { side_[i] = nullptr; ev_[i] = nullptr; }
+    for (int i = 0; i < kMaxBranches; ++i) ev_[i] = nullptr;
   }
   ~Plan() {
     reset_graph();
@@ -456,7 +437,7 @@ class Plan {
     int kind;   // 0 = kernel op, 1 = fork, 2 = join
   };
   void add_ctl(int kind, int b, const char* name) {
-    if (b <= 0 || b >= kMaxBranches) throw std::runtime_error("plan: fork/join need a side branch id in [1,3]");
+    if (b <= 0 || b >= kMaxBranches) throw std::runtime_error("plan: fork/join need a side branch id in [1,2]");
     items_.push_back(Item{name, nullptr, b, kind});
     reset_graph();
   }
@@ -480,7 +461,6 @@ class Plan {
   }
   std::vector<Item> items_;
   int cur_branch_ = 0;
-  cudaStream_t side_[kMaxBranches];
   cudaStream_t cur_main_ = nullptr;
   cudaEvent_t ev_[kMaxBranches];
   cudaEvent_t ev_main_ = nullptr;
@@ -502,8 +482,6 @@ class StepDriver {
         y_host_(P<const char>(y_host)), y_row_(y_row_bytes), ring_(P<float>(loss_ring)), ring_len_(ring_len) {
     auto flag = [](const char* n) { const char* v = getenv(n); return v != nullptr && v[0] == '1'; };
     probe_ = flag("SPARKFLOW_DRV_PROBE");
-    no_h2d_ = flag("SPARKFLOW_DRV_NO_H2D");
-    if (const char* f = getenv("SPARKFLOW_DRV_H2D_FRAC")) h2d_frac_ = atof(f);      // diagnostics only
     if (probe_) ck(cudaEventCreate(&base_), "cudaEventCreate(base)");
   }
   ~StepDriver() {
@@ -558,10 +536,9 @@ class StepDriver {
         ck(cudaEventRecord(base_, compute_), "cudaEventRecord(base)");
         base_recorded_ = true;
       }
-      if (!no_h2d_)
-      ck(cudaMemcpyAsync(e.x_stage, x_host_ + static_cast<size_t>(sp[k]) * x_row_,
-                         static_cast<size_t>(static_cast<double>(e.batch) * h2d_frac_) * x_row_, cudaMemcpyHostToDevice, copy_), "cudaMemcpyAsync(x)");
-      if (e.y_stage && y_host_ && !no_h2d_)
+      ck(cudaMemcpyAsync(e.x_stage, x_host_ + static_cast<size_t>(sp[k]) * x_row_, static_cast<size_t>(e.batch) * x_row_,
+                         cudaMemcpyHostToDevice, copy_), "cudaMemcpyAsync(x)");
+      if (e.y_stage && y_host_)
         ck(cudaMemcpyAsync(e.y_stage, y_host_ + static_cast<size_t>(sp[k]) * y_row_, static_cast<size_t>(e.batch) * y_row_,
                            cudaMemcpyHostToDevice, copy_), "cudaMemcpyAsync(y)");
       if (e.prep) e.prep->replay(reinterpret_cast<uintptr_t>(copy_));
@@ -577,62 +554,6 @@ class StepDriver {
       ck(cudaEventRecord(e.free_, compute_), "cudaEventRecord(free)");
       const auto t5 = clk::now();
       host_ns_[0] += ns(t0, t1); host_ns_[1] += ns(t1, t2); host_ns_[2] += ns(t2, t3); host_ns_[3] += ns(t3, t4); host_ns_[4] += ns(t4, t5);
-      e.pending = step_;
-      e.primed = true;
-      ++step_;
-    }
-  }
-  // ---- zero-copy mode: the step graphs fetch their successor's minibatch themselves (fetch_kernel on a side
-  // branch), so one step costs the host ONE cudaGraphLaunch: no copy-engine DMA, no events.  Completion is a pinned
-  // word the step's last kernel writes (spun on by this thread); the minibatch schedule is a pinned ring the
-  // fetch kernel reads.  Plans must be registered in slot order: the graph of slot s fetches into slot s+1.
-  // `self_fetch_plans[s]`: an (un-captured) plan that fetches + prepares input set s, used for the first minibatch of a call
-  void enable_fetch(uintptr_t sched_host, int ring_len, py::list self_fetch_plans) {
-    if (ring_len <= 0 || (ring_len & (ring_len - 1))) throw std::runtime_error("StepDriver: schedule ring must be a power of two");
-    if (static_cast<size_t>(py::len(self_fetch_plans)) != entries_.size()) throw std::runtime_error("StepDriver: one fetch plan per step plan");
-    sched_ = P<long long>(sched_host);
-    sched_mask_ = static_cast<unsigned int>(ring_len - 1);
-    self_fetch_.clear();
-    self_fetch_keep_.clear();
-    for (auto item : self_fetch_plans) {
-      self_fetch_keep_.push_back(py::reinterpret_borrow<py::object>(item));
-      self_fetch_.push_back(item.cast<Plan*>());
-    }
-    fetch_mode_ = true;
-  }
-  void run_fetch(py::array_t<int32_t, py::array::c_style | py::array::forcecast> ids,
-                 py::array_t<int64_t, py::array::c_style | py::array::forcecast> starts) {
-    if (!fetch_mode_) throw std::runtime_error("StepDriver.run_fetch: enable_fetch first");
-    const int n = static_cast<int>(ids.size());
-    if (starts.size() != n) throw std::runtime_error("StepDriver.run_fetch: ids/starts length mismatch");
-    if (n == 0) return;
-    const int32_t* ip = ids.data();
-    const int64_t* sp = starts.data();
-    const int S_ = static_cast<int>(entries_.size());
-    py::gil_scoped_release nogil;
-    using clk = std::chrono::steady_clock;
-    auto ns = [](clk::time_point a, clk::time_point b) { return std::chrono::duration_cast<std::chrono::nanoseconds>(b - a).count(); };
-    // the first minibatch of this call is fetched by a stand-alone launch into the first plan's input set
-    if (ip[0] < 0 || ip[0] >= S_) throw std::runtime_error("StepDriver.run_fetch: bad plan id");
-    sched_[fetch_seq_ & sched_mask_] = sp[0];
-    ++fetch_seq_;
-    self_fetch_[ip[0]]->run(reinterpret_cast<uintptr_t>(compute_));
-    for (int k = 0; k < n; ++k) {
-      if (ip[k] < 0 || ip[k] >= S_) throw std::runtime_error("StepDriver.run_fetch: bad plan id");
-      if (k > 0 && ip[k] != (ip[k - 1] + 1) % S_) throw std::runtime_error("StepDriver.run_fetch: plan ids must walk the slots in order");
-      Entry& e = entries_[ip[k]];
-      const auto t0 = clk::now();
-      wait_done(e);
-      const auto t1 = clk::now();
-      // what this graph's fetch node brings in: the next step's minibatch (the last one re-reads its own rows)
-      sched_[fetch_seq_ & sched_mask_] = sp[k + 1 < n ? k + 1 : k];
-      ++fetch_seq_;
-      std::atomic_thread_fence(std::memory_order_seq_cst);
-      const auto t2 = clk::now();
-      e.plan->replay(reinterpret_cast<uintptr_t>(compute_));
-      const auto t3 = clk::now();
-      host_ns_[0] += ns(t0, t1); host_ns_[2] += ns(t1, t2); host_ns_[3] += ns(t2, t3);
-      ++e.launched;
       e.pending = step_;
       e.primed = true;
       ++step_;
@@ -691,7 +612,7 @@ class StepDriver {
     py::gil_scoped_release nogil;
     for (auto& e : entries_)
       if (e.primed && e.pending >= 0) {
-        if (fetch_mode_ || done_mode_) wait_done(e);
+        if (done_mode_) wait_done(e);
         else ck(cudaEventSynchronize(e.free_), "cudaEventSynchronize(flush)");
         harvest(e);
       }
@@ -715,7 +636,7 @@ class StepDriver {
     }
     ck(q, "cudaEventQuery(slot free)");
   }
-  // zero-copy mode: spin on the pinned completion word written by the step's last kernel (no CUDA call at all)
+  // resident mode: spin on the pinned completion word written by the step's last kernel (no CUDA call at all)
   void wait_done(Entry& e) {
     if (e.launched == 0) return;
     volatile unsigned int* done = reinterpret_cast<volatile unsigned int*>(e.loss_out) + 1;
@@ -735,7 +656,7 @@ class StepDriver {
     e.pending = -1;
   }
   void harvest(Entry& e) {
-    if (probe_ && !fetch_mode_ && e.pending >= 0 && probe_rows_.size() < 4096 * 4) {
+    if (probe_ && e.pending >= 0 && probe_rows_.size() < 4096 * 4) {
       float a = 0.f, b = 0.f, c = 0.f;
       cudaEventElapsedTime(&a, base_, e.ready);
       cudaEventElapsedTime(&b, base_, e.start);
@@ -750,7 +671,7 @@ class StepDriver {
   }
   struct Entry {
     long long pending = -1;
-    unsigned long long launched = 0;      // zero-copy mode: graph launches so far (the completion word counts them)
+    unsigned long long launched = 0;      // resident mode: graph launches so far (the completion word counts them)
     py::object keep, keep_prep;
     Plan* plan = nullptr;
     Plan* prep = nullptr;
@@ -770,14 +691,7 @@ class StepDriver {
   int ring_len_;
   long long step_ = 0;
   long long host_ns_[5] = {0, 0, 0, 0, 0};
-  bool probe_ = false, no_h2d_ = false, base_recorded_ = false;
-  double h2d_frac_ = 1.0;
-  bool fetch_mode_ = false, done_mode_ = false;
-  long long* sched_ = nullptr;
-  unsigned int sched_mask_ = 0;
-  unsigned long long fetch_seq_ = 0;
-  std::vector<Plan*> self_fetch_;
-  std::vector<py::object> self_fetch_keep_;
+  bool probe_ = false, base_recorded_ = false, done_mode_ = false;
   cudaEvent_t base_ = nullptr;
   std::vector<float> probe_rows_;      // (step, H2D done, graph may start, graph done) in us since the first step
   std::vector<Entry> entries_;
@@ -1120,10 +1034,6 @@ PYBIND11_MODULE(_C, m) {
         const SfPostFlagsArgs a = parse_post_flags(d);
         p.add("post_flags", [=](cudaStream_t st) { return sf_post_flags_launch(&a, st); });
       })
-      .def("add_fetch", [](Plan& p, const py::dict& d, int grid) {
-        const SfFetchArgs a = parse_fetch(d);
-        p.add("fetch", [=](cudaStream_t st) { return sf_fetch_launch(&a, grid, st); });
-      })
       .def("add_pull", [](Plan& p, const py::dict& d, uintptr_t local_sync, int grid) {
         const SfPullArgs a = parse_pull(d);
         p.add("pull", [=](cudaStream_t st) { return sf_pull_launch(&a, P<uint32_t>(local_sync), grid, st); });
@@ -1151,20 +1061,11 @@ PYBIND11_MODULE(_C, m) {
       .def("run", &StepDriver::run)
       .def("steps", &StepDriver::steps)
       .def("flush", &StepDriver::flush)
-      .def("enable_fetch", &StepDriver::enable_fetch)
-      .def("run_fetch", &StepDriver::run_fetch)
       .def("run_resident", &StepDriver::run_resident)
       .def("host_ns", &StepDriver::host_ns)
       .def("probe", &StepDriver::probe);
 
   // direct (un-planned) entry points, used by tests and the eager paths
-  m.def("fetch", [](const py::dict& d, int grid, uintptr_t stream) {
-    const SfFetchArgs a = parse_fetch(d);
-    ck_rc(sf_fetch_launch(&a, grid, S(stream)), "fetch");
-  });
-  m.def("hostcopy", [](uintptr_t src_host, uintptr_t dst, size_t bytes, int grid, uintptr_t stream) {
-    ck_rc(sf_hostcopy(P<const void>(src_host), P<void>(dst), bytes, grid, S(stream)), "hostcopy");
-  });
   m.def("cast_transpose", [](uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, uintptr_t outT,
                              int ld_t, int rows, int cols, uintptr_t stream) {
     ck_rc(idx ? sf_gather_cast_transpose(P<const float>(in), ld_in, P<const int32_t>(idx), P<__nv_bfloat16>(out),

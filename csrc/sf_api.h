@@ -136,25 +136,6 @@ unsigned int sf_trace_count();
 // ---------------------------------------------------------------------------
 // fp32 [rows, cols] (ld_in) -> bf16 [rows, ld_out] and optional transpose bf16 [cols, ld_t]
 int sf_gather_rows_f32(const float* in, int ld_in, const int32_t* idx, float* out, int ld_out, int rows, int cols, cudaStream_t st);
-int sf_hostcopy(const void* src_host, void* dst, size_t bytes, int grid, cudaStream_t st);
-
-// In-graph minibatch fetch (zero-copy): SM loads stream one minibatch (features + label rows, fp32) from the pinned
-// host partition into device staging, for the step AFTER the one whose graph contains this node.
-struct SfFetchDesc {              // lives in DEVICE memory (rewritten when the host partition moves)
-  const float* x_host; const float* y_host;
-  long long x_ld, y_ld;           // floats per row
-};
-struct SfFetchArgs {
-  const SfFetchDesc* desc;
-  const long long* sched;         // pinned host ring of minibatch row starts, indexed by the fetch sequence number
-  unsigned int ring_mask;
-  unsigned int* counter;          // device: fetches completed so far (= sequence number of this fetch)
-  unsigned int* sync;             // device: CTA arrival counter
-  float* x_out;                   // [rows, cols] fp32
-  float* y_out;                   // [rows, y_cols] or nullptr
-  int rows, cols, y_cols;
-};
-int sf_fetch_launch(const SfFetchArgs* a, int grid, cudaStream_t st);
 int sf_cast_transpose(const float* in, int ld_in, __nv_bfloat16* out, int ld_out,
                       __nv_bfloat16* outT, int ld_t, int rows, int cols, cudaStream_t st);
 // gather rows by index then cast/transposes (minibatch assembly on the device)

@@ -353,7 +353,6 @@ class DeviceWorker:
         self.tile_map = torch.from_numpy(lay.tile_map()).to(dev)
         self._plans: Dict[Tuple[int, int], object] = {}
         self._ordered: set = set()
-        self._fetch = None
         self._input_sets: Dict[Tuple[int, int], Dict[str, Any]] = {}
         self._bufs: Dict[Tuple[int, int], StepBuffers] = {}
         self._keep: List[object] = []
@@ -456,26 +455,6 @@ class DeviceWorker:
                        if self.use_dbuf else {}))
 
     # ------------------------------------------------------------------------------------------
-    # ---- zero-copy minibatch fetch (in-graph SM loads from the pinned host partition) ------------------------
-    FETCH_RING = 1024
-
-    def fetch_ctx(self) -> Dict[str, Any]:
-        """Schedule ring (pinned), fetch sequence counter / CTA counter / partition descriptor (device)."""
-        if self._fetch is None:
-            self._fetch = dict(sched=torch.zeros(self.FETCH_RING, dtype=torch.int64).pin_memory(),
-                               counter=torch.zeros(1, dtype=torch.int32, device=self.device),
-                               sync=torch.zeros(1, dtype=torch.int32, device=self.device),
-                               desc=torch.zeros(4, dtype=torch.int64, device=self.device))
-        return self._fetch
-
-    def set_fetch_partition(self, X: torch.Tensor, Y: Optional[torch.Tensor]) -> None:
-        """Point the fetch kernels at a (new) pinned host partition; captured graphs stay valid."""
-        ctx = self.fetch_ctx()
-        host = torch.tensor([X.data_ptr(), 0 if Y is None else Y.data_ptr(), X.shape[1], 0 if Y is None else Y.shape[1]], dtype=torch.int64)
-        with torch.cuda.stream(self.stream):
-            ctx["desc"].copy_(host)
-        self.stream.synchronize()
-
     def input_set(self, B: int, slot: int) -> Dict[str, Any]:
         from .plan_builder import use_mn_possible
 
@@ -493,25 +472,6 @@ class DeviceWorker:
                 y=None if lp.target_is_input or not lp.label_dim else torch.zeros(B, lp.label_dim, dtype=torch.float32, device=dev))
         return self._input_sets[key]
 
-    def fetch_args(self, B: int, slot: int) -> Dict[str, Any]:
-        """Argument dict of a fetch launch that fills input set ``slot``."""
-        ctx, ins = self.fetch_ctx(), self.input_set(B, slot)
-        return dict(desc=native.ptr(ctx["desc"]), sched=ctx["sched"].data_ptr(), ring_mask=self.FETCH_RING - 1,
-                    counter=native.ptr(ctx["counter"]), sync=native.ptr(ctx["sync"]), x_out=native.ptr(ins["x32"]), y_out=native.ptr(ins["y"]),
-                    rows=B, cols=self.plan.input_dim, y_cols=0 if ins["y"] is None else ins["y"].shape[1])
-
-    def fetch_plan(self, B: int, slot: int):
-        """Stand-alone (eager) plan that fetches + prepares input set ``slot``: the first minibatch of a driver call."""
-        from . import plan_builder
-
-        key = ("fetch", B, slot)
-        if key not in self._plans:
-            plan = self.C.Plan()
-            plan_builder.add_fetch_ops(plan, dict(args=self.fetch_args(B, slot), target=self.input_set(B, slot)), B, self.plan.input_dim)
-            self._plans[key] = plan
-            self._order_after_build()
-        return self._plans[key]
-
     def _order_after_build(self) -> None:
         """Plan building allocates (zero-fills) and uploads through torch's CURRENT stream; the worker's streams are
         non-blocking ones, so nothing orders those fills before the plan's first kernels unless we say so."""
@@ -519,11 +479,9 @@ class DeviceWorker:
         self.stream.wait_stream(cur)
         self.copy_stream.wait_stream(cur)
 
-    def build_plan(self, B: int, slot: int = 0, with_pull: bool = True, with_push: bool = True, fetch_slots: int = 0,
+    def build_plan(self, B: int, slot: int = 0, with_pull: bool = True, with_push: bool = True,
                    resident: Optional[Tuple[torch.Tensor, Optional[torch.Tensor]]] = None, staged: bool = False):
-        """Compile the training step for batch size ``B`` reading from staging-buffer set ``slot``.  With
-        ``fetch_slots`` = S > 0 the plan is a zero-copy one: it consumes input set ``slot`` and its graph fetches
-        the next minibatch into input set ``(slot + 1) % S``.
+        """Compile the training step for batch size ``B`` reading from staging-buffer set ``slot``.
 
         ``staged`` (implied by ``resident``): the step consumes input set ``slot`` and ``bufs.prep`` is the plan that
         prepares it - cast of the rows copied into ``bufs.x_stage``, or, with ``resident`` = (X, Y) device tensors, the
@@ -533,22 +491,13 @@ class DeviceWorker:
         from . import plan_builder
 
         staged = staged or resident is not None
-        key = (B, slot, with_pull, with_push, fetch_slots, staged, None if resident is None else resident[0].data_ptr())
+        key = (B, slot, with_pull, with_push, staged, None if resident is None else resident[0].data_ptr())
         if key not in self._plans and staged:
             ins = self.input_set(B, slot)
             built = plan_builder.build(self, B, train=True, with_pull=with_pull, with_push=with_push, inputs=ins)
             prep, idx = plan_builder.build_prep(self, B, ins, None if resident is None else dict(x=resident[0], y=resident[1]))
             self._plans[key] = built.plan
             self._bufs[key] = StepBuffers(built.x_stage, built.y_stage, built.loss_out, built.result, idx, prep)
-            self._keep.append(built.keep)
-            self.launches_per_step = len(built.plan)
-            self._last_names = list(built.plan.names())
-        if key not in self._plans and fetch_slots > 0:
-            built = plan_builder.build(self, B, train=True, with_pull=with_pull, with_push=with_push, inputs=self.input_set(B, slot),
-                                       fetch=dict(args=self.fetch_args(B, (slot + 1) % fetch_slots),
-                                                  target=self.input_set(B, (slot + 1) % fetch_slots)))
-            self._plans[key] = built.plan
-            self._bufs[key] = StepBuffers(built.x_stage, built.y_stage, built.loss_out, built.result)
             self._keep.append(built.keep)
             self.launches_per_step = len(built.plan)
             self._last_names = list(built.plan.names())

@@ -134,15 +134,6 @@ def use_mn_possible(train: bool) -> bool:
     return not train or os.environ.get("SPARKFLOW_WGRAD_MN", "1") == "1"
 
 
-def add_fetch_ops(plan, fetch: Dict[str, Any], B: int, D: int) -> None:
-    """fetch node (linear zero-copy stream of the minibatch into fp32 staging) + the cast / transpose that turns it into
-    the first layer's operands, both for the input set ``fetch['target']``."""
-    P = native.ptr
-    t = fetch["target"]
-    plan.add_fetch(fetch["args"], int(os.environ.get("SPARKFLOW_FETCH_CTAS", "8")))
-    plan.add_cast_transpose(P(t["x32"]), D, 0, P(t["a0"]), t["a0"].shape[1], P(t["a0T"]), 0 if t["a0T"] is None else t["a0T"].shape[1], B, D)
-
-
 def build_prep(worker, B: int, inputs: Dict[str, Any], resident: Optional[Dict[str, Any]] = None):
     """Plan that prepares input set ``inputs`` (see ``build``) for one training step, run before the step's graph on the
     stream that stages the minibatch.  DMA staging: cast (+ transpose) of the fp32 rows already copied into ``x32``.
@@ -169,15 +160,12 @@ def build_prep(worker, B: int, inputs: Dict[str, Any], resident: Optional[Dict[s
 
 
 def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = True, upto: Optional[int] = None,
-          post: Optional[str] = None, with_loss: bool = False, inputs: Optional[Dict[str, Any]] = None,
-          fetch: Optional[Dict[str, Any]] = None) -> BuiltPlan:
+          post: Optional[str] = None, with_loss: bool = False, inputs: Optional[Dict[str, Any]] = None) -> BuiltPlan:
     """``train``: full step (fwd + loss + bwd + push).  Otherwise forward up to dense index ``upto``
     (None = last) producing an fp32 result (+ArgMax), or forward + loss only when ``with_loss``.
 
     ``inputs``: dict(x32, a0, a0T, y) already holding this step's minibatch (fp32 rows, bf16 operands, labels) when the
-    graph starts - filled by ``build_prep``'s plan or by a fetch node - so the graph has no cast kernel and starts with
-    the pull; ``fetch``: dict(args, target) of the fetch node that fills the NEXT slot's input set from the pinned host
-    partition on a side branch of this graph."""
+    graph starts - filled by ``build_prep``'s plan - so the graph has no cast kernel and starts with the pull."""
     C, dev, lay, lp = worker.C, worker.device, worker.layout, worker.plan
     check_grammar(lp)
     P = native.ptr
@@ -247,12 +235,6 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     trainable = [i for i, l in enumerate(layers) if l.kind in ("dense", "conv")]
     first_trainable = trainable[0]
 
-    # ---------------- next step's minibatch: zero-copy fetch on its own branch for the whole step ----------------
-    if fetch is not None:
-        plan.fork(3)
-        plan.branch(3)
-        add_fetch_ops(plan, fetch, B, D)
-        plan.branch(0)
     # ---------------- pull || input cast ----------------
     # with `inputs` the operands are ready when the graph starts: the pull heads the main branch and the first GEMM
     # follows it over a programmatic edge (a join would be a full-completion edge).  The sharded snapshot pull keeps the
@@ -435,7 +417,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
 
     def side(fn):
         """run `fn` (which adds ops) on a wgrad branch: branches 2 and 1 alternate, so no wgrad queues behind the previous
-        one (branch 3 belongs to the fetch node)"""
+        one"""
         if branches:
             b = 2 - n_side[0] % 2
             n_side[0] += 1
@@ -564,8 +546,6 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         plan.add_post_flags(worker._post_flags_args(loss_out, phase=1))
     for b in (2, 1)[:n_side[0]]:
         plan.join(b)
-    if fetch is not None:
-        plan.join(3)
     if with_push:
         extra = dict(done_dev=P(done_dev)) if done_dev is not None else {}
         if sharded:

@@ -188,9 +188,6 @@ class B200Engine(Engine):
         self._driver = None
         self._driver_plans = {}
         self._driver_last = None
-        self._fetch_drivers = {}
-        self._fetch_partition_set = False
-        self.h2d_mode = os.environ.get("SPARKFLOW_H2D", "dma")
         self.partition_mode = os.environ.get("SPARKFLOW_PARTITION", "pinned")
         self.resident = False
         self.Xd = self.Yd = self.perm_d = None
@@ -222,8 +219,6 @@ class B200Engine(Engine):
                 self.perm_d = torch.arange(self.partition_rows, dtype=torch.int32, device=self.w.device)
             self.w.stream.synchronize()
             self._resident_driver = {}
-        if self._fetch_partition_set:
-            self.w.set_fetch_partition(self.X, self.Y)
 
     def _host_batch(self, rows: Rows, slot: int):
         if isinstance(rows, slice):
@@ -318,8 +313,6 @@ class B200Engine(Engine):
             return
         self.w.stream.synchronize()
         self.w.copy_stream.synchronize()
-        for drv in self._fetch_drivers.values():
-            drv.flush()
         from ..ops.native import host_ext
 
         H = host_ext()
@@ -332,20 +325,14 @@ class B200Engine(Engine):
         if self.Y is not None:
             H.gather_rows(self.Y.data_ptr(), self._Y2.data_ptr(), idx, self.Y.shape[1] * 4, 4)
             self.Y, self._Y2 = self._Y2, self.Y
-        if not self._fetch_drivers:
-            self._driver = None                 # DMA driver: host base pointers are baked into it
-            self._driver_plans = {}
-        if self._fetch_partition_set:
-            self.w.set_fetch_partition(self.X, self.Y)      # fetch-mode graphs read the partition through a device descriptor
+        self._driver = None                     # the DMA driver has the host base pointers baked into it
+        self._driver_plans = {}
 
     # ---- native inner loop -------------------------------------------------------------------------
     def train_contiguous(self, starts: Sequence[int], batch: int, pull: bool = True) -> None:
         """Run ``len(starts)`` steps on contiguous row blocks ``[s, s + batch)`` through the C++ StepDriver - no Python
-        in the loop.  ``SPARKFLOW_H2D=dma`` (default): copy-engine H2D of every minibatch on a side stream, SLOTS-deep,
-        event hand-off to the step graph.  ``SPARKFLOW_H2D=fetch``: every step's CUDA graph fetches the NEXT minibatch
-        from the pinned partition itself (zero-copy SM loads + cast on a side branch), so a step costs the host one
-        ``cudaGraphLaunch`` and nothing sits between two graphs.  Fetch takes the cast off the critical path, but SM
-        reads of cold host pages are slower than the DMA engine, which is why dma is the default."""
+        in the loop.  A pinned partition is fed by a copy-engine H2D of every minibatch on the copy stream, SLOTS-deep,
+        with an event hand-off to the step graph; an HBM-resident one by a device-side row-id copy and gather."""
         w = self.w
         if not w.use_graphs or len(starts) == 0:
             for s0 in starts:
@@ -354,9 +341,6 @@ class B200Engine(Engine):
         starts = [int(v) for v in starts]
         if self.resident:
             self._train_contiguous_resident(starts, batch, pull)
-            return
-        if self.h2d_mode == "fetch":
-            self._train_fetch(starts, batch, pull)
             return
         key = (batch, pull)
         drv_ids = self._driver_plans.get(key)
@@ -416,38 +400,6 @@ class B200Engine(Engine):
         n = len(starts)
         ids = np.asarray([(drv.steps() + k) % self.SLOTS for k in range(n)], dtype=np.int32)
         drv.run_resident(ids, np.asarray(starts, dtype=np.int64), self.perm_d.data_ptr())
-        self.d2h_bytes += n * 8
-        self._driver = drv
-        self._driver_last = (drv.steps() - 1) % self.LOSS_RING
-        self.step_idx += n
-
-    def _train_fetch(self, starts: List[int], batch: int, pull: bool) -> None:
-        w = self.w
-        key = (batch, pull)
-        drv = self._fetch_drivers.get(key)
-        if drv is None:
-            S = self.SLOTS
-            if not self._fetch_partition_set:
-                w.set_fetch_partition(self.X, self.Y)
-                self._fetch_partition_set = True
-            d = w.C.StepDriver(w.stream.cuda_stream, w.copy_stream.cuda_stream, self.X.data_ptr(), self.X.shape[1] * 4,
-                               0 if self.Y is None else self.Y.data_ptr(), 0 if self.Y is None else self.Y.shape[1] * 4,
-                               self.loss_ring.data_ptr(), self.LOSS_RING)
-            for slot in range(S):
-                plan, bufs = w.build_plan(batch, slot, with_pull=pull, fetch_slots=S)
-                if not plan.captured():
-                    plan.capture(w.stream.cuda_stream)
-                d.add_plan(plan, 0, 0, bufs.loss_out.data_ptr(), batch)
-            d.enable_fetch(w.fetch_ctx()["sched"].data_ptr(), w.FETCH_RING, [w.fetch_plan(batch, slot) for slot in range(S)])
-            drv = self._fetch_drivers[key] = d
-        self.w.stream.synchronize()       # python-path steps (if any) are done before the driver takes over the ring
-        for slot in range(self.SLOTS):
-            self._harvest(slot)
-        n = len(starts)
-        ids = np.asarray([(drv.steps() + k) % self.SLOTS for k in range(n)], dtype=np.int32)
-        drv.run_fetch(ids, np.asarray(starts, dtype=np.int64))
-        # every step's graph pulls one minibatch over PCIe (the first one of the call by a stand-alone fetch launch)
-        self.h2d_bytes += (n + 1) * batch * (self.X.shape[1] + (0 if self.Y is None else self.Y.shape[1])) * 4
         self.d2h_bytes += n * 8
         self._driver = drv
         self._driver_last = (drv.steps() - 1) % self.LOSS_RING

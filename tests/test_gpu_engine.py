@@ -212,20 +212,17 @@ def test_applier_batch_is_sequential_pushes(opt, max_batch):
     master.close()
 
 
-@pytest.mark.parametrize("mode", ["fetch", "dma", "resident"])
+@pytest.mark.parametrize("partition", ["pinned", "resident"])
 @pytest.mark.parametrize("served", [False, True])
-def test_train_contiguous_native_loop_tracks_oracle(mode, served, monkeypatch):
-    """the C++ StepDriver loop: zero-copy in-graph minibatch fetch (one cudaGraphLaunch per step) and the copy-engine
-    variant both walk the same minibatches as the oracle, before and after a physical shuffle of the pinned partition"""
-    if mode == "resident":
-        monkeypatch.setenv("SPARKFLOW_PARTITION", "resident")       # HBM-resident partition, device-side gather / shuffle
-    else:
-        monkeypatch.setenv("SPARKFLOW_H2D", mode)
+def test_train_contiguous_native_loop_tracks_oracle(partition, served, monkeypatch):
+    """the C++ StepDriver loop walks the same minibatches as the oracle, before and after a shuffle of the partition:
+    a pinned one (copy-engine H2D per step, physical shuffle) and an HBM-resident one (device-side gather / shuffle)"""
+    monkeypatch.setenv("SPARKFLOW_PARTITION", partition)
     spec = OptimizerSpec.from_tf_kwargs("adam", dict(learning_rate=0.001))
     ir, master, worker, w0, (tf_in, tf_lab, d, c, kind) = _setup("simple_dnn", spec, True, served=served, dbuf=served)
     X, Y = _data(640, d, c, kind)
     eng = B200Engine(worker)
-    assert eng.partition_mode == "resident" if mode == "resident" else eng.h2d_mode == mode
+    assert eng.partition_mode == partition
     eng.load_partition(X, Y)
     ps = ParameterServer(w0, spec, acquire_lock=True)
     ref = TorchEngine(ir, tf_in, tf_lab, LocalTransport(ps))

@@ -500,31 +500,6 @@ def test_maxpool_fwd_bwd(C):
     torch.testing.assert_close(db, dz.float().sum(0), rtol=1e-2, atol=1e-2)
 
 
-@pytest.mark.parametrize("rows,cols,ycols,B,start,ldpad", [(1000, 784, 10, 300, 37, 0), (500, 50, 3, 64, 436, 0), (256, 36, 1, 33, 0, 0),
-                                                           (400, 30, 2, 50, 11, 6)])
-def test_fetch_kernel_zero_copy_minibatch(C, rows, cols, ycols, B, start, ldpad):
-    """in-graph minibatch fetch: SM loads stream a minibatch (features + labels) from pinned host memory into staging"""
-    g = torch.Generator().manual_seed(1)
-    Xfull = torch.randn(rows, cols + ldpad, generator=g).pin_memory()
-    Yfull = torch.randn(rows, ycols + ldpad, generator=g).pin_memory()
-    x_out = torch.full((B, cols), 7.0, device="cuda")
-    y_out = torch.zeros(B, ycols, device="cuda")
-    sched = torch.zeros(8, dtype=torch.int64).pin_memory()
-    counter = torch.zeros(1, dtype=torch.int32, device="cuda")
-    sync = torch.zeros(1, dtype=torch.int32, device="cuda")
-    desc = torch.tensor([Xfull.data_ptr(), Yfull.data_ptr(), cols + ldpad, ycols + ldpad], dtype=torch.int64).cuda()
-    args = dict(desc=native.ptr(desc), sched=sched.data_ptr(), ring_mask=7, counter=native.ptr(counter), sync=native.ptr(sync),
-                x_out=native.ptr(x_out), y_out=native.ptr(y_out), rows=B, cols=cols, y_cols=ycols)
-    sched[0] = 5            # first fetch (sequence 0) reads entry 0 ...
-    sched[1] = start        # ... the second one entry 1
-    for _ in range(2):
-        C.fetch(args, 5, native.current_stream())
-    torch.cuda.synchronize()
-    assert int(counter.item()) == 2 and int(sync.item()) == 0
-    assert torch.equal(x_out.cpu(), Xfull[start:start + B, :cols])
-    assert torch.equal(y_out.cpu(), Yfull[start:start + B, :ycols])
-
-
 @pytest.mark.parametrize("n,h,w,cin,kh,kw,cout,act", [(5, 28, 28, 1, 5, 5, 32, "relu"), (3, 12, 12, 2, 3, 3, 16, "tanh"), (2, 9, 9, 3, 2, 2, 64, None)])
 def test_conv_first_fused_fwd_and_wgrad(C, n, h, w, cin, kh, kw, cout, act):
     """First conv + bias + activation + 2x2 max-pool as one direct kernel, and its fused weight / bias gradient, against

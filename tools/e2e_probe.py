@@ -30,12 +30,12 @@ step, ready, start, end = p.T
 gap = start[1:] - end[:-1]                 # compute stream idle between consecutive graphs (front-end view)
 h2d_late = ready[1:] - end[:-1]            # > 0: the step's H2D finished after the previous graph did
 dur = end - start
-out = dict(slots=eng.SLOTS, no_h2d=os.environ.get("SPARKFLOW_DRV_NO_H2D", "0"), steps=len(p),
+out = dict(slots=eng.SLOTS, steps=len(p),
            period_us=float(np.median(np.diff(end))), period_mean_us=float(np.mean(np.diff(end))),
            dur_us_median=float(np.median(dur)), dur_us_p90=float(np.percentile(dur, 90)), dur_us_max=float(dur.max()),
            gap_us_median=float(np.median(gap)), gap_us_p90=float(np.percentile(gap, 90)), gap_us_max=float(gap.max()),
            h2d_late_frac=float(np.mean(h2d_late > 0)), h2d_late_us_p90=float(np.percentile(h2d_late, 90)),
            first_rows=[[round(float(v), 1) for v in r] for r in np.c_[step, ready - start[0], start - start[0], end - start[0]][:20]])
 print(json.dumps(out))
-json.dump(out, open("bench_out/e2e_probe_%s_%s.json" % (eng.SLOTS, out["no_h2d"]), "w"))
+json.dump(out, open("bench_out/e2e_probe_%s.json" % eng.SLOTS, "w"))
 sess.close()

@@ -1,6 +1,5 @@
 """How much does a concurrent host->device transfer slow the step graph down?  Replays the captured simple_dnn step
-back to back while a side stream (a) idles, (b) runs copy-engine DMAs of one minibatch, (c) runs the zero-copy fetch
-kernel (SM loads from pinned host memory) of the same bytes."""
+back to back while a side stream (a) idles, (b) runs copy-engine DMAs of one minibatch."""
 import json
 import sys
 import time
@@ -10,11 +9,9 @@ import torch
 
 sys.path.insert(0, ".")
 from sparkflow_b200.models import zoo
-from sparkflow_b200.ops import native
 from sparkflow_b200.ops.optimizers import OptimizerSpec
 from sparkflow_b200.parallel.session import TrainingSession
 
-C = native.cuda_ext()
 B = 300
 spec = OptimizerSpec.from_tf_kwargs("adam", dict(learning_rate=0.001))
 sess = TrainingSession(zoo.build("simple_dnn"), "x:0", "y:0", spec, acquire_lock=False, engine="b200", seed=0, devices=[0]).open()
@@ -57,23 +54,16 @@ measure("alone", lambda i: None, 0)
 def dma(i):
     with torch.cuda.stream(side):
         dst[i % 4].copy_(host[i % 64], non_blocking=True)
-def zc(grid):
-    def f(i):
-        C.hostcopy(host[i % 64].data_ptr(), dst[i % 4].data_ptr(), nbytes, grid, side.cuda_stream)
-    return f
 measure("dma_h2d", dma, 600)
-for grid in (8, 32, 96):
-    measure("zero_copy_grid%d" % grid, zc(grid), 600)
 # side transfers alone (no step running)
-for name, fn in (("dma_alone", dma), ("zero_copy32_alone", zc(32)), ("zero_copy96_alone", zc(96)), ("zero_copy8_alone", zc(8))):
-    s0, s1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    s0.record(side)
-    for i in range(200):
-        fn(i)
-    s1.record(side)
-    torch.cuda.synchronize()
-    out[name] = dict(side_us_each=s0.elapsed_time(s1) * 1e3 / 200, GBs=nbytes / (s0.elapsed_time(s1) * 1e-3 / 200) / 1e9)
+s0, s1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+torch.cuda.synchronize()
+s0.record(side)
+for i in range(200):
+    dma(i)
+s1.record(side)
+torch.cuda.synchronize()
+out["dma_alone"] = dict(side_us_each=s0.elapsed_time(s1) * 1e3 / 200, GBs=nbytes / (s0.elapsed_time(s1) * 1e-3 / 200) / 1e9)
 assert torch.equal(dst[(199) % 4].cpu(), host[199 % 64])
 print(json.dumps(out, indent=1))
 json.dump(out, open("bench_out/h2d_interference.json", "w"), indent=1)

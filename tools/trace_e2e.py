@@ -47,7 +47,7 @@ if cur:
     steps.append(cur)
 # per-kernel view of one step in the middle of the run (CTA records grouped by kernel id)
 mid = steps[len(steps) // 2]
-names = {1: "gemm", 2: "cast/fetch", 3: "softmax", 4: "mse", 5: "argmax", 6: "push/post", 7: "pull"}
+names = {1: "gemm", 2: "cast", 3: "softmax", 4: "mse", 5: "argmax", 6: "push/post", 7: "pull"}
 per = {}
 for r in rec:
     t0, t1, t2, kid = int(r["t0"]), int(r["t1"]), int(r["t2"]), int(r["kid"])
