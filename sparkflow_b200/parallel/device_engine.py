@@ -496,6 +496,7 @@ class DeviceWorker:
             ins = self.input_set(B, slot)
             built = plan_builder.build(self, B, train=True, with_pull=with_pull, with_push=with_push, inputs=ins)
             prep, idx = plan_builder.build_prep(self, B, ins, None if resident is None else dict(x=resident[0], y=resident[1]))
+            self.last_debug = built.debug
             self._plans[key] = built.plan
             self._bufs[key] = StepBuffers(built.x_stage, built.y_stage, built.loss_out, built.result, idx, prep)
             self._keep.append(built.keep)

@@ -446,6 +446,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             else:
                 wd.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
             wg = C.Gemm(wd)
+            r["wgrad"] = wg
             emit(wg, f"wgrad{i}", on_side=wgrad_on_side(i))
             if i == first_trainable:
                 break
@@ -524,6 +525,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 cw.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
             wg = C.Gemm(cw)
             gemms.append(wg)
+            r["wgrad"] = wg
             if wgrad_on_side(i):
                 side(lambda wg=wg, i=i: plan.add_gemm(wg, f"wgrad{i}"))
             else:
