@@ -8,6 +8,7 @@ pytestmark = pytest.mark.gpu
 from sparkflow_b200.ops import native
 from sparkflow_b200.ops.layout import ParamLayout, round_up
 from sparkflow_b200.ops.optimizers import OPT_IDS, OptimizerSpec, apply_update, init_slots
+from push_helpers import OPTIMIZERS
 
 ACT = {None: 0, "relu": 1, "sigmoid": 2, "tanh": 3}
 
@@ -261,21 +262,7 @@ def _push_setup(C, spec, lock_mode=0):
     return args, keep
 
 
-@pytest.mark.parametrize("name,kw", [
-    ("gradient_descent", dict(learning_rate=0.1)),
-    ("momentum", dict(learning_rate=0.1, momentum=0.9)),
-    ("momentum", dict(learning_rate=0.1, momentum=0.9, use_nesterov=True)),
-    ("adam", dict(learning_rate=0.01, beta1=0.85, beta2=0.98, epsilon=1e-8)),
-    ("rmsprop", dict(learning_rate=0.05, decay=0.95, momentum=0.1, epsilon=1e-10)),
-    ("rmsprop", dict(learning_rate=0.05, decay=0.95, momentum=0.1, epsilon=1e-6, centered=True)),
-    ("adagrad", dict(learning_rate=0.1, initial_accumulator_value=0.1)),
-    ("adadelta", dict(learning_rate=1.0, rho=0.95, epsilon=1e-6)),
-    ("adagrad_da", dict(learning_rate=0.1, l1_regularization_strength=0.001, l2_regularization_strength=0.01)),
-    ("ftrl", dict(learning_rate=0.1, l1_regularization_strength=0.001, l2_regularization_strength=0.01)),
-    ("proximal_adagrad", dict(learning_rate=0.1, l1_regularization_strength=0.001, l2_regularization_strength=0.01)),
-    ("proximal_gradient_descent", dict(learning_rate=0.1, l1_regularization_strength=0.001,
-                                       l2_regularization_strength=0.01)),
-])
+@pytest.mark.parametrize("name,kw", OPTIMIZERS)
 @pytest.mark.parametrize("lock_mode", [0, 1])
 def test_push_matches_reference_optimizer(C, name, kw, lock_mode):
     spec = OptimizerSpec.from_tf_kwargs(name, kw)
