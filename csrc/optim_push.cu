@@ -11,7 +11,9 @@
 //        Lock mode: device writer-priority RW lock (mirror of sparkflow/RWLock.py semantics) held
 //        in the master's control block, taken by CTA 0 and released by the last CTA to finish.
 // pull  (reference: GET /parameters): copies the master's bf16 publish buffer (and optionally the
-//        fp32 params) into the local replica under the read side of the same lock.
+//        fp32 params) into the local replica under the read side of the same lock.  A locked worker-applied push
+//        also publishes into the pushing worker's replica, so its next pull copies nothing while no other push
+//        came in between (replica_is_current).
 //
 // All ten TF-1.x optimizers of tensorflow_async.py:19-30 are implemented as update functors.
 #include "sm90_ptx.cuh"
@@ -107,9 +109,28 @@ template <bool SYS> __device__ void rw_acquire_read(uint32_t* lock) {
 }
 template <bool SYS> __device__ void rw_release_read(uint32_t* lock) { lk_red_release<SYS>(lock, 0u - 1u); }
 
+// Does a locked pull's snapshot equal what the replica already holds?  `mine` is the SF_CTRL_VERSION value the worker's
+// own last push created (its push publishes into the replica too); `ver` receives the version read.
+// Seqlock-style read with the lock word as the sequence: the lock word first, then the version, both acquire.
+//  - Every writer bumps SF_CTRL_VERSION before its release of the write bit, and every later change of the lock word is
+//    an atomic RMW, so an acquire load of the lock word that reads any value coherence-after a writer's release
+//    synchronizes with it: the version load that follows sees that writer's bump.  A version equal to `mine` therefore
+//    means no push was applied after the worker's own one and before the lock word was read.
+//  - Only the writer that set bit 16 clears it, so a lock word without it (and without waiting writers) means no push
+//    was in progress when it was read.
+// Together: at the instant the lock word was read the publish buffer held exactly the worker's own last push, i.e. the
+// replica.  A writer that takes the lock after that instant is ordered after this pull, as it would be had the pull
+// taken the read lock first; a second read of the lock word after the version would only reject such writers.
+template <bool SYS> __device__ __forceinline__ bool replica_is_current(uint32_t* ctrl, uint32_t mine, uint32_t& ver) {
+  if ((lk_ld_acquire<SYS>(ctrl + SF_CTRL_LOCK) & ~kLockReaders) != 0u) return false;      // a writer holds or awaits the lock
+  ver = lk_ld_acquire<SYS>(ctrl + SF_CTRL_VERSION);
+  return ver == mine;
+}
+
 // ---- in-grid coordination on the worker's own memory --------------------------------------
 // local_sync words: 0 = grant epoch, 1 = granted value (optimizer step t), 2 = done counter,
-//                   3 = launch counter.  All CTAs of the grid must be co-resident (grid <= #SMs).
+//                   3 = launch counter, 5 = (push) the version the push creates when it publishes into the worker's
+//                   replica.  All CTAs of the grid must be co-resident (grid <= #SMs).
 __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -117,6 +138,21 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
 }
 __device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// The launch counter (word 3) of a locked push / pull is read RELAXED: the previous launch that wrote it completed before
+// this grid started, and this launch's last CTA rewrites it only after every CTA's release-ordered arrival on the done
+// counter.  A relaxed load does not hold back the lock / version round trip that follows it, so the two overlap.
+__device__ __forceinline__ uint32_t ld_launch_epoch(const uint32_t* local_sync) {
+  uint32_t v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(local_sync + 3) : "memory");
+  return v;
+}
+// Arrival on the done counter (word 2): release for this CTA's stores (bar.sync makes it cumulative over the CTA), acquire
+// for the last CTA, which then sees every CTA's stores without a second round trip.
+__device__ __forceinline__ uint32_t arrive_done(uint32_t* local_sync) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(old) : "l"(local_sync + 2) : "memory");
+  return old;
 }
 
 // ---- optimizer rules (TF 1.x training_ops semantics) ---------------------------------------
@@ -512,10 +548,11 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
   if (tid == 0) {
     uint32_t t;
     if (locked) {
-      const uint32_t epoch = ld_acquire_gpu(local_sync + 3);
+      const uint32_t epoch = ld_launch_epoch(local_sync);
       if (blockIdx.x == 0) {
         rw_acquire_write<SYS>(a.ctrl + SF_CTRL_LOCK);
         t = ld_relaxed_sys(a.ctrl + SF_CTRL_STEP) + 1;
+        if (a.replica_version != nullptr) local_sync[5] = ld_relaxed_sys(a.ctrl + SF_CTRL_VERSION) + 1;     // this push's version
         local_sync[1] = t;
         st_release_gpu(local_sync + 0, epoch + 1);
       } else {
@@ -539,11 +576,10 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
   // ---------------- completion ----------------
   __syncthreads();
   if (tid == 0) {
-    // lock mode: the release-add orders this CTA's stores (bar.sync is cumulative) before the lock release
-    // performed by the last CTA; Hogwild promises no ordering at all, so the counter is relaxed.
-    const uint32_t prev = locked ? lk_add_release<false>(local_sync + 2, 1u) : atomicAdd(local_sync + 2, 1u);
+    // lock mode: the arrival orders this CTA's stores before the lock release performed by the last CTA; Hogwild
+    // promises no ordering at all, so the counter is relaxed.
+    const uint32_t prev = locked ? arrive_done(local_sync) : atomicAdd(local_sync + 2, 1u);
     if (prev == gridDim.x - 1) {                  // last CTA of this push
-      if (locked) (void)ld_acquire_gpu(local_sync + 2);
       local_sync[2] = 0;
       publish_loss(a.loss_out, a.loss_acc, a.done_dev);
       if (a.drop) {
@@ -552,6 +588,8 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_STEP, 1u);
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_PUSHES, 1u);
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_VERSION, 1u);
+        // the pushing worker's replica holds this version; only its next pull, a later kernel, reads the word
+        if (a.replica_version != nullptr) *a.replica_version = local_sync[5];
       }
       if (locked) {
         rw_release_write<SYS>(a.ctrl + SF_CTRL_LOCK);
@@ -587,61 +625,67 @@ pull_kernel(const SfPullArgs a, uint32_t* local_sync) {
   }
   const bool dbuf = locked && a.dbuf != 0;
   __shared__ uint32_t s_cur;
+  constexpr uint32_t kElided = 2u;      // local_sync[1]: the replica is current, no lock is taken and nothing copied
+  uint32_t ver = 0;
   if (locked) {
     if (tid == 0) {
-      const uint32_t epoch = ld_acquire_gpu(local_sync + 3);
+      const uint32_t mine = (blockIdx.x == 0 && a.replica_version != nullptr) ? *a.replica_version : 0u;
+      const uint32_t epoch = ld_launch_epoch(local_sync);
       if (blockIdx.x == 0) {
         uint32_t cur = 0;
         if (dbuf) cur = atom_add_acqrel_sys(a.ctrl + SF_CTRL_PUB, 1u) >> 31;      // register + learn the complete buffer
+        else if (a.replica_version != nullptr && replica_is_current<SYS>(a.ctrl, mine, ver)) cur = kElided;
         else rw_acquire_read<SYS>(a.ctrl + SF_CTRL_LOCK);
         local_sync[1] = cur;
         st_release_gpu(local_sync + 0, epoch + 1);
+        s_cur = cur;
       } else {
         const unsigned long long t0 = gtime_ns();
         while (ld_acquire_gpu(local_sync + 0) != epoch + 1) {
           if (gtime_ns() - t0 > kLockTimeoutNs) sf_fail(0x404);
         }
+        s_cur = local_sync[1];
       }
       s_epoch = epoch;
-      s_cur = local_sync[1];
     }
     __syncthreads();
   }
   // successors may pre-launch only once the waits above are over: while this kernel spins on the applier or on a writer's
   // lock, their CTAs (one per SM at GEMM shared-memory sizes) would hold the SMs the kernel it waits for needs
   pdl_launch_dependents();
+  const bool elided = locked && s_cur == kElided;
   const uint32_t cur = dbuf ? s_cur : 0u;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t gid = static_cast<size_t>(blockIdx.x) * blockDim.x + tid;
-  {
-    const uint4* s = reinterpret_cast<const uint4*>(cur ? a.src_alt : a.src);
-    uint4* d = reinterpret_cast<uint4*>(a.dst);
-    const size_t n16 = a.n_bf16 / 8;
-    // 4 independent 16-byte loads in flight per thread to cover the ~2 us NVLink latency
-    size_t i = gid;
-    for (; i + 3 * stride < n16; i += 4 * stride) {
-      const uint4 v0 = ld_stream_u4(s + i), v1 = ld_stream_u4(s + i + stride),
-                  v2 = ld_stream_u4(s + i + 2 * stride), v3 = ld_stream_u4(s + i + 3 * stride);
-      d[i] = v0; d[i + stride] = v1; d[i + 2 * stride] = v2; d[i + 3 * stride] = v3;
+  if (!elided) {
+    {
+      const uint4* s = reinterpret_cast<const uint4*>(cur ? a.src_alt : a.src);
+      uint4* d = reinterpret_cast<uint4*>(a.dst);
+      const size_t n16 = a.n_bf16 / 8;
+      // 4 independent 16-byte loads in flight per thread to cover the ~2 us NVLink latency
+      size_t i = gid;
+      for (; i + 3 * stride < n16; i += 4 * stride) {
+        const uint4 v0 = ld_stream_u4(s + i), v1 = ld_stream_u4(s + i + stride),
+                    v2 = ld_stream_u4(s + i + 2 * stride), v3 = ld_stream_u4(s + i + 3 * stride);
+        d[i] = v0; d[i + stride] = v1; d[i + 2 * stride] = v2; d[i + 3 * stride] = v3;
+      }
+      for (; i < n16; i += stride) d[i] = ld_stream_u4(s + i);
     }
-    for (; i < n16; i += stride) d[i] = ld_stream_u4(s + i);
+    if (dbuf) {                        // 1-D variables: the fp32 copy that belongs to the same published version
+      const float* vp = a.vec_pub[cur];
+      for (size_t i = gid; i < a.n_f32; i += stride) a.dst_f32[i] = ld_relaxed_sys_f32(vp + i);
+    } else if (a.src_state != nullptr) {      // 1-D variables: gather .x of the interleaved master state
+      for (size_t i = gid; i < a.n_f32; i += stride) a.dst_f32[i] = ld_stream_f4(a.src_state + i).x;
+    }
   }
-  if (dbuf) {                        // 1-D variables: the fp32 copy that belongs to the same published version
-    const float* vp = a.vec_pub[cur];
-    for (size_t i = gid; i < a.n_f32; i += stride) a.dst_f32[i] = ld_relaxed_sys_f32(vp + i);
-  } else if (a.src_state != nullptr) {      // 1-D variables: gather .x of the interleaved master state
-    for (size_t i = gid; i < a.n_f32; i += stride) a.dst_f32[i] = ld_stream_f4(a.src_state + i).x;
-  }
-  if (gid == 0 && a.seen_version != nullptr) *a.seen_version = ld_relaxed_sys(a.ctrl + SF_CTRL_VERSION);
+  if (gid == 0 && a.seen_version != nullptr) *a.seen_version = elided ? ver : ld_relaxed_sys(a.ctrl + SF_CTRL_VERSION);
   if (locked) {
     __syncthreads();                 // every load of this CTA has returned (values were stored to the replica)
     if (tid == 0) {
-      const uint32_t prev = lk_add_release<false>(local_sync + 2, 1u);
-      if (prev == gridDim.x - 1) {
-        (void)ld_acquire_gpu(local_sync + 2);
+      if (arrive_done(local_sync) == gridDim.x - 1) {
         local_sync[2] = 0;
         if (dbuf) lk_red_release<SYS>(a.ctrl + SF_CTRL_PUB, 0u - 1u);
-        else rw_release_read<SYS>(a.ctrl + SF_CTRL_LOCK);
+        else if (!elided) rw_release_read<SYS>(a.ctrl + SF_CTRL_LOCK);
         st_release_gpu(local_sync + 3, s_epoch + 1);
       }
     }

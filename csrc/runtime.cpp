@@ -174,6 +174,9 @@ SfPushArgs parse_push(const py::dict& d) {
   a.scope_sys = getd<int>(d, "scope_sys", 1);
   a.grad_scale = getd<float>(d, "grad_scale", 1.0f);
   a.h = parse_hyper(getd<py::dict>(d, "hyper", py::dict()));
+  a.replica_version = P<uint32_t>(getd<uintptr_t>(d, "replica_version", 0));
+  if (a.replica_version && (a.lock_mode != SF_LOCK_RW || a.n_shadow_dst != 2 || a.shadow_is_mc))
+    throw std::runtime_error("push: replica_version needs lock mode and the replica as the second of two publish destinations");
   {
     auto rows = getd<std::vector<std::vector<int64_t>>>(d, "seg_rows", {});
     if (!rows.empty() && rows.size() <= SF_MAX_INLINE_SEGS) {
@@ -326,6 +329,9 @@ SfPullArgs parse_pull(const py::dict& d) {
   a.src_alt = P<const __nv_bfloat16>(getd<uintptr_t>(d, "src_alt", 0));
   a.vec_pub[0] = P<const float>(getd<uintptr_t>(d, "vec_pub0", 0));
   a.vec_pub[1] = P<const float>(getd<uintptr_t>(d, "vec_pub1", 0));
+  a.replica_version = P<const uint32_t>(getd<uintptr_t>(d, "replica_version", 0));
+  if (a.replica_version && (a.lock_mode != SF_LOCK_RW || a.dbuf || a.wait_applied))
+    throw std::runtime_error("pull: replica_version needs lock mode and a worker-applied push");
   if (a.dbuf && (!a.src_alt || (a.n_f32 && (!a.vec_pub[0] || !a.vec_pub[1])))) throw std::runtime_error("pull: dbuf needs src_alt and vec_pub0/1");
   if (a.wait_applied && !a.my_posted) throw std::runtime_error("pull: wait_applied needs my_posted");
   if (a.n_bf16 % 8) throw std::runtime_error("pull: bf16 size must be a 16-byte multiple");

@@ -244,6 +244,9 @@ struct SfPushArgs {
   int scope_sys;                  // 1: lock / counters use .sys scope (multi-GPU world); 0: .gpu (single GPU)
   float grad_scale;
   SfHyper h;
+  // lock mode, worker-applied push that also publishes into the pushing worker's replica (shadow_dst[1], vec_pub[0]):
+  // local word that receives the SF_CTRL_VERSION value this push creates, so the worker's next pull can skip its copy
+  uint32_t* replica_version;
 };
 
 // control block layout (uint32 words) living in master memory
@@ -282,6 +285,9 @@ struct SfPullArgs {
   int dbuf;
   const __nv_bfloat16* src_alt;   // publish buffer 1 (src is buffer 0)
   const float* vec_pub[2];        // fp32 copies of the 1-D variables, one per buffer
+  // lock mode: local word naming the version the replica (dst, dst_f32) already holds (SfPushArgs.replica_version).
+  // While no writer holds or waits for the lock and SF_CTRL_VERSION equals it, the pull takes no lock and copies nothing.
+  const uint32_t* replica_version;
 };
 int sf_pull_launch(const SfPullArgs* a, uint32_t* local_sync, int grid, cudaStream_t st);
 

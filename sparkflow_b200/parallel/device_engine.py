@@ -260,7 +260,9 @@ class DeviceWorker:
     def __init__(self, ir: GraphIR, tf_input: str, tf_label: Optional[str], spec: OptimizerSpec, master: MasterState,
                  acquire_lock: bool = False, pull_mode: Optional[str] = None, use_graphs: bool = True,
                  device: Optional[torch.device] = None, plan: Optional[LayerPlan] = None, shared: bool = True,
-                 worker_index: int = 0):
+                 worker_index: int = 0, reads_between_pulls: bool = False):
+        """``reads_between_pulls``: steps without a pull (several minibatches per pull) or a partition loss read this
+        worker's replica, and must see the weights of its last pull."""
         self.C = native.cuda_ext()
         self.ir = ir
         self.plan: LayerPlan = plan if plan is not None else compile_graph(ir, tf_input, tf_label, None, need_loss=True)
@@ -288,6 +290,11 @@ class DeviceWorker:
             self.pull_mode = "copy" if self.lock_mode else "inbox"     # lock: seqlock snapshot; Hogwild: GEMMs read the inbox in place
         if self.pull_mode == "direct" and self.lock_mode:
             self.pull_mode = "copy"            # a locked pull must be a private snapshot
+        # locked worker-applied push: it also publishes into this worker's replica, and the next pull skips its copy when
+        # no other push came in between.  Not when something reads the replica without pulling first: those reads must
+        # see the weights of the last pull, not of the last push.
+        self.own_publish = bool(self.lock_mode and not self.served and not self.sharded and self.pull_mode == "copy"
+                                and not reads_between_pulls)
         self.use_graphs = use_graphs and os.environ.get("SPARKFLOW_NO_GRAPHS") != "1"
         self.use_branches = os.environ.get("SPARKFLOW_NO_BRANCHES") != "1"
         self.fuse_loss = os.environ.get("SPARKFLOW_NO_FUSED_LOSS") != "1"
@@ -349,6 +356,8 @@ class DeviceWorker:
         self.sync_push = torch.zeros(8, dtype=torch.int32, device=dev)
         self.sync_pull = torch.zeros(8, dtype=torch.int32, device=dev)
         self.seen_version = torch.zeros(1, dtype=torch.int32, device=dev)
+        # version of the master's publish the replica holds (own_publish); -1: none yet, the first pull copies
+        self.replica_version = torch.full((1,), -1, dtype=torch.int32, device=dev)
         self.segs_dev = torch.frombuffer(bytearray(self.C.pack_segs(lay.seg_rows())), dtype=torch.uint8).to(dev)
         self.tile_map = torch.from_numpy(lay.tile_map()).to(dev)
         self._plans: Dict[Tuple[int, int], object] = {}
@@ -377,10 +386,16 @@ class DeviceWorker:
 
     def _push_args(self, loss_out: torch.Tensor, drop: int = 0) -> dict:
         m = self.master
-        return dict(state=native.ptr(m.state), ctrl=native.ptr(m.ctrl), shadow_dst=[native.ptr(m.shadow)], grad=native.ptr(self.grads),
+        args = dict(state=native.ptr(m.state), ctrl=native.ptr(m.ctrl), shadow_dst=[native.ptr(m.shadow)], grad=native.ptr(self.grads),
                     loss_acc=native.ptr(self.loss_acc), loss_out=native.ptr(loss_out), segs=native.ptr(self.segs_dev),
                     tile_map=native.ptr(self.tile_map), num_tiles=int(self.tile_map.shape[0]), seg_rows=self.layout.seg_rows(),
                     optimizer=self.spec.opt_id, lock_mode=self.lock_mode, drop=drop, scope_sys=self.scope_sys, grad_scale=1.0, hyper=self.spec.native_hyper())
+        if self.own_publish:
+            # the replica has the publish buffer's flat layout, vec_local the 1-D tail's (indexed from vec_offset)
+            args.update(shadow_dst=[native.ptr(m.shadow), native.ptr(self.replica)], replica_version=native.ptr(self.replica_version))
+            if self.layout.vec_count:
+                args.update(vec_pub=[native.ptr(self.vec_local)], vec_offset=self.layout.vec_offset)
+        return args
 
     def _post_args(self, loss_out: torch.Tensor, drop: int = 0) -> dict:
         m = self.master
@@ -451,6 +466,7 @@ class DeviceWorker:
                     scope_sys=self.scope_sys,
                     wait_applied=(m.flags_ptr(self.worker_index) + self.C.MB_APPLIED * 4) if self.served else 0,
                     my_posted=(native.ptr(self.sync_push) + 16) if self.served else 0,
+                    replica_version=native.ptr(self.replica_version) if self.own_publish else 0,
                     **(dict(dbuf=1, src_alt=native.ptr(m.shadow_alt), vec_pub0=native.ptr(m.vec_pub[0]), vec_pub1=native.ptr(m.vec_pub[1]))
                        if self.use_dbuf else {}))
 

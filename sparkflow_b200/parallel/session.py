@@ -272,7 +272,8 @@ class TrainingSession:
                 # mailbox index = position of the device in the session's device list (NOT its CUDA ordinal)
                 widx = self.ctx.rank if self.ctx.world > 1 else lane
                 w = DeviceWorker(self.ir, self.tf_input, self.tf_label, self.spec, master, acquire_lock=self.acquire_lock,
-                                 pull_mode=self.pull_mode, device=device, shared=shared, worker_index=widx)
+                                 pull_mode=self.pull_mode, device=device, shared=shared, worker_index=widx,
+                                 reads_between_pulls=self.msi > 1 or bool(self.verbose) or self.loss_callback is not None)
                 self._dev_workers[lane] = w
                 self._workers.append(w)
             return B200Engine(w)
