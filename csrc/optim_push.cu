@@ -130,7 +130,8 @@ template <bool SYS> __device__ __forceinline__ bool replica_is_current(uint32_t*
 // ---- in-grid coordination on the worker's own memory --------------------------------------
 // local_sync words: 0 = grant epoch, 1 = granted value (optimizer step t), 2 = done counter,
 //                   3 = launch counter, 5 = (push) the version the push creates when it publishes into the worker's
-//                   replica.  All CTAs of the grid must be co-resident (grid <= #SMs).
+//                   replica, 6 = (push) count of pushes whose early tuple loads were stale (push_grant).
+//                   All CTAs of the grid must be co-resident (grid <= #SMs).
 __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -153,6 +154,57 @@ __device__ __forceinline__ uint32_t arrive_done(uint32_t* local_sync) {
   uint32_t old;
   asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(old) : "l"(local_sync + 2) : "memory");
   return old;
+}
+
+// Locked push with a replica_version word: the grant and the first tile's master-tuple loads run BEFORE the
+// programmatic-dependency wait (under the predecessor's tail: the push pre-launches once the last weight-gradient GEMM
+// has passed its main loop); only the gradient, the loss words and what the tuples feed wait for it.  Block 0 reads
+// SF_CTRL_VERSION under the write lock; the early tuple loads are used when it equals the replica_version `mine` of the
+// worker's own last push, and reloaded after the wait otherwise (the first push, `mine` = -1; after another worker's push
+// or a host write of the master state).  Why a match means the early loads saw the current state:
+//  - The tuple loads are performed before the worker's previous push could still store: that push completed before this
+//    grid started (the same premise as ld_launch_epoch: kernels of a step plan let their successor launch only after
+//    their own wait, and steps are separate launches).  Every CTA's tuple loads are consumed before its release-ordered
+//    arrival on the done counter, and the last arrival precedes the lock release, so a writer that takes the lock after
+//    this push cannot affect them.
+//  - VERSION == mine, read under the write lock, means no push was applied between the worker's own last push and this
+//    acquire: every applied push (worker-applied or applier) bumps VERSION before it releases the write bit, and this
+//    acquire synchronizes with that release; a dropped push writes no state, and host writes of the master state bump
+//    VERSION themselves (MasterState.load_weights / load_slots).  A writer whose stores overlapped the early loads released
+//    the lock before this acquire, so its bump is seen and the tuples are reloaded.
+//  - No new deadlock: the lock is now held while the kernel waits for its predecessor, the last weight-gradient GEMM.
+//    By then the graph has completed every other dependency of the push, and that GEMM's CTAs are resident (one wave: it
+//    lets the push launch only after its main loop), so it completes without this push.  Without programmatic launch the
+//    wait returns at once and the order is the plain one.
+// The lock is held for at most the predecessor's remaining epilogue longer; the part of the push after the wait gets
+// shorter by about as much.
+template <bool SYS>
+__device__ __forceinline__ void push_grant(const SfPushArgs& a, uint32_t* local_sync, bool early, uint32_t* s_t, uint32_t* s_epoch,
+                                           uint32_t* s_valid) {
+  if (threadIdx.x == 0) {
+    const uint32_t mine = early ? *a.replica_version : 0u;
+    const uint32_t epoch = ld_launch_epoch(local_sync);
+    uint32_t t, ver = 0;
+    if (blockIdx.x == 0) {
+      rw_acquire_write<SYS>(a.ctrl + SF_CTRL_LOCK);
+      t = ld_relaxed_sys(a.ctrl + SF_CTRL_STEP) + 1;
+      if (early) local_sync[5] = ver = ld_relaxed_sys(a.ctrl + SF_CTRL_VERSION) + 1;     // this push's version
+      local_sync[1] = t;
+      st_release_gpu(local_sync + 0, epoch + 1);
+    } else {
+      const unsigned long long t0 = gtime_ns();
+      while (ld_acquire_gpu(local_sync + 0) != epoch + 1) {
+        if (early) __nanosleep(32);      // before the wait the poll shares the SM with the predecessor's epilogue
+        if (gtime_ns() - t0 > kLockTimeoutNs) sf_fail(0x403);
+      }
+      t = local_sync[1];
+      if (early) ver = local_sync[5];
+    }
+    *s_epoch = epoch;
+    *s_t = t;
+    *s_valid = early && ver - 1u == mine;
+  }
+  __syncthreads();
 }
 
 // ---- optimizer rules (TF 1.x training_ops semantics) ---------------------------------------
@@ -308,9 +360,39 @@ __device__ __forceinline__ void tile_load_grad(const float* grad, int64_t e, int
   }
 }
 
-// phase 1 of a tile: geometry + every load of the thread's half-rows (tuples and the first gradient), nothing consumed yet
+// the master-tuple loads of one half-row (geometry already in T)
+template <int HALVES>
+__device__ __forceinline__ void tile_load_state(const SfPushArgs& a, TileRegs<HALVES>& T, int half, int skip) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (!a.drop && j < T.nv[half] && !(skip & 4)) v = ld_weak_f4(reinterpret_cast<const float*>(a.state + T.e[half] + j));
+    T.u[half][j] = Upd{v.x, v.y, v.z, v.w};
+  }
+}
+// the first gradient's loads of one half-row
+template <int HALVES>
+__device__ __forceinline__ void tile_load_first_grad(float* grad0, TileRegs<HALVES>& T, int half, int skip) {
+  if (!(skip & 4)) tile_load_grad(grad0, T.e[half], T.nv[half], T.vec, T.g[half]);
+  else T.g[half][0] = T.g[half][1] = T.g[half][2] = T.g[half][3] = 0.f;
+}
+// ZERO: the gradient of one half-row is consumed: zero it for the next step's accumulating epilogues
 template <bool ZERO, int HALVES>
-__device__ __forceinline__ void push_tile_load(const SfPushArgs& a, float* grad0, int tile, TileRegs<HALVES>& T, int skip, bool dry) {
+__device__ __forceinline__ void tile_clear_grad(float* grad0, TileRegs<HALVES>& T, int half, bool dry) {
+  if (ZERO && T.nv[half] > 0 && !dry) {
+    if (T.vec) {
+      *reinterpret_cast<float4*>(grad0 + T.e[half]) = make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (j < T.nv[half]) grad0[T.e[half] + j] = 0.f;
+    }
+  }
+}
+
+// the tile's geometry: segment, origin and the thread's half-rows
+template <int HALVES>
+__device__ __forceinline__ void push_tile_geometry(const SfPushArgs& a, int tile, TileRegs<HALVES>& T) {
   const int tid = threadIdx.x;
   if (a.n_inline_segs > 0) {                         // tables live in constant (parameter) space
     int si = 0;
@@ -335,24 +417,36 @@ __device__ __forceinline__ void push_tile_load(const SfPushArgs& a, float* grad0
     const int r = T.r0 + ty + 16 * half;
     T.nv[half] = (r < sg.rows && T.c < sg.cols) ? ((sg.cols - T.c) >= 4 ? 4 : (sg.cols - T.c)) : 0;
     T.e[half] = sg.offset + static_cast<int64_t>(r) * sg.cols + T.c;
-    if (!(skip & 4)) tile_load_grad(grad0, T.e[half], T.nv[half], T.vec, T.g[half]);
-    else T.g[half][0] = T.g[half][1] = T.g[half][2] = T.g[half][3] = 0.f;
+  }
+}
+
+// phase 1a of a tile: geometry + the master-tuple loads.  Nothing here depends on the pushing step's results.
+template <int HALVES>
+__device__ __forceinline__ void push_tile_state(const SfPushArgs& a, int tile, TileRegs<HALVES>& T, int skip) {
+  push_tile_geometry(a, tile, T);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (!a.drop && j < T.nv[half] && !(skip & 4)) v = ld_weak_f4(reinterpret_cast<const float*>(a.state + T.e[half] + j));
-      T.u[half][j] = Upd{v.x, v.y, v.z, v.w};
-    }
-    if (ZERO && T.nv[half] > 0 && !dry) {
-      // the gradient is consumed: zero it for the next step's accumulating epilogues
-      if (T.vec) {
-        *reinterpret_cast<float4*>(grad0 + T.e[half]) = make_float4(0.f, 0.f, 0.f, 0.f);
-      } else {
+  for (int half = 0; half < HALVES; ++half) tile_load_state(a, T, half, skip);
+}
+
+// phase 1b of a tile: the first gradient's loads and (ZERO) its clear
+template <bool ZERO, int HALVES>
+__device__ __forceinline__ void push_tile_grad(float* grad0, TileRegs<HALVES>& T, int skip, bool dry) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (j < T.nv[half]) grad0[T.e[half] + j] = 0.f;
-      }
-    }
+  for (int half = 0; half < HALVES; ++half) {
+    tile_load_first_grad(grad0, T, half, skip);
+    tile_clear_grad<ZERO>(grad0, T, half, dry);
+  }
+}
+
+// phase 1 of a tile: geometry + every load of the thread's half-rows (tuples and the first gradient), nothing consumed yet
+template <bool ZERO, int HALVES>
+__device__ __forceinline__ void push_tile_load(const SfPushArgs& a, float* grad0, int tile, TileRegs<HALVES>& T, int skip, bool dry) {
+  push_tile_geometry(a, tile, T);
+#pragma unroll
+  for (int half = 0; half < HALVES; ++half) {
+    tile_load_first_grad(grad0, T, half, skip);
+    tile_load_state(a, T, half, skip);
+    tile_clear_grad<ZERO>(grad0, T, half, dry);
   }
 }
 
@@ -527,75 +621,110 @@ __device__ __forceinline__ void publish_loss(float* loss_out, float* loss_acc, u
   }
   signal_done(loss_out, done_dev);
 }
+// publish_loss with the loss (*loss_acc) and the count (*done_dev) loaded ahead by the caller
+__device__ __forceinline__ void publish_loaded_loss(float* loss_out, float* loss_acc, unsigned int* done_dev, float l, unsigned int done) {
+  if (loss_acc != nullptr) *loss_acc = 0.f;
+  if (done_dev == nullptr) {
+    if (loss_acc != nullptr) *loss_out = l;
+    return;
+  }
+  const unsigned int v = done + 1;
+  *done_dev = v;
+  if (loss_acc != nullptr) {
+    const unsigned long long w = static_cast<unsigned long long>(__float_as_uint(l)) | (static_cast<unsigned long long>(v) << 32);
+    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(loss_out), "l"(w) : "memory");
+    return;
+  }
+  asm volatile("fence.acq_rel.sys;" ::: "memory");
+  st_release_sys(reinterpret_cast<uint32_t*>(loss_out) + 1, v);
+}
 
 template <int OPT, bool SYS>
 __global__ void __launch_bounds__(kPushThreads, 2)
 push_kernel(const SfPushArgs a, uint32_t* local_sync) {
   __shared__ uint32_t s_t;
   __shared__ uint32_t s_epoch;
+  __shared__ uint32_t s_valid;
+  __shared__ unsigned long long s_ph[3];      // trace: phase stamps of block 0's first tile
   __shared__ __align__(16) __nv_bfloat16 s_tr[kTileC][kTileR + 8];
   TraceScope trace;
   pdl_launch_dependents();
   const int tid = threadIdx.x;
   const bool locked = a.lock_mode == SF_LOCK_RW;
+  const bool early = a.replica_version != nullptr;      // lock mode (runtime.cpp): see push_grant
+  const int skip = a.dbg_skip;
+  TileRegs<2> T;
+  unsigned long long t_grant = 0ull, t_grad = 0ull;
   // Hogwild reads the global step count racily; it does not depend on this step's kernels, so the
   // round trip to the master overlaps the predecessor's tail (before the programmatic-dependency wait).
   if (!locked && tid == 0) s_t = ld_relaxed_sys(a.ctrl + SF_CTRL_STEP) + 1;
+  if (early) {
+    if (static_cast<int>(blockIdx.x) < a.num_tiles) push_tile_state(a, blockIdx.x, T, skip);      // in flight during the grant
+    push_grant<SYS>(a, local_sync, true, &s_t, &s_epoch, &s_valid);
+    if (trace.on) t_grant = gtime_ns();
+  }
   pdl_wait();
   trace.mark();
+  float loss = 0.f;
+  unsigned int done = 0;
+  if (early && tid == 0) {         // any CTA may be the last: each loads the two words the last one publishes
+    if (a.loss_acc != nullptr) loss = *a.loss_acc;
+    if (a.done_dev != nullptr) done = *a.done_dev;
+  }
 
   // ---------------- acquire / step number ----------------
-  if (tid == 0) {
-    uint32_t t;
-    if (locked) {
-      const uint32_t epoch = ld_launch_epoch(local_sync);
-      if (blockIdx.x == 0) {
-        rw_acquire_write<SYS>(a.ctrl + SF_CTRL_LOCK);
-        t = ld_relaxed_sys(a.ctrl + SF_CTRL_STEP) + 1;
-        if (a.replica_version != nullptr) local_sync[5] = ld_relaxed_sys(a.ctrl + SF_CTRL_VERSION) + 1;     // this push's version
-        local_sync[1] = t;
-        st_release_gpu(local_sync + 0, epoch + 1);
-      } else {
-        const unsigned long long t0 = gtime_ns();
-        while (ld_acquire_gpu(local_sync + 0) != epoch + 1) {
-          if (gtime_ns() - t0 > kLockTimeoutNs) sf_fail(0x403);
-        }
-        t = local_sync[1];
-      }
-      s_epoch = epoch;
-      s_t = t;
-    }
+  if (locked && !early) {
+    push_grant<SYS>(a, local_sync, false, &s_t, &s_epoch, &s_valid);
+    if (trace.on) t_grant = gtime_ns();
   }
-  if (locked) __syncthreads();      // Hogwild: nothing to wait for, loads below start immediately
 
   // ---------------- tiles ----------------
   float* const grads[1] = {a.grad};
-  for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x)
-    push_tile<OPT, true>(a, grads, 1, tile, &s_t, !locked && tile == static_cast<int>(blockIdx.x), s_tr, a.shadow_dst[0], a.vec_pub[0]);
+  for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+    const bool first = tile == static_cast<int>(blockIdx.x);
+    const bool lead = trace.on && blockIdx.x == 0 && first;
+    if (!early || !first) {
+      push_tile_load<true>(a, a.grad, tile, T, skip, false);
+    } else {
+      if (!s_valid)      // the early loads may predate another writer's push: reload
+#pragma unroll
+        for (int half = 0; half < 2; ++half) tile_load_state(a, T, half, skip);
+      push_tile_grad<true>(a.grad, T, skip, false);
+    }
+    if (lead) t_grad = gtime_ns() + static_cast<unsigned long long>(T.g[0][0] == 12345.678f);      // gradient loads returned
+    push_tile_apply<OPT, true, 2>(a, grads, 1, T, &s_t, !locked && first, s_tr, a.shadow_dst[0], a.vec_pub[0], lead ? s_ph : nullptr,
+                                  0, 0, skip, false);
+  }
 
   // ---------------- completion ----------------
   __syncthreads();
   if (tid == 0) {
+    const unsigned long long t_st = trace.on ? gtime_ns() : 0ull;
     // lock mode: the arrival orders this CTA's stores before the lock release performed by the last CTA; Hogwild
     // promises no ordering at all, so the counter is relaxed.
     const uint32_t prev = locked ? arrive_done(local_sync) : atomicAdd(local_sync + 2, 1u);
     if (prev == gridDim.x - 1) {                  // last CTA of this push
+      const unsigned long long t_arr = trace.on ? gtime_ns() : 0ull;
       local_sync[2] = 0;
-      publish_loss(a.loss_out, a.loss_acc, a.done_dev);
+      if (early) publish_loaded_loss(a.loss_out, a.loss_acc, a.done_dev, loss, done);
+      else publish_loss(a.loss_out, a.loss_acc, a.done_dev);
       if (a.drop) {
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_DROPPED, 1u);
       } else {
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_STEP, 1u);
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_PUSHES, 1u);
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_VERSION, 1u);
-        // the pushing worker's replica holds this version; only its next pull, a later kernel, reads the word
-        if (a.replica_version != nullptr) *a.replica_version = local_sync[5];
+        // the pushing worker's replica holds this version; only its next pull or push, a later kernel, reads the word
+        if (early) *a.replica_version = local_sync[5];
+        if (early && !s_valid) local_sync[6] += 1u;      // pushes that reloaded their tuples after the wait
       }
       if (locked) {
         rw_release_write<SYS>(a.ctrl + SF_CTRL_LOCK);
         st_release_gpu(local_sync + 3, s_epoch + 1);
       }
+      trace.phases(KID_PUSH_TAIL, t_st, t_arr, gtime_ns());
     }
+    if (blockIdx.x == 0) trace.phases(KID_PUSH_LEAD, t_grant, t_grad, s_ph[1]);
   }
   trace.end(KID_PUSH);
 }

@@ -45,7 +45,10 @@ __device__ unsigned int g_trace_n = 0;
 
 enum KernelId { KID_GEMM = 1, KID_CAST = 2, KID_SOFTMAX = 3, KID_MSE = 4, KID_ARGMAX = 5, KID_PUSH = 6, KID_PULL = 7,
                 KID_IM2COL = 8, KID_COL2IM = 9, KID_POOL_FWD = 10, KID_POOL_BWD = 11, KID_POOL_GEN_FWD = 12, KID_POOL_GEN_BWD = 13,
-                KID_ACT_BWD = 14 };
+                KID_ACT_BWD = 14,
+                // phase stamps (ids 100 and up): one extra record of three stamps in t0 / t1 / t2
+                KID_PUSH_LEAD = 106,      // push, block 0: grant seen, gradient loads returned, optimizer math done
+                KID_PUSH_TAIL = 107 };    // push, last CTA: stores issued, done-counter arrival returned, tail done
 
 __device__ __forceinline__ unsigned long long trace_now() {
   unsigned long long t;
@@ -71,6 +74,13 @@ struct TraceScope {
         const unsigned int b = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
         g_trace_buf[i] = TraceRec{t0, t1, trace_now(), kid, b};
       }
+    }
+  }
+  // one phase-stamp record (kid >= 100) written by the thread that holds the scope
+  __device__ __forceinline__ void phases(unsigned int kid, unsigned long long a, unsigned long long b, unsigned long long c) {
+    if (on) {
+      const unsigned int i = atomicAdd(&g_trace_n, 1u);
+      if (i < g_trace_cap) g_trace_buf[i] = TraceRec{a, b, c, kid, blockIdx.x};
     }
   }
 };

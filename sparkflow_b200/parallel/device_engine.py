@@ -209,7 +209,10 @@ class MasterState:
         for i in range(self.spec.num_slots):
             host[:, 1 + i] = self.spec.slot_init(i)
         self.state.copy_(host)
+        version = self.ctrl[1:2].clone()
         self.ctrl.zero_()
+        self.ctrl[1:2] = version
+        self._advance_version()
         pub = torch.from_numpy(self.layout.publish_reference(flat)).to(torch.bfloat16)
         self.shadow.copy_(pub)
         if self.ml.n_mailboxes > 0:
@@ -229,7 +232,15 @@ class MasterState:
             self.state[:, 1 + i].copy_(torch.from_numpy(self.layout.flatten(per_var)))
         self.ctrl[2] = int(step)
         self.ctrl[3] = int(step)
+        self._advance_version()
         _sync_current(self.device)
+
+    def _advance_version(self) -> None:
+        """A host write of the master state moves SF_CTRL_VERSION on, and never back: a worker whose replica_version
+        equals it trusts what it read at its own last push (the locked push's early tuple loads, the locked pull's
+        skipped copy).  While it is 0 no push has been applied, so no worker holds a matching version and it stays 0."""
+        v = self.ctrl[1:2]
+        v.add_((v != 0).to(v.dtype))
 
     def counters(self) -> Dict[str, int]:
         c = self.ctrl.cpu().numpy()

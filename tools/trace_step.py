@@ -97,9 +97,17 @@ for s in summ:
 pushes = [s["end"] for s in summ if s["kid"] == 6]
 if len(pushes) > 1:
     print("step period (push end to push end, us):", ["%.2f" % (b - a) for a, b in zip(pushes, pushes[1:])])
+PUSH_PHASES = (106, 107)
+print("--- push phases, us from the push's ready: 106 = block 0 [grant seen, gradient loads returned, optimizer math done]; "
+      "107 = last CTA [stores issued, done-counter arrival returned, tail done]")
+for s in summ:
+    if s["kid"] == 6:
+        recs = [r for r in rows if r["kid"] in PUSH_PHASES and s["start"] <= r["t0"] <= s["end"]]
+        print("push ready %9.2f, end %+6.2f: " % (s["ready"], s["end"] - s["ready"])
+              + "  ".join("%d [%s]" % (r["kid"], ", ".join("%+6.2f" % (r[k] - s["ready"]) for k in ("t0", "t1", "t2"))) for r in recs))
 print("--- gemm phases (block 0 of each gemm): 101 = MMA thread [role start, first operands, last MMA issued]; 102 = epilogue [wait start, acc ready, done]; 103 = [chunk 0 in registers, alpha+bias, activation]; 104 = [dropout, loss head, act'(aux)]; 105 = [padding+colsum, fp32 out, bf16 out]")
 for r in rows:
-    if r["kid"] >= 100 and r["block"] == 0:
+    if r["kid"] >= 100 and r["block"] == 0 and r["kid"] not in PUSH_PHASES:
         print(r)
 os.makedirs(out_dir, exist_ok=True)
 json.dump(dict(summary=summ, rows=rows, plan=list(plan.names())),
