@@ -362,24 +362,18 @@ __device__ __forceinline__ void tile_load_grad(const float* grad, int64_t e, int
 
 // the master-tuple loads of one half-row (geometry already in T)
 template <int HALVES>
-__device__ __forceinline__ void tile_load_state(const SfPushArgs& a, TileRegs<HALVES>& T, int half, int skip) {
+__device__ __forceinline__ void tile_load_state(const SfPushArgs& a, TileRegs<HALVES>& T, int half) {
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!a.drop && j < T.nv[half] && !(skip & 4)) v = ld_weak_f4(reinterpret_cast<const float*>(a.state + T.e[half] + j));
+    if (!a.drop && j < T.nv[half]) v = ld_weak_f4(reinterpret_cast<const float*>(a.state + T.e[half] + j));
     T.u[half][j] = Upd{v.x, v.y, v.z, v.w};
   }
 }
-// the first gradient's loads of one half-row
-template <int HALVES>
-__device__ __forceinline__ void tile_load_first_grad(float* grad0, TileRegs<HALVES>& T, int half, int skip) {
-  if (!(skip & 4)) tile_load_grad(grad0, T.e[half], T.nv[half], T.vec, T.g[half]);
-  else T.g[half][0] = T.g[half][1] = T.g[half][2] = T.g[half][3] = 0.f;
-}
 // ZERO: the gradient of one half-row is consumed: zero it for the next step's accumulating epilogues
 template <bool ZERO, int HALVES>
-__device__ __forceinline__ void tile_clear_grad(float* grad0, TileRegs<HALVES>& T, int half, bool dry) {
-  if (ZERO && T.nv[half] > 0 && !dry) {
+__device__ __forceinline__ void tile_clear_grad(float* grad0, TileRegs<HALVES>& T, int half) {
+  if (ZERO && T.nv[half] > 0) {
     if (T.vec) {
       *reinterpret_cast<float4*>(grad0 + T.e[half]) = make_float4(0.f, 0.f, 0.f, 0.f);
     } else {
@@ -422,31 +416,31 @@ __device__ __forceinline__ void push_tile_geometry(const SfPushArgs& a, int tile
 
 // phase 1a of a tile: geometry + the master-tuple loads.  Nothing here depends on the pushing step's results.
 template <int HALVES>
-__device__ __forceinline__ void push_tile_state(const SfPushArgs& a, int tile, TileRegs<HALVES>& T, int skip) {
+__device__ __forceinline__ void push_tile_state(const SfPushArgs& a, int tile, TileRegs<HALVES>& T) {
   push_tile_geometry(a, tile, T);
 #pragma unroll
-  for (int half = 0; half < HALVES; ++half) tile_load_state(a, T, half, skip);
+  for (int half = 0; half < HALVES; ++half) tile_load_state(a, T, half);
 }
 
 // phase 1b of a tile: the first gradient's loads and (ZERO) its clear
 template <bool ZERO, int HALVES>
-__device__ __forceinline__ void push_tile_grad(float* grad0, TileRegs<HALVES>& T, int skip, bool dry) {
+__device__ __forceinline__ void push_tile_grad(float* grad0, TileRegs<HALVES>& T) {
 #pragma unroll
   for (int half = 0; half < HALVES; ++half) {
-    tile_load_first_grad(grad0, T, half, skip);
-    tile_clear_grad<ZERO>(grad0, T, half, dry);
+    tile_load_grad(grad0, T.e[half], T.nv[half], T.vec, T.g[half]);
+    tile_clear_grad<ZERO>(grad0, T, half);
   }
 }
 
 // phase 1 of a tile: geometry + every load of the thread's half-rows (tuples and the first gradient), nothing consumed yet
 template <bool ZERO, int HALVES>
-__device__ __forceinline__ void push_tile_load(const SfPushArgs& a, float* grad0, int tile, TileRegs<HALVES>& T, int skip, bool dry) {
+__device__ __forceinline__ void push_tile_load(const SfPushArgs& a, float* grad0, int tile, TileRegs<HALVES>& T) {
   push_tile_geometry(a, tile, T);
 #pragma unroll
   for (int half = 0; half < HALVES; ++half) {
-    tile_load_first_grad(grad0, T, half, skip);
-    tile_load_state(a, T, half, skip);
-    tile_clear_grad<ZERO>(grad0, T, half, dry);
+    tile_load_grad(grad0, T.e[half], T.nv[half], T.vec, T.g[half]);
+    tile_load_state(a, T, half);
+    tile_clear_grad<ZERO>(grad0, T, half);
   }
 }
 
@@ -455,7 +449,7 @@ template <int OPT, bool ZERO, int HALVES>
 __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* const* grads, int n_grads, TileRegs<HALVES>& T,
                                                 const uint32_t* s_t_ptr, bool sync_for_t, __nv_bfloat16 (*s_tr)[kTileR + 8],
                                                 __nv_bfloat16* pub0, float* vec0, unsigned long long* tp, long long off_bf16,
-                                                long long off_f32, int skip, bool dry) {
+                                                long long off_f32) {
   constexpr int NS = Slots<OPT>::n;
   const int tid = threadIdx.x;
   const bool mc = a.shadow_is_mc != 0;
@@ -469,7 +463,7 @@ __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* cons
   if (!a.drop) {
     for (int k = 0; k < n_grads; ++k) {
       float gn[HALVES][4];
-      if (k + 1 < n_grads && !(skip & 4)) {
+      if (k + 1 < n_grads) {
 #pragma unroll
         for (int half = 0; half < HALVES; ++half) tile_load_grad(grads[k + 1], T.e[half], T.nv[half], T.vec, gn[half]);
       }
@@ -491,7 +485,7 @@ __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* cons
       }
     }
   }
-  if (a.mb_zero && !dry) {
+  if (a.mb_zero) {
     // accumulating wgrad epilogues (split-K conv) add into the mailbox: hand it back zeroed
     for (int k = 0; k < n_grads; ++k)
 #pragma unroll
@@ -520,9 +514,8 @@ __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* cons
           const Upd& q = T.u[half][j];
           w[j] = q.p;
           float* dst = reinterpret_cast<float*>(a.state + T.e[half] + j);
-          if (!(skip & 2)) st_weak_f4(dst, q.p, NS >= 1 ? q.s0 : 0.f, NS >= 2 ? q.s1 : 0.f, NS >= 3 ? q.s2 : 0.f);
-          if (skip & 1) {
-          } else if (a.n_vec_dst > 0) {                               // sharded master: every replica's fp32 tail
+          st_weak_f4(dst, q.p, NS >= 1 ? q.s0 : 0.f, NS >= 2 ? q.s1 : 0.f, NS >= 3 ? q.s2 : 0.f);
+          if (a.n_vec_dst > 0) {                                      // sharded master: every replica's fp32 tail
             if (T.e[half] + j >= a.vec_offset) {
               const long long vi = T.e[half] + j - a.vec_offset;
               for (int d = 0; d < a.n_vec_dst; ++d) st_vec_f32(a.vec_dst[d] + off_f32 + vi, q.p, mc);
@@ -535,7 +528,7 @@ __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* cons
         }
       }
       // row-major bf16 publish: [rows, w_ld]; w_ld is a multiple of 8 and c of 4, pads carry zeros
-      if (sg.w_off >= 0 && !(skip & 1)) {
+      if (sg.w_off >= 0) {
         const int64_t wo = sg.w_off + static_cast<int64_t>(r) * sg.w_ld + c;
         const uint2 q = make_uint2(pack_bf16x2(w[0], w[1]), pack_bf16x2(w[2], w[3]));
         for (int d = 0; d < a.n_shadow_dst; ++d) st_shadow8((d == 0 ? pub0 : a.shadow_dst[d] + off_bf16) + wo, q, mc && d == 0);
@@ -552,7 +545,7 @@ __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* cons
     // transposed bf16 publish: [cols, wt_ld]; each thread owns 8 consecutive rows of one column
     const int cl = tid >> 2, part = tid & 3;
     const int cc = c0 + cl, rr = r0 + part * 8;
-    if (cl < kTileC && cc < sg.cols && rr < sg.rows && !(skip & 1)) {
+    if (cl < kTileC && cc < sg.cols && rr < sg.rows) {
       const int64_t to = sg.wt_off + static_cast<int64_t>(cc) * sg.wt_ld + rr;
       const uint4 q = *reinterpret_cast<const uint4*>(&s_tr[cl][part * 8]);
       for (int d = 0; d < a.n_shadow_dst; ++d) st_shadow16((d == 0 ? pub0 : a.shadow_dst[d] + off_bf16) + to, q, mc && d == 0);
@@ -561,68 +554,30 @@ __device__ __forceinline__ void push_tile_apply(const SfPushArgs& a, float* cons
   }
 }
 
-template <int OPT, bool ZERO, int HALVES = 2>
-__device__ __forceinline__ void push_tile(const SfPushArgs& a, float* const* grads, int n_grads, int tile,
-                                          const uint32_t* s_t_ptr, bool sync_for_t, __nv_bfloat16 (*s_tr)[kTileR + 8],
-                                          __nv_bfloat16* pub0, float* vec0, unsigned long long* tp = nullptr,
-                                          long long off_bf16 = 0, long long off_f32 = 0, bool dry = false) {
-  // dry: execute the whole instruction stream without touching memory (keeps the code resident in the SM's instruction cache)
-  const int skip = dry ? 7 : a.dbg_skip;
-  TileRegs<HALVES> T;
-  push_tile_load<ZERO, HALVES>(a, grads[0], tile, T, skip, dry);
-  if (tp != nullptr) tp[0] = gtime_ns();      // loads issued
-  push_tile_apply<OPT, ZERO, HALVES>(a, grads, n_grads, T, s_t_ptr, sync_for_t, s_tr, pub0, vec0, tp, off_bf16, off_f32, skip, dry);
-}
-
 // A run of tiles on one CTA with the NEXT tile's loads in flight while the current one is applied (the applier of a big
-// shard: ~60 tiles per CTA; without this every tile pays a full HBM round trip with nothing else outstanding).
+// shard: ~60 tiles per CTA; without this every tile pays a full HBM round trip with nothing else outstanding).  With at
+// most one tile per CTA it is the plain sequence: load the tile, apply it.
 template <int OPT, int HALVES>
 __device__ __forceinline__ void push_tiles_pipelined(const SfPushArgs& a, float* const* grads, int n_grads, int tile, int tile_hi, int stride,
                                                      const uint32_t* s_t_ptr, __nv_bfloat16 (*s_tr)[kTileR + 8], __nv_bfloat16* pub0,
                                                      float* vec0, unsigned long long* tp, long long off_bf16, long long off_f32) {
-  const int skip = a.dbg_skip;
   TileRegs<HALVES> cur, nxt;
   if (tile >= tile_hi) return;
-  push_tile_load<false, HALVES>(a, grads[0], tile, cur, skip, false);
+  push_tile_load<false, HALVES>(a, grads[0], tile, cur);
   for (; tile < tile_hi; tile += stride) {
     const bool more = tile + stride < tile_hi;
-    if (more) push_tile_load<false, HALVES>(a, grads[0], tile + stride, nxt, skip, false);
-    if (tp != nullptr) tp[0] = gtime_ns();
-    push_tile_apply<OPT, false, HALVES>(a, grads, n_grads, cur, s_t_ptr, false, s_tr, pub0, vec0, tp, off_bf16, off_f32, skip, false);
+    if (more) push_tile_load<false, HALVES>(a, grads[0], tile + stride, nxt);
+    if (tp != nullptr) tp[0] = gtime_ns();      // loads issued
+    push_tile_apply<OPT, false, HALVES>(a, grads, n_grads, cur, s_t_ptr, false, s_tr, pub0, vec0, tp, off_bf16, off_f32);
     if (more) cur = nxt;
   }
 }
 
-// step-completion word for a spinning host: ((uint32*)loss_out)[1] = ++*done_dev, ordered after the loss store
-__device__ __forceinline__ void signal_done(float* loss_out, unsigned int* done_dev) {
-  if (done_dev == nullptr) return;
-  const unsigned int v = *done_dev + 1;
-  *done_dev = v;
-  asm volatile("fence.acq_rel.sys;" ::: "memory");
-  st_release_sys(reinterpret_cast<uint32_t*>(loss_out) + 1, v);
-}
-
-// End-of-step hand-off to the host: the mean loss and the step count.  With a spinning host (done_dev) both travel in
-// ONE aligned 8-byte store to the pinned word pair {loss, count} - single-copy atomic, so no system fence (measured
-// several us, on the critical path of every step) is needed to order "loss before count".
-__device__ __forceinline__ void publish_loss(float* loss_out, float* loss_acc, unsigned int* done_dev) {
-  if (loss_acc != nullptr && done_dev != nullptr) {
-    const float l = *loss_acc;
-    *loss_acc = 0.f;
-    const unsigned int v = *done_dev + 1;
-    *done_dev = v;
-    const unsigned long long w = static_cast<unsigned long long>(__float_as_uint(l)) | (static_cast<unsigned long long>(v) << 32);
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(loss_out), "l"(w) : "memory");
-    return;
-  }
-  if (loss_acc != nullptr) {
-    *loss_out = *loss_acc;
-    *loss_acc = 0.f;
-  }
-  signal_done(loss_out, done_dev);
-}
-// publish_loss with the loss (*loss_acc) and the count (*done_dev) loaded ahead by the caller
-__device__ __forceinline__ void publish_loaded_loss(float* loss_out, float* loss_acc, unsigned int* done_dev, float l, unsigned int done) {
+// End-of-step hand-off to the host: the mean loss `l` and the step count, with *loss_acc and *done_dev (`done`) loaded by
+// the caller.  With a spinning host (done_dev) both travel in ONE aligned 8-byte store to the pinned word pair
+// {loss, count} - single-copy atomic, so no system fence (measured several us, on the critical path of every step) is
+// needed to order "loss before count".  Without a loss, ((uint32*)loss_out)[1] = ++*done_dev after a system fence.
+__device__ __forceinline__ void publish_loss(float* loss_out, float* loss_acc, unsigned int* done_dev, float l, unsigned int done) {
   if (loss_acc != nullptr) *loss_acc = 0.f;
   if (done_dev == nullptr) {
     if (loss_acc != nullptr) *loss_out = l;
@@ -652,14 +607,13 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
   const int tid = threadIdx.x;
   const bool locked = a.lock_mode == SF_LOCK_RW;
   const bool early = a.replica_version != nullptr;      // lock mode (runtime.cpp): see push_grant
-  const int skip = a.dbg_skip;
   TileRegs<2> T;
   unsigned long long t_grant = 0ull, t_grad = 0ull;
   // Hogwild reads the global step count racily; it does not depend on this step's kernels, so the
   // round trip to the master overlaps the predecessor's tail (before the programmatic-dependency wait).
   if (!locked && tid == 0) s_t = ld_relaxed_sys(a.ctrl + SF_CTRL_STEP) + 1;
   if (early) {
-    if (static_cast<int>(blockIdx.x) < a.num_tiles) push_tile_state(a, blockIdx.x, T, skip);      // in flight during the grant
+    if (static_cast<int>(blockIdx.x) < a.num_tiles) push_tile_state(a, blockIdx.x, T);      // in flight during the grant
     push_grant<SYS>(a, local_sync, true, &s_t, &s_epoch, &s_valid);
     if (trace.on) t_grant = gtime_ns();
   }
@@ -667,7 +621,7 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
   trace.mark();
   float loss = 0.f;
   unsigned int done = 0;
-  if (early && tid == 0) {         // any CTA may be the last: each loads the two words the last one publishes
+  if (tid == 0) {                  // any CTA may be the last: each loads the two words the last one publishes
     if (a.loss_acc != nullptr) loss = *a.loss_acc;
     if (a.done_dev != nullptr) done = *a.done_dev;
   }
@@ -684,16 +638,16 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
     const bool first = tile == static_cast<int>(blockIdx.x);
     const bool lead = trace.on && blockIdx.x == 0 && first;
     if (!early || !first) {
-      push_tile_load<true>(a, a.grad, tile, T, skip, false);
+      push_tile_load<true>(a, a.grad, tile, T);
     } else {
       if (!s_valid)      // the early loads may predate another writer's push: reload
 #pragma unroll
-        for (int half = 0; half < 2; ++half) tile_load_state(a, T, half, skip);
-      push_tile_grad<true>(a.grad, T, skip, false);
+        for (int half = 0; half < 2; ++half) tile_load_state(a, T, half);
+      push_tile_grad<true>(a.grad, T);
     }
     if (lead) t_grad = gtime_ns() + static_cast<unsigned long long>(T.g[0][0] == 12345.678f);      // gradient loads returned
     push_tile_apply<OPT, true, 2>(a, grads, 1, T, &s_t, !locked && first, s_tr, a.shadow_dst[0], a.vec_pub[0], lead ? s_ph : nullptr,
-                                  0, 0, skip, false);
+                                  0, 0);
   }
 
   // ---------------- completion ----------------
@@ -706,8 +660,7 @@ push_kernel(const SfPushArgs a, uint32_t* local_sync) {
     if (prev == gridDim.x - 1) {                  // last CTA of this push
       const unsigned long long t_arr = trace.on ? gtime_ns() : 0ull;
       local_sync[2] = 0;
-      if (early) publish_loaded_loss(a.loss_out, a.loss_acc, a.done_dev, loss, done);
-      else publish_loss(a.loss_out, a.loss_acc, a.done_dev);
+      publish_loss(a.loss_out, a.loss_acc, a.done_dev, loss, done);
       if (a.drop) {
         lk_red_relaxed<SYS>(a.ctrl + SF_CTRL_DROPPED, 1u);
       } else {
@@ -863,7 +816,7 @@ post_kernel(const SfPostArgs a, uint32_t* local_sync) {
     if (prev == gridDim.x - 1) {
       (void)ld_acquire_gpu(local_sync + 2);
       local_sync[2] = 0;
-      publish_loss(a.loss_out, a.loss_acc, a.done_dev);
+      publish_loss(a.loss_out, a.loss_acc, a.done_dev, a.loss_acc != nullptr ? *a.loss_acc : 0.f, a.done_dev != nullptr ? *a.done_dev : 0u);
       if (!a.drop) {
         st_release_gpu(local_sync + 4, s_seq + 1);
         st_release_sys(a.flags + SF_MB_POSTED, s_seq + 1);
@@ -881,22 +834,25 @@ post_kernel(const SfPostArgs a, uint32_t* local_sync) {
 // CTA 0 is the leader: its first warp scans every worker's POSTED / APPLIED words in one round trip
 // (lane = worker), (lock mode) takes the write lock ONCE for the whole batch, and publishes (epoch, ready mask,
 // step) to the other CTAs through master-local memory; every CTA then runs its share of the tiles, applying the
-// posted gradients one after the other IN REGISTERS (push_tile): each push is still its own optimizer step with
-// its own step number - exactly the reference's parameter server, one update per push in arrival (round-robin)
+// posted gradients one after the other IN REGISTERS (push_tiles_pipelined): each push is still its own optimizer step
+// with its own step number - exactly the reference's parameter server, one update per push in arrival (round-robin)
 // order - but the tuples and the bf16 publish move once per batch.  The leader bumps the counters by the batch
-// size, releases the lock and acknowledges every consumed mailbox through its APPLIED word.
+// size, releases the lock and acknowledges every consumed mailbox through its APPLIED word.  A shard's applier (ack
+// words given) also has every CTA acknowledge the consumed workers in their own memory as soon as its tiles are out.
 // sync words: 0 = epoch of the published decision, 1 = ready mask (0 = nothing), 2 = first step number,
-//             3 = done counter, 4 = round-robin cursor.
+//             3 = done counter, 4 = round-robin cursor, 5 = publish buffer / slot of the pass;
+//             stats only: 8-9 = time of the decision, 10-11 = time of the last acknowledged decision.
 // ---------------------------------------------------------------------------
 constexpr int kApplierThreads = 512;
+// 120 registers: a 512-thread CTA leaves 4K of its SM's registers to the kernels beside it.  The tile loop needs no more
+// (no spill at this bound); with only a 512-thread launch bound ptxas takes up to 124, and the SM has none left over.
 template <int OPT, bool SYS>
-__global__ void __launch_bounds__(kApplierThreads, 1)
+__global__ void __maxnreg__(120)
 applier_kernel(const SfApplierArgs a, const uint32_t seq) {
   __shared__ uint32_t s_t;
   __shared__ uint32_t s_mask;
   __shared__ uint32_t s_buf;
   __shared__ int s_n;
-  __shared__ uint32_t s_found;
   __shared__ float* s_grads[8];
   __shared__ __align__(16) __nv_bfloat16 s_tr[kTileC][kTileR + 8];
   const int tid = threadIdx.x;
@@ -961,10 +917,10 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
             t = ld_relaxed_sys(a.push.ctrl + SF_CTRL_STEP) + 1;
             if (a.n_ver > 0) {
               // seqlock: stamp `begin` in every replica before the first publish store of this pass can land
-              const uint32_t ver = (a.ver_local != nullptr ? ld_relaxed_sys(a.ver_local) : a.sync[6]) + 1;
+              const uint32_t ver = ld_relaxed_sys(a.ver_local) + 1;
               for (int d = 0; d < a.n_ver; ++d) st_u32_pub(a.ver_begin[d], ver, a.ver_mc != 0);
               asm volatile("fence.acq_rel.sys;" ::: "memory");
-              if (a.slot_off_bf16 != 0) buf = ver & 1u;          // two publish slots: this pass lands in slot ver & 1
+              buf = ver & 1u;                                    // two publish slots: this pass lands in slot ver & 1
             }
           }
           if (a.stats != nullptr) a.sync[8] = static_cast<uint32_t>(gtime_ns()), a.sync[9] = static_cast<uint32_t>(gtime_ns() >> 32);
@@ -977,33 +933,11 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
           s_buf = buf;
         }
       }
-    } else if (a.warm_polls <= 0) {
-      if (tid == 0) {
-        const unsigned long long t0 = gtime_ns();
-        while (ld_acquire_gpu(a.sync + 0) != epoch) {
-          __nanosleep(20);
-          if (gtime_ns() - t0 > a.idle_timeout_ns + kLockTimeoutNs) sf_fail(0x408);
-        }
-      }
-    } else {
-      // follower with warm-up: poll in short bursts; between bursts the whole CTA runs the tile code dry
+    } else if (tid == 0) {
       const unsigned long long t0 = gtime_ns();
-      const int my_tile = (a.tile_end > a.tile_begin ? a.tile_begin : 0) + (static_cast<int>(blockIdx.x) - 1) % max(1, (a.tile_end > a.tile_begin ? a.tile_end - a.tile_begin : a.push.num_tiles));
-      while (true) {
-        if (tid == 0) {
-          uint32_t found = 0;
-          for (int i = 0; i < a.warm_polls && !found; ++i) {
-            found = ld_acquire_gpu(a.sync + 0) == epoch ? 1u : 0u;
-            if (!found) __nanosleep(20);
-          }
-          s_found = found;
-          if (gtime_ns() - t0 > a.idle_timeout_ns + kLockTimeoutNs) sf_fail(0x408);
-        }
-        __syncthreads();
-        if (s_found) break;
-        s_t = 1;
-        push_tile<OPT, false, 1>(a.push, s_grads, 1, my_tile, &s_t, false, s_tr, a.push.shadow_dst[0], a.push.vec_pub[0], nullptr, 0, 0, true);
-        __syncthreads();
+      while (ld_acquire_gpu(a.sync + 0) != epoch) {
+        __nanosleep(20);
+        if (gtime_ns() - t0 > a.idle_timeout_ns + kLockTimeoutNs) sf_fail(0x408);
       }
     }
     if (!leader && tid == 0) {
@@ -1028,8 +962,8 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
     }
     __syncthreads();
     const int n = s_n;
-    const long long off_bf16 = (a.slot_off_bf16 != 0 && s_buf) ? a.slot_off_bf16 : 0;
-    const long long off_f32 = (a.slot_off_bf16 != 0 && s_buf) ? a.slot_off_f32 : 0;
+    const long long off_bf16 = s_buf ? a.slot_off_bf16 : 0;      // two publish slots (0 without)
+    const long long off_f32 = s_buf ? a.slot_off_f32 : 0;
     __nv_bfloat16* const pub0 = ((a.dbuf && s_buf) ? a.shadow_alt : a.push.shadow_dst[0]) + off_bf16;
     float* const vec0 = (a.dbuf && s_buf) ? a.vec_pub_alt : a.push.vec_pub[0];
     const int tile_lo = a.tile_end > a.tile_begin ? a.tile_begin : 0;
@@ -1038,17 +972,8 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
     __shared__ unsigned long long tpt[3];
     if (probe) tpt[0] = tpt[1] = tpt[2] = 0ull;
     const unsigned long long tpa = probe ? gtime_ns() : 0ull;          // s_grads built, barrier passed
-    // warm mode: CTA 0 only coordinates (its tile code would be cold: it spends its idle time scanning the flags)
-    const int tile_ctas = a.warm_polls > 0 ? static_cast<int>(gridDim.x) - 1 : static_cast<int>(gridDim.x);
-    const int tile_cta = a.warm_polls > 0 ? static_cast<int>(blockIdx.x) - 1 : static_cast<int>(blockIdx.x);
-    if (tile_cta >= 0) {
-      if (tile_hi - tile_lo > tile_ctas)      // several tiles per CTA: keep the next tile's loads in flight
-        push_tiles_pipelined<OPT, 1>(a.push, s_grads, n, tile_lo + tile_cta, tile_hi, tile_ctas, &s_t, s_tr, pub0, vec0, probe ? tpt : nullptr,
-                                     off_bf16, off_f32);
-      else
-        for (int tile = tile_lo + tile_cta; tile < tile_hi; tile += tile_ctas)
-          push_tile<OPT, false, 1>(a.push, s_grads, n, tile, &s_t, false, s_tr, pub0, vec0, probe ? tpt : nullptr, off_bf16, off_f32);
-    }
+    push_tiles_pipelined<OPT, 1>(a.push, s_grads, n, tile_lo + static_cast<int>(blockIdx.x), tile_hi, static_cast<int>(gridDim.x), &s_t, s_tr,
+                                 pub0, vec0, probe ? tpt : nullptr, off_bf16, off_f32);
     __syncthreads();
     const unsigned long long tp1 = probe ? gtime_ns() : 0ull;
     if (probe && tpt[0] != 0ull) {
@@ -1060,7 +985,8 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
       const unsigned long long q0 = gtime_ns(), q1 = gtime_ns();
       a.stats[13] += q1 - q0;              // cost of one %globaltimer read
     }
-    if (a.ack_counting) {
+    const bool counting = a.ack[0] != nullptr;          // a shard's applier: every CTA acknowledges (runtime.cpp)
+    if (counting) {
       // distributed acknowledgement: this CTA is done with the consumed mailboxes and its share of the publish is on its
       // way.  ONE system fence per CTA (thread 0; bar.sync makes it cumulative over the CTA's stores), then relaxed
       // counts: every CTA pays its NVLink flush in parallel instead of the leader paying it after all of them.
@@ -1069,14 +995,13 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
       if (tid < 8 && (mask >> tid & 1u) && a.ack[tid] != nullptr)
         asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(a.ack[tid]), "r"(1u) : "memory");
       // seqlock `end`: count this CTA's completion in every replica (after the fence: its publish stores are performed)
-      if (a.n_ver > 0 && tid >= 8 && tid < 8 + a.n_ver) {
+      if (tid >= 8 && tid < 8 + a.n_ver) {
         if (a.ver_mc) asm volatile("multimem.red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(a.ver_end[tid - 8]), "r"(1u) : "memory");
         else asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(a.ver_end[tid - 8]), "r"(1u) : "memory");
       }
     }
     if (tid == 0) {
-      if (a.n_ver > 0 && !a.ack_counting) asm volatile("fence.acq_rel.sys;" ::: "memory");     // this CTA's publish stores are performed everywhere
-      if (a.ack_counting) lk_red_relaxed<false>(a.sync + 3, 1u);       // ordered after the fence above
+      if (counting) lk_red_relaxed<false>(a.sync + 3, 1u);       // ordered after the fence above
       else lk_red_release<false>(a.sync + 3, 1u);
       if (probe) {
         const unsigned long long tp2 = gtime_ns();
@@ -1098,14 +1023,6 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
         // the freshly written buffer becomes the current one (release: after every CTA's publish stores, which the
         // acquire of the done counter above made visible to this thread)
         if (a.dbuf) (void)atom_xor_release_sys(a.push.ctrl + SF_CTRL_PUB, 0x80000000u);
-        if (a.n_ver > 0 && !a.ack_counting) {
-          // every CTA fenced its publish stores before arriving: the pass is complete in every replica -> stamp `end`
-          const uint32_t ver = a.sync[6] + 1;
-          asm volatile("fence.acq_rel.sys;" ::: "memory");
-          for (int d = 0; d < a.n_ver; ++d) st_u32_pub(a.ver_end[d], ver, a.ver_mc != 0);
-          a.sync[6] = ver;
-          asm volatile("fence.acq_rel.sys;" ::: "memory");
-        }
         lk_red_relaxed<SYS>(a.push.ctrl + SF_CTRL_STEP, static_cast<uint32_t>(n));
         lk_red_relaxed<SYS>(a.push.ctrl + SF_CTRL_PUSHES, static_cast<uint32_t>(n));
         lk_red_relaxed<SYS>(a.push.ctrl + SF_CTRL_VERSION, static_cast<uint32_t>(n));
@@ -1123,11 +1040,6 @@ applier_kernel(const SfApplierArgs a, const uint32_t seq) {
       if (mask >> tid & 1u) {
         asm volatile("fence.acq_rel.gpu;" ::: "memory");
         st_release_sys(a.flags + tid * SF_MB_WORDS + SF_MB_APPLIED, posted);
-        // sharded master: the acknowledgement lands in the worker's OWN memory (its next step spins locally)
-        if (a.ack[tid] != nullptr && !a.ack_counting) {
-          asm volatile("fence.acq_rel.sys;" ::: "memory");
-          st_release_sys(a.ack[tid], posted);
-        }
       }
       if (a.stats != nullptr) {
         __syncwarp();
@@ -1213,8 +1125,7 @@ sync_pull_kernel(const SfSyncPullArgs a) {
   // ---- read-your-writes: this shard's applier has consumed my last post (it acknowledges into MY memory) ----
   unsigned long long t_seen = 0;
   if (tid == 0) {
-    const uint32_t grid_r = static_cast<uint32_t>(a.ack_grid[shard]);
-    const uint32_t want = *a.my_posted * (grid_r ? grid_r : 1u);
+    const uint32_t want = *a.my_posted * static_cast<uint32_t>(a.ack_grid[shard]);
     const unsigned long long t0 = gtime_ns();
     // relaxed polling (the word lives in local memory, remote appliers write it); the data the acknowledgement covers is
     // consumed by LATER kernels (kernel boundary) or validated by the seqlock below
@@ -1254,20 +1165,11 @@ sync_pull_kernel(const SfSyncPullArgs a) {
       // seqlock reader without fences: the stamp loads are relaxed.sys (served by L2, the coherence point of local
       // memory); the copy's loads cannot issue before the version is known (bar.sync below) and the re-check of `begin`
       // is issued after the copy's values were consumed by its stores (bar.sync), i.e. in program order.
-      // `begin` = passes started, `end` = CTA completions (grid_r per pass).
-      const uint32_t grid_r = static_cast<uint32_t>(a.ack_grid[shard]);
-      uint32_t b;
-      if (a.slot_off_bf16 != 0) {
-        // two slots: never wait.  Quiescent -> the newest pass is complete; a pass in flight -> the one before it is
-        // (the leader starts a pass only after every CTA of the previous one fenced its publish stores)
-        b = ld_relaxed_sys(a.ver_begin + shard * a.ver_stride);
-        if (ld_relaxed_sys(a.ver_end + shard * a.ver_stride) != b * (grid_r ? grid_r : 1u)) b -= 1u;
-      } else {
-        while (ld_relaxed_sys(a.ver_end + shard * a.ver_stride) != (b = ld_relaxed_sys(a.ver_begin + shard * a.ver_stride)) * (grid_r ? grid_r : 1u)) {
-          __nanosleep(20);                       // an update of this shard is landing right now
-          if (gtime_ns() - t0 > kLockTimeoutNs) sf_fail(0x40A);
-        }
-      }
+      // `begin` = passes started, `end` = CTA completions (ack_grid per pass).
+      // Two slots: never wait.  Quiescent -> the newest pass is complete; a pass in flight -> the one before it is
+      // (the leader starts a pass only after every CTA of the previous one fenced its publish stores)
+      uint32_t b = ld_relaxed_sys(a.ver_begin + shard * a.ver_stride);
+      if (ld_relaxed_sys(a.ver_end + shard * a.ver_stride) != b * static_cast<uint32_t>(a.ack_grid[shard])) b -= 1u;
       s_e = b;
       if (cps > 1) {
         sy[5] = b;
@@ -1277,16 +1179,16 @@ sync_pull_kernel(const SfSyncPullArgs a) {
     __syncthreads();
     {
       const uint32_t ver = s_e;
-      const long long so_b = (a.slot_off_bf16 != 0 && (ver & 1u)) ? a.slot_off_bf16 : 0, so_f = (a.slot_off_bf16 != 0 && (ver & 1u)) ? a.slot_off_f32 : 0;
+      const long long so_b = (ver & 1u) ? a.slot_off_bf16 : 0, so_f = (ver & 1u) ? a.slot_off_f32 : 0;
       for (int tile = a.bounds[shard] + part; tile < a.bounds[shard + 1]; tile += cps * kCopyBatch)
         copy_tiles_publish(a, tile, a.bounds[shard + 1], cps, so_b, so_f);
     }
     __syncthreads();
     if (tid == 0) {
       const uint32_t e = s_e;
-      // single slot: nothing may have started; two slots: slot e & 1 is rewritten by pass e + 2
+      // slot e & 1 is rewritten by pass e + 2
       const uint32_t b2 = ld_relaxed_sys(a.ver_begin + shard * a.ver_stride);
-      const bool clean = a.slot_off_bf16 != 0 ? (static_cast<int32_t>(b2 - e) <= 1) : (b2 == e);
+      const bool clean = static_cast<int32_t>(b2 - e) <= 1;
       uint32_t ok;
       if (cps == 1) {
         ok = clean ? 1u : 0u;
@@ -1349,7 +1251,7 @@ post_flags_kernel(const SfPostFlagsArgs a) {
     return;
   }
   if (tid == 0) {
-    publish_loss(a.loss_out, a.loss_acc, a.done_dev);
+    publish_loss(a.loss_out, a.loss_acc, a.done_dev, a.loss_acc != nullptr ? *a.loss_acc : 0.f, a.done_dev != nullptr ? *a.done_dev : 0u);
   }
   if (!a.drop && a.phase == 2 && tid < a.n_shards) {
     // every gradient store (wgrad epilogues, tail forwarding) belongs to a kernel that COMPLETED before this one started

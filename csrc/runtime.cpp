@@ -160,7 +160,6 @@ SfPushArgs parse_push(const py::dict& d) {
   a.n_vec_dst = static_cast<int>(vds.size());
   for (size_t i = 0; i < vds.size(); ++i) a.vec_dst[i] = P<float>(vds[i]);
   a.mb_zero = getd<int>(d, "mb_zero", 0);
-  a.dbg_skip = getd<int>(d, "dbg_skip", 0);
   a.grad = P<float>(getd<uintptr_t>(d, "grad", 0));
   a.loss_acc = P<float>(getd<uintptr_t>(d, "loss_acc", 0));
   a.loss_out = P<float>(getd<uintptr_t>(d, "loss_out", 0));
@@ -249,11 +248,15 @@ SfSyncPullArgs parse_sync_pull(const py::dict& d) {
   a.stats = P<unsigned long long>(getd<uintptr_t>(d, "stats", 0));
   {
     auto ag = getd<std::vector<int>>(d, "ack_grid", {});
-    for (size_t i = 0; i < ag.size() && i < SF_MAX_SHARDS; ++i) a.ack_grid[i] = ag[i];
+    if (static_cast<int>(ag.size()) != a.n_shards) throw std::runtime_error("sync_pull: one ack_grid entry per shard");
+    for (int i = 0; i < a.n_shards; ++i) {
+      if (ag[i] < 1) throw std::runtime_error("sync_pull: ack_grid entries must be >= 1");
+      a.ack_grid[i] = ag[i];
+    }
   }
   if (!a.applied || !a.my_posted) throw std::runtime_error("sync_pull: applied / my_posted are required");
-  if (a.copy && (!a.ver_begin || !a.ver_end || !a.src || !a.dst || !a.segs || !a.tile_map || !a.sync))
-    throw std::runtime_error("sync_pull: copy needs ver_begin/ver_end/src/dst/segs/tile_map/sync");
+  if (a.copy && (!a.ver_begin || !a.ver_end || !a.src || !a.dst || !a.segs || !a.tile_map || !a.sync || !a.slot_off_bf16 || !a.slot_off_f32))
+    throw std::runtime_error("sync_pull: copy needs ver_begin/ver_end/src/dst/segs/tile_map/sync/slot_off_bf16/slot_off_f32");
   return a;
 }
 
@@ -290,7 +293,10 @@ py::bytes pack_ryw(int n_shards, const std::vector<int>& ack_grid, uintptr_t app
   std::memset(&r, 0, sizeof(r));
   if (n_shards < 1 || n_shards > SF_MAX_SHARDS || static_cast<int>(ack_grid.size()) != n_shards) throw std::runtime_error("pack_ryw: n_shards in [1, 8], one grid size per shard");
   r.n_shards = n_shards;
-  for (int i = 0; i < n_shards; ++i) r.ack_grid[i] = ack_grid[i];
+  for (int i = 0; i < n_shards; ++i) {
+    if (ack_grid[i] < 1) throw std::runtime_error("pack_ryw: grid sizes must be >= 1");
+    r.ack_grid[i] = ack_grid[i];
+  }
   r.applied = P<const uint32_t>(applied);
   r.my_posted = P<const uint32_t>(my_posted);
   r.stats = P<unsigned long long>(stats);
@@ -732,7 +738,11 @@ class Applier {
     {
       auto acks = getd<std::vector<uintptr_t>>(shard, "ack", {});
       if (acks.size() > 8) throw std::runtime_error("applier: at most 8 ack words");
-      for (size_t i = 0; i < acks.size(); ++i) args_.ack[i] = P<uint32_t>(acks[i]);
+      if (!acks.empty() && static_cast<int>(acks.size()) != n_workers) throw std::runtime_error("applier: one ack word per worker, or none");
+      for (size_t i = 0; i < acks.size(); ++i) {
+        if (!acks[i]) throw std::runtime_error("applier: ack words must be non-null");
+        args_.ack[i] = P<uint32_t>(acks[i]);
+      }
       auto vb = getd<std::vector<uintptr_t>>(shard, "ver_begin", {});
       auto ve = getd<std::vector<uintptr_t>>(shard, "ver_end", {});
       if (vb.size() != ve.size() || vb.size() > 8) throw std::runtime_error("applier: ver_begin / ver_end lists must match (<= 8)");
@@ -740,12 +750,12 @@ class Applier {
       for (size_t i = 0; i < vb.size(); ++i) { args_.ver_begin[i] = P<uint32_t>(vb[i]); args_.ver_end[i] = P<uint32_t>(ve[i]); }
       args_.ver_mc = getd<int>(shard, "ver_mc", 0);
       args_.stats = P<unsigned long long>(getd<uintptr_t>(shard, "stats", 0));
-      args_.ack_counting = getd<int>(shard, "ack_counting", 0);
       args_.linger = getd<int>(shard, "linger", 0);
-      args_.warm_polls = getd<int>(shard, "warm_polls", 0);
       args_.ver_local = P<const uint32_t>(getd<uintptr_t>(shard, "ver_local", 0));
       args_.slot_off_bf16 = getd<long long>(shard, "slot_off_bf16", 0);
       args_.slot_off_f32 = getd<long long>(shard, "slot_off_f32", 0);
+      if (args_.n_ver > 0 && (acks.empty() || !args_.ver_local || !args_.slot_off_bf16 || !args_.slot_off_f32))
+        throw std::runtime_error("applier: seqlock stamps need ack words, ver_local and both slot offsets");
     }
     ck(cudaGetDevice(&device_), "cudaGetDevice");
     int lo = 0, hi = 0;

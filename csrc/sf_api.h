@@ -224,7 +224,6 @@ struct SfPushArgs {
   float* vec_dst[8];              // sharded master: fp32 publish of the 1-D variables into every replica (one multicast
   int n_vec_dst;                  // alias when shadow_is_mc); indexed from vec_offset.  0 = use vec_pub
   int mb_zero;                    // applier: zero the consumed mailbox elements (accumulating wgrad epilogues add into them)
-  int dbg_skip;                   // profiling only: bit 0 = no publish stores, bit 1 = no state stores, bit 2 = no state / gradient loads
   float* grad;                    // local flat gradient (consumed, then zeroed for the next step)
   float* loss_acc;                // local: loss accumulated by the loss kernel (consumed + zeroed)
   float* loss_out;                // last step's loss for the host to read (device or pinned host memory)
@@ -315,12 +314,8 @@ struct SfApplierArgs {
   size_t mailbox_stride;          // floats
   uint32_t* flags;                // [n_workers][SF_MB_WORDS]
   int n_workers;
-  uint32_t* sync;                 // 8 words of master-local memory for the in-grid protocol
+  uint32_t* sync;                 // 12 words of master-local memory for the in-grid protocol (applier_kernel)
   unsigned long long idle_timeout_ns;   // listening window: a launch exits after this long without any posted mailbox
-  int warm_polls;                       // > 0: follower CTAs re-execute the tile code as a dry run (no memory traffic)
-                                        // after every `warm_polls` unsuccessful polls, and CTA 0 only coordinates (owns no
-                                        // tile): the pass is bound by instruction fetch when the code was evicted by the
-                                        // training kernels sharing the SM (measured: 7 us cold vs the memory-bound ~2 us)
   int linger;                           // 1: keep listening after a pass (warm instruction cache / TLB for the next one: the
                                         // pass is latency bound); 0: a launch exits as soon as nothing more is posted
   int dbuf;                       // double-buffered publish: passes alternate between (push.shadow_dst[0], push.vec_pub[0])
@@ -330,24 +325,20 @@ struct SfApplierArgs {
   // ---- sharded master: this applier owns push tiles [tile_begin, tile_end) (0, 0 = all) ----
   int tile_begin, tile_end;
   uint32_t* ack[8];               // per worker: acknowledgement word of THIS shard inside the worker's own memory (peer
-                                  // mapped); nullptr = acknowledge through flags[w][SF_MB_APPLIED] only
-  int ack_counting;               // 1: every CTA adds 1 to the word of each consumed worker right after its own tiles
-                                  // (red.release.sys: one NVLink flush per CTA, all in parallel) - the worker waits for
-                                  // posts * gridDim acknowledgements; 0: the leader stores the sequence number after the pass
-  // seqlock stamps of this shard in every replica's publish segment: begin is bumped before the first publish store of a
-  // pass, end after the last one; a reader's snapshot of the shard is consistent iff it read end == e before and
-  // begin == e after copying.  n_ver = 1 + ver_mc: one multimem.st reaches every replica; else one store per peer.
+                                  // mapped), one per worker or none.  Given: every CTA adds 1 to the word of each consumed
+                                  // worker right after its own tiles (one NVLink flush per CTA, all in parallel) - the
+                                  // worker waits for posts * gridDim acknowledgements
+  // seqlock stamps of this shard in every replica's publish segment (lock mode; needs ack words, ver_local and the slot
+  // offsets): `begin` counts the passes STARTED (stamped by the leader before the first publish store), `end` counts CTA
+  // completions (every CTA adds 1 after its own fence): the shard is quiescent iff end == begin * gridDim.
+  // n_ver = 1 + ver_mc: one multimem.st reaches every replica; else one store per peer.
   uint32_t* ver_begin[8];
   uint32_t* ver_end[8];
   int n_ver;
   int ver_mc;
-  // ack_counting mode: `begin` counts the passes STARTED (stamped by the leader before the first publish store), `end`
-  // counts CTA completions (every CTA adds 1 after its own fence): the shard is quiescent iff end == begin * gridDim.
-  // No leader-side end stamp, no serialised fences after the pass.  ver_local: this shard's begin stamp in the OWN
-  // replica (unicast address; survives applier restarts).
-  const uint32_t* ver_local;
-  // two publish slots per replica (lock mode): pass v writes slot v & 1 = every publish destination advanced by these
-  // element offsets, so a reader can always copy the newest COMPLETE pass while the next one is landing in the other slot
+  const uint32_t* ver_local;      // this shard's begin stamp in the OWN replica (unicast address; survives applier restarts)
+  // two publish slots per replica: pass v writes slot v & 1 = every publish destination advanced by these element
+  // offsets, so a reader can always copy the newest COMPLETE pass while the next one is landing in the other slot
   long long slot_off_bf16, slot_off_f32;
   unsigned long long* stats;      // optional: [0] sum(ns decide -> tiles done), [1] sum(ns decide -> acknowledged), [2] passes, [3] pushes
 };
@@ -367,12 +358,12 @@ struct SfSyncPullArgs {
   int bounds[SF_MAX_SHARDS + 1];
   const uint32_t* applied;        // local: word r * 16 = acknowledgement word of shard r for this worker
   const uint32_t* my_posted;      // local: sequence number of my last post
-  int ack_grid[SF_MAX_SHARDS];    // CTAs of shard r's applier: the word counts CTA acknowledgements (0: it holds the sequence number)
+  int ack_grid[SF_MAX_SHARDS];    // CTAs of shard r's applier (>= 1): the word counts CTA acknowledgements
   int copy;                       // 1: snapshot inbox -> working replica
   const uint32_t* ver_begin;      // local inbox stamps: word r * ver_stride
   const uint32_t* ver_end;
   int ver_stride;
-  long long slot_off_bf16, slot_off_f32;   // second publish slot (0: single slot, the reader waits for quiescence instead)
+  long long slot_off_bf16, slot_off_f32;   // second publish slot (SfApplierArgs), required with copy
   const __nv_bfloat16* src;       // inbox publish buffer (local copy fed by the appliers' multicast stores)
   __nv_bfloat16* dst;             // working replica
   const float* src_vec;           // inbox fp32 copy of the 1-D tail (indexed from vec_offset)

@@ -60,7 +60,7 @@ WAIT_CODES = {0x100: "gemm: TMA producer waiting for a free smem stage", 0x200: 
               0x405: "pull / first GEMM: read-your-writes wait for the applier(s) to acknowledge my last post",
               0x406: "post: waiting for my mailbox to be consumed", 0x407: "applier: leader waiting for the other CTAs",
               0x408: "applier: follower CTA waiting for the leader's decision", 0x409: "applier: stale pull registrations (double-buffered publish)",
-              0x40A: "sync_pull: a shard's seqlock stamps never became consistent", 0x40B: "sync_pull: CTAs of a shard waiting for each other's version",
+              0x40B: "sync_pull: CTAs of a shard waiting for each other's version",
               0x40C: "sync_pull: no consistent snapshot of a shard within the bound", 0x40D: "sync_pull: waiting for the shard leader's version pick"}
 
 

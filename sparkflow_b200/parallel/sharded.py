@@ -105,8 +105,6 @@ class ShardedMaster:
         self.pub = SymmetricHeap(pub_bytes, ctx if self.spmd else None, idx, multicast=True, tag="pub")
         self.seg = SymmetricHeap(seg_bytes, ctx if self.spmd else None, idx, multicast=False, tag="seg")
         self.multicast = self.pub.multicast
-        # follower CTAs of an applier keep their tile code warm with dry runs between polls; CTA 0 then owns no tile
-        self.warm_polls = int(os.environ.get("SPARKFLOW_APPLIER_WARM_POLLS", "0"))
         self.appliers: Dict[int, object] = {}
         self._stats: Dict[int, torch.Tensor] = {}
         self._keep: List[object] = []
@@ -323,13 +321,11 @@ class ShardedMaster:
                             shadow_is_mc=1 if self.multicast else 0, vec_dst=vec_dst if lay.vec_count else [], vec_offset=lay.vec_offset,
                             grad=0, applier=1, segs=native.ptr(segs_dev), tile_map=native.ptr(tile_map), num_tiles=self.n_tiles,
                             seg_rows=lay.seg_rows(), optimizer=self.spec.opt_id, lock_mode=0, drop=0, scope_sys=1 if scope_sys else 0,
-                            grad_scale=1.0, hyper=self.spec.native_hyper(), mb_zero=1 if self.mb_zero else 0,
-                            dbg_skip=int(os.environ.get("SPARKFLOW_DEBUG_SKIP", "0")))
+                            grad_scale=1.0, hyper=self.spec.native_hyper(), mb_zero=1 if self.mb_zero else 0)
                 if s not in self._stats:
                     self._stats[s] = torch.zeros(16, dtype=torch.int64, device=dev)
                 shard = dict(tile_begin=self.bounds[s], tile_end=self.bounds[s + 1], ack=[self.ack_ptr(w, s) for w in range(self.n)],
-                             stats=native.ptr(self._stats[s]), ack_counting=1,
-                             linger=int(os.environ.get("SPARKFLOW_APPLIER_LINGER", "1")), warm_polls=self.warm_polls)
+                             stats=native.ptr(self._stats[s]), linger=int(os.environ.get("SPARKFLOW_APPLIER_LINGER", "1")))
                 if self.lock_mode:
                     shard.update(ver_begin=[p + s * VER_STRIDE * 4 for p in stamps], ver_end=[p + (s * VER_STRIDE + 16) * 4 for p in stamps],
                                  ver_mc=1 if self.multicast else 0, ver_local=self.pub_ptr(s, self.o_stamps) + s * VER_STRIDE * 4,
@@ -348,7 +344,7 @@ class ShardedMaster:
         # must be resident at once: small shards get one CTA per tile (lowest pass latency), larger ones are capped so
         # the training kernels of the same GPU keep most of the SMs (big models: up to half of them).
         cap = 40 if n_own <= 160 else 74
-        return int(os.environ.get("SPARKFLOW_APPLIER_CTAS", "0")) or (min(cap, n_own) + (1 if self.warm_polls > 0 else 0))
+        return int(os.environ.get("SPARKFLOW_APPLIER_CTAS", "0")) or min(cap, n_own)
 
     def applier_latency(self) -> Dict[str, float]:
         """Device-measured averages of the owned shards' appliers: decision -> all tiles applied + published (`apply_us`),

@@ -857,6 +857,32 @@ def test_sharded_two_slot_seqlock_protocol_model():
         assert len(accepted) == 30
 
 
+def test_sharded_protocol_args_reject_what_the_kernels_do_not_handle():
+    """Host-side checks of the sharded master's arguments, raised before anything is launched: workers count one
+    acknowledgement per applier CTA (a grid entry < 1 is rejected), a lock-mode snapshot reads one of two publish slots
+    (a copy without slot offsets is rejected), and a stamping applier acknowledges per CTA and stamps from its own replica
+    (stamps without ack words, ver_local or slot offsets are rejected)."""
+    from sparkflow_b200.ops import native
+
+    C = native.cuda_ext()
+    with pytest.raises(RuntimeError, match="grid sizes"):
+        C.pack_ryw(2, [3, 0], 16, 16, 0)
+    assert len(C.pack_ryw(2, [3, 1], 16, 16, 0)) > 0
+    base = dict(n_shards=2, bounds=[0, 4, 8], applied=16, my_posted=16)
+    for ack_grid in ([3, 0], [3]):
+        with pytest.raises(RuntimeError, match="ack_grid"):
+            C.sync_pull(dict(base, ack_grid=ack_grid), 0)
+    copy = dict(base, ack_grid=[3, 3], copy=1, ver_begin=16, ver_end=16, src=16, dst=16, segs=16, tile_map=16, sync=16)
+    with pytest.raises(RuntimeError, match="slot_off"):
+        C.sync_pull(dict(copy, slot_off_bf16=8), 0)
+    push = dict(state=16, ctrl=16, grad=0, applier=1, segs=16, tile_map=16, num_tiles=8)
+    stamps = dict(ack=[16, 16], ver_begin=[16], ver_end=[16], ver_local=16, slot_off_bf16=8, slot_off_f32=8)
+    for shard, msg in ((dict(stamps, ack=[16]), "one ack word per worker"), (dict(stamps, ack=[]), "seqlock stamps"),
+                       (dict(stamps, ver_local=0), "seqlock stamps"), (dict(stamps, slot_off_f32=0), "seqlock stamps")):
+        with pytest.raises(RuntimeError, match=msg):
+            C.Applier(push, 16, 64, 16, 2, 16, 1e-4, 1, 1, 0, 0, 0, shard)
+
+
 def test_symmetric_heap_fd_rendezvous_and_shard_bounds(tmp_path):
     """Host-side plumbing of the sharded master that needs no GPU: (a) physical-memory handles travel between ranks as file
     descriptors over abstract Unix sockets (parallel/symm.py: _FdServer / _fetch_fd) - checked with an ordinary file
