@@ -76,9 +76,12 @@ struct SfGemmEpilogue {
   long long route_off;
   // fused dropout (reference: the tfDropout keep-prob placeholder of tf.nn.dropout, ml_util.py:70-71): after the
   // activation every element is kept with probability drop_keep and scaled by 1 / drop_keep.  The mask is
-  // Philox4x32-10 keyed by drop_seed over the counter (row, column / 4, *drop_ctr, drop_stream), so it is a pure
-  // function of (sample row, feature, step number, layer) - no mask tensor is stored: the backward pass recovers it
-  // from the stored activation (aux_keep: aux holds act(z) * mask / keep, so mask = aux != 0).
+  // Philox4x32-10 keyed by (drop_seed, 0x5F3759DF) over the counter (row, column / 4, *drop_ctr, drop_stream), lane
+  // column % 4 kept iff it is below keep * 2^32: a pure function of (sample row, feature, step number, layer, seed).
+  // The training plans mix the worker index and the address of the plan's step counter into the seed, so workers and
+  // plans of one worker draw different masks; forward-only plans have no counter (step number 0).  No mask tensor is
+  // stored: the backward pass recovers it from the stored activation (aux_keep: aux holds act(z) * mask / keep, so
+  // mask = aux != 0).
   float drop_keep;                // 0 or >= 1: no dropout
   unsigned int drop_seed, drop_stream;
   const unsigned int* drop_ctr;   // device word that changes every step (nullptr: 0)

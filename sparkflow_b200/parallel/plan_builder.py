@@ -354,12 +354,15 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         last = i == stop_layer
         d = dict(a=P(cur["buf"]), lda=cur["ld"], b=P(wsrc) + ks.wt_off * 2, ldb=ks.wt_ld, M=B, N=ks.cols, K=ks.rows,
                  bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], **ryw_args())
+        drop = None
         if l.dropout_keep:
-            # fused Philox dropout: the mask is a function of (row, column, step counter of this plan, layer)
+            # fused Philox dropout: the mask is a function of (row, column, step counter of this plan, layer) under a
+            # seed that also mixes in the worker index and the address of the plan's step counter
             seed = (int(os.environ.get("SPARKFLOW_DROPOUT_SEED", "20260921")) ^ (0x9E3779B9 * (worker.worker_index + 1))
                     ^ ((P(done_dev) >> 4) if done_dev is not None else 0)) & 0xFFFFFFFF
             d.update(drop_keep=float(l.dropout_keep), drop_seed=seed, drop_stream=i, drop_ctr=P(done_dev) if done_dev is not None else 0)
-        rec[i] = dict(a_in=cur["buf"], a_in_ld=cur["ld"], a_inT=cur.get("bufT"))
+            drop = dict(keep=float(l.dropout_keep), seed=seed, stream=i, ctr=done_dev)
+        rec[i] = dict(a_in=cur["buf"], a_in_ld=cur["ld"], a_inT=cur.get("bufT"), drop=drop)
         if last:
             fuse_loss = train and worker.fuse_loss and (lp.loss == "mse" or ks.cols <= 32)
             if fuse_loss:

@@ -361,10 +361,10 @@ def test_train_contiguous_native_loop_tracks_oracle(partition, served, monkeypat
     master.close()
 
 
-def test_fused_dropout_mask_statistics_and_gradients():
-    """K13: tf.nn.dropout after a dense layer runs inside the compiled plan (Philox mask in the GEMM epilogue).  The mask
-    is recovered from the stored activation; forward statistics and every gradient are checked against PyTorch given
-    that observed mask (reference semantics: keep with prob p, scale by 1/p - tf.nn.dropout; ml_util.py:70-71)."""
+def test_fused_dropout_mask_statistics():
+    """K13: tf.nn.dropout after a dense layer runs inside the compiled plan (Philox mask in the GEMM epilogue).  The
+    statistics of the mask recovered from the stored activation (reference semantics: keep with prob p, scale by 1/p -
+    tf.nn.dropout; ml_util.py:70-71).  The exact mask and the gradients are checked in test_gpu_dropout.py."""
     from sparkflow_b200.graph import tfcompat as tf
     from sparkflow_b200.graph_utils import build_graph
 
@@ -418,19 +418,4 @@ def test_fused_dropout_mask_statistics_and_gradients():
     assert torch.allclose(a2[big & (m2 > 0)], h2[big & (m2 > 0)] / 0.75, rtol=3e-2, atol=3e-2)
     # the two layers' masks are different streams, rows differ, columns differ
     assert (m1[0] != m1[1]).any() and (m1[:, 0] != m1[:, 1]).any()
-    # ---- gradients given the observed masks (autograd on the same computation) ----
-    Wt = [w.clone().requires_grad_(True) for w in W]
-    xh = xb
-    z1 = torch.relu(xh @ Wt[0] + Wt[1]) * m1 * 2.0
-    z2 = torch.tanh(z1.to(torch.bfloat16).float() @ Wt[2] + Wt[3]) * m2 / 0.75
-    logits = z2.to(torch.bfloat16).float() @ Wt[4] + Wt[5]
-    loss = -(torch.from_numpy(Y) * torch.log_softmax(logits, 1)).sum(1).mean()
-    loss.backward()
-    got = lay.unflatten(worker.grads.cpu().numpy())
-    for g, w, v in zip(got, Wt, ir.trainable):
-        ref = w.grad.numpy()
-        scale = max(np.abs(ref).max(), 1e-6)
-        assert np.abs(g - ref).max() < 6e-2 * scale, (v.name, np.abs(g - ref).max(), scale)
-    assert abs(float(worker.loss_acc.cpu()[0]) - float(loss)) < 2e-2 * max(1.0, float(loss))
-    # a second step draws a different mask only when the step counter moves: without a push the counter is unchanged
     master.close()

@@ -13,13 +13,16 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from sparkflow_b200.graph import tfcompat as tf
 from sparkflow_b200.graph.executor import GraphProgram
 from sparkflow_b200.graph.ir import GraphIR
+from sparkflow_b200.graph_utils import build_graph
 from sparkflow_b200.models import zoo
 from sparkflow_b200.models.compiler import UnsupportedGraph, compile_graph
 from sparkflow_b200.ops.layout import ParamLayout
 from sparkflow_b200.ops.optimizers import OptimizerSpec
 from sparkflow_b200.parallel.plan_builder import check_grammar, fused_first_conv, use_mn_possible
+from dropout_ref import dropout_mask
 from push_helpers import wait_pushes
 
 DEV = torch.device("cuda:0") if torch.cuda.is_available() else torch.device("cpu")
@@ -39,6 +42,44 @@ MODELS = {
 }
 DENSE = [m for m in MODELS if not m.startswith("cnn")]
 CNNS = [m for m in MODELS if m.startswith("cnn")]
+
+
+def _mlp_drop():
+    """a dropout after every hidden layer, one per activation kind and keep probability, through both TF spellings"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    kp = tf.placeholder_with_default(0.5, shape=[], name="keep_prob")
+    h = tf.nn.dropout(tf.layers.dense(x, 300, activation=tf.nn.relu), keep_prob=kp)
+    h = tf.layers.dropout(tf.layers.dense(h, 130, activation=tf.nn.tanh), rate=0.25, training=True)
+    h = tf.nn.dropout(tf.layers.dense(h, 70, activation=tf.nn.sigmoid), keep_prob=0.9)
+    h = tf.nn.dropout(tf.layers.dense(h, 40), keep_prob=0.6)
+    logits = tf.layers.dense(h, 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def _ae_drop():
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    code = tf.nn.dropout(tf.layers.dense(x, 200, activation=tf.nn.sigmoid), keep_prob=0.8)
+    rec = tf.layers.dense(code, 784, activation=tf.nn.sigmoid)
+    return tf.losses.mean_squared_error(rec, x)
+
+
+def _cnn_drop():
+    """cnn_same with TensorFlow's "Deep MNIST" dropout (keep 0.5) on its 1024-unit layer"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    c1 = tf.layers.max_pooling2d(tf.layers.conv2d(img, 32, 5, padding="same", activation=tf.nn.relu), 2, 2, padding="same")
+    c2 = tf.layers.max_pooling2d(tf.layers.conv2d(c1, 64, 5, padding="same", activation=tf.nn.relu), 2, 2, padding="same")
+    h = tf.nn.dropout(tf.layers.dense(tf.layers.flatten(c2), 1024, activation=tf.nn.relu), keep_prob=0.5)
+    logits = tf.layers.dense(h, 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+# graphs with dropout, built here rather than in the zoo: name -> (graph function, label kind)
+DROP_MODELS = {"mlp_drop": (_mlp_drop, "onehot"), "ae_drop": (_ae_drop, None), "cnn_drop": (_cnn_drop, "onehot")}
 # B = 1, odd, one past a 128-row tile; for the CNNs these also switch the split-K conv weight gradient off and on
 DENSE_B = (1, 7, 129, 300, 1000)
 CNN_B = (1, 7, 130, 300)
@@ -73,9 +114,16 @@ TOL = {                                  # measured: per-step test; delivered-gr
     "cnn": (7e-4, 2.5e-3),               # 2.2e-4, 7.6e-4
     "cnn_same": (2.5e-3, 7e-3),          # 7.8e-4, 2.1e-3
     "cnn_strided": (6e-4, 1.5e-3),       # 1.8e-4, 4.8e-4; 4.2e-4, 9.7e-4
+    # dropout graphs (tests/test_gpu_dropout.py): the stored activations match the oracle's bit for bit up to the same
+    # one-step bf16 roundings, but 1 / keep scales them up and a small batch (B = 7) carries a rounding step of layer 0
+    # into every later layer
+    "mlp_drop": (8e-3, 1.6e-2),          # 2.7e-3, 5.2e-3
+    "ae_drop": (5e-4, 2e-3),             # 1.7e-4, 6.6e-4
+    "cnn_drop": (2.5e-3, 4e-3),          # 7.7e-4, 1.3e-3
 }
 FWD_TOL = (1e-3, 4e-3)                   # predict output; measured 2.7e-4, 1.2e-3
 LOSS_TOL = 5e-5                          # relative; measured 1.3e-5
+DROP_LOSS_TOL = {"mlp_drop": 9e-4, "ae_drop": LOSS_TOL, "cnn_drop": LOSS_TOL}    # measured 2.9e-4, 7.2e-7, 4.9e-6
 # what the push delivery (mailbox, routed tiles, forwarded tails) may add to the step's own gradient: the run-to-run
 # spread of the atomically accumulated bias and split-K gradients (relative Frobenius; measured 2.2e-6, cnn_strided)
 DELIVERY_TOL = 1e-5
@@ -91,8 +139,12 @@ _MODEL_CACHE = {}
 def _model(name):
     """(GraphIR, LayerPlan, label tensor name or None)"""
     if name not in _MODEL_CACHE:
-        kw, kind = MODELS[name]
-        ir = GraphIR.from_metagraph(zoo.build(name, **kw))
+        if name in DROP_MODELS:
+            fn, kind = DROP_MODELS[name]
+            ir = GraphIR.from_metagraph(build_graph(fn))
+        else:
+            kw, kind = MODELS[name]
+            ir = GraphIR.from_metagraph(zoo.build(name, **kw))
         label = "y:0" if kind else None
         _MODEL_CACHE[name] = (ir, compile_graph(ir, "x:0", label), label)
     return _MODEL_CACHE[name]
@@ -100,7 +152,7 @@ def _model(name):
 
 def _data(name, n, seed):
     _, lp, _ = _model(name)
-    kind = MODELS[name][1]
+    kind = (DROP_MODELS if name in DROP_MODELS else MODELS)[name][1]
     rng = np.random.default_rng(seed)
     X = rng.random((n, lp.input_dim), dtype=np.float32)
     if kind == "onehot":
@@ -172,6 +224,30 @@ class _StoreAct(torch.autograd.Function):
         return g * (a if ctx.masked else _dact(a, ctx.act)), None, None
 
 
+def _drop_dact(a, act, keep):
+    """d(stored a) / dz of a kept unit of a dropout layer, from its stored value a = act(z) / keep: the backward kernel
+    takes act' at a * keep and scales by 1 / keep"""
+    return _dact(a * keep, act) / keep
+
+
+class _StoreDrop(torch.autograd.Function):
+    """act(z) * mask / keep stored in bf16 (a fused dropout).  No mask is stored: the backward kernel recovers it from
+    the stored value (a != 0) and takes g * mask / keep * act'(a * keep), or, for a ReLU, uses the step's recorded
+    ``active`` units."""
+
+    @staticmethod
+    def forward(ctx, z, act, keep, mask, active):
+        a = _bf16(_ACT[act](z) * mask / keep)
+        d = active.to(a.dtype) / keep if active is not None else _drop_dact(a, act, keep)
+        ctx.save_for_backward(d * mask)
+        return a
+
+    @staticmethod
+    def backward(ctx, g):
+        (d,) = ctx.saved_tensors
+        return g * d, None, None, None, None
+
+
 def _conv(x, w, l, rg):
     """NHWC conv with TF geometry as pad + im2col (unfold) + GEMM; ``rg`` marks the bf16 gradient stores: the col2im
     output (wrt x) and dpatch (wrt the patch matrix)."""
@@ -228,28 +304,41 @@ def _pool_gather(a, l, idx):
     return a.reshape(B, H * W, C).gather(1, flat).reshape(B, oh, ow, C)
 
 
-def _forward(lp, weights, X, Y, emulate_bf16, argmax=None, relu_mask=None, device=DEV):
+def _forward(lp, weights, X, Y, emulate_bf16, argmax=None, relu_mask=None, drop_mask=None, device=DEV):
     """float64 forward pass of the layer plan.  Returns (loss, network output, parameter leaves, pools, pre-activations)
     with pools = {pool layer: (activation it pooled, winner index)} and pre-activations = {dense layer: z}.
-    ``relu_mask``: {layer: units the step found active}, see ``oracle``."""
-    argmax, relu_mask = argmax or {}, relu_mask or {}
+    ``relu_mask``: {layer: units the step found active}, ``drop_mask``: {dropout layer: kept units}, see ``oracle``."""
+    argmax, relu_mask, drop_mask = argmax or {}, relu_mask or {}, drop_mask or {}
     em = emulate_bf16
     # straight through: the rounded value forward, the float64 gradient back (autograd of a cast to bf16 would round it)
     bf = (lambda t: t + (_bf16(t) - t).detach()) if em else (lambda t: t)
     rg = _RoundGrad.apply if em else (lambda t: t)
 
-    def store(z, act, layer, mag):
-        """``mag``: sum of the magnitudes of the terms of z, the scale of its fp32 accumulation error"""
+    def store(z, act, layer, mag, keep=0.0):
+        """``mag``: sum of the magnitudes of the terms of z, the scale of its fp32 accumulation error; ``keep``: keep
+        probability of the layer's dropout (0: none)"""
+        kept = None
+        if keep:
+            if layer not in drop_mask:
+                raise ValueError(f"layer {layer} has a dropout: its mask must be given")
+            kept = torch.as_tensor(np.asarray(drop_mask[layer]), device=z.device).to(torch.bool)
+            assert kept.shape == z.shape, (layer, kept.shape, z.shape)
         if not em:
-            return _ACT[act](z)
+            a = _ACT[act](z)
+            return a if kept is None else a / keep * kept.to(a.dtype)         # tf.nn.dropout: x / keep * floor(keep + U)
         mask = relu_mask.get(layer) if act == "Relu" else None
         if mask is not None:
             # the step may only disagree on a unit whose pre-activation is zero up to the tensor cores' fp32 accumulation
-            # (and a bf16 input one rounding step apart); a wrong unit would sit near |z| ~ sum|terms| / sqrt(K)
+            # (and a bf16 input one rounding step apart); a wrong unit would sit near |z| ~ sum|terms| / sqrt(K).  A unit
+            # the dropout removed stores 0 whatever its pre-activation: the step's record says nothing about it.
             zd = z.detach()
             off = mask != (zd > 0)
+            if kept is not None:
+                off &= kept
             ratio = float((zd[off].abs() / mag[off]).max()) if bool(off.any()) else 0.0
             assert ratio <= 1e-3, f"layer {layer}: the step's ReLU mask disagrees where |z| = {ratio:.1e} x its sum of |terms|"
+        if kept is not None:
+            return _StoreDrop.apply(z, act, keep, kept.to(z.dtype), mask)
         return _StoreAct.apply(z, act, mask)
 
     def magnitude(h, w, b, l):
@@ -307,7 +396,7 @@ def _forward(lp, weights, X, Y, emulate_bf16, argmax=None, relu_mask=None, devic
             z = z + b
         zs[i] = z.detach()
         if i != last:
-            h = store(z, l.act, i, magnitude(h, w, b, l))
+            h = store(z, l.act, i, magnitude(h, w, b, l), l.dropout_keep)
             continue
         if lp.loss == "softmax_xent":
             out = z
@@ -326,7 +415,7 @@ def _grads(loss, params):
     return [(g if g is not None else torch.zeros_like(p)).detach().cpu().numpy() for g, p in zip(gs, params)]
 
 
-def oracle(lp, weights, X, Y, emulate_bf16, argmax=None, relu_mask=None):
+def oracle(lp, weights, X, Y, emulate_bf16, argmax=None, relu_mask=None, drop_mask=None):
     """Loss and the gradient of every trainable variable (``ir.trainable`` order) of one step on rows X / labels Y,
     computed by autograd in float64.
 
@@ -336,8 +425,10 @@ def oracle(lp, weights, X, Y, emulate_bf16, argmax=None, relu_mask=None):
     winner index [B, oh, ow, C]} recorded by the step's pooling kernels, so max-pool ties resolve as the kernels did.
     ``relu_mask``: {dense / conv layer: bool tensor of its output}, the ReLU units the step found active, so a
     pre-activation within rounding of zero switches the unit as it did in the step (checked to be the only
-    disagreement)."""
-    loss, _, params, _, _ = _forward(lp, weights, X, Y, emulate_bf16, argmax, relu_mask)
+    disagreement).  ``drop_mask``: {dense layer with a dropout: bool [B, N] of the units it keeps}, required for every
+    such layer; the layer computes act(z) / keep * mask as tf.nn.dropout does, and with ``emulate_bf16`` stores it in
+    bf16 and differentiates it as the backward kernel does (``_StoreDrop``)."""
+    loss, _, params, _, _ = _forward(lp, weights, X, Y, emulate_bf16, argmax, relu_mask, drop_mask)
     return float(loss.detach()), _grads(loss, params)
 
 
@@ -461,6 +552,82 @@ def test_tolerances_reject_plausible_gradient_bugs(name, B):
         assert _rejects(grads, ref, tol), f"{name} B={B}: the tolerance {tol} accepts the gradient {what}"
 
 
+def host_drop_masks(lp, B, seed, ctr, streams=None):
+    """{dense layer with a dropout: kept units [B, N]} of a step whose plan uses ``seed`` and step counter ``ctr``; the
+    stream of layer i is i (plan_builder), or ``streams[i]``"""
+    streams = streams or {}
+    return {i: dropout_mask(B, l.out_shape[0], np.float32(l.dropout_keep), seed, streams.get(i, i), ctr)
+            for i, l in enumerate(lp.layers) if l.kind == "dense" and l.dropout_keep}
+
+
+def _random_uniform_tensor(ir, l):
+    """the RandomUniform output of the tf.nn.dropout sub-graph on layer ``l``'s output"""
+    scope = l.tensors["dropout"].split(":")[0].rsplit("/", 1)[0]
+    name = f"{scope}/random_uniform/RandomUniform"
+    assert ir.nodes[name].op == "RandomUniform", name
+    return name + ":0"
+
+
+@pytest.mark.parametrize("name", list(DROP_MODELS))
+def test_dropout_oracle_matches_interpreter(name):
+    """The exact oracle with a dropout mask against the interpreter running the graph's own tf.nn.dropout /
+    tf.layers.dropout sub-graphs, their RandomUniform fed 0.999 where the mask keeps a unit and 0 where it drops it
+    (floor(keep + u) is then the mask)."""
+    ir, lp, label = _model(name)
+    B = 7
+    X, Y = _data(name, B, seed=3)
+    w = _weights(name)
+
+    def run_both(masks):
+        feeds = {"x:0": X}
+        if label:
+            feeds[label] = Y
+        for i, m in masks.items():
+            feeds[_random_uniform_tensor(ir, lp.layers[i])] = np.where(m, 0.999, 0.0).astype(np.float32)
+        l_int, g_int = GraphProgram(ir).loss_and_grads(feeds, w)
+        l_ora, g_ora = oracle(lp, w, X, Y, emulate_bf16=False, drop_mask=masks)
+        assert abs(l_ora - l_int) <= 1e-5 * max(1.0, abs(l_int)), (l_ora, l_int)
+        _assert_grads(f"{name} exact oracle vs interpreter", lp.var_order, g_ora, [g.numpy() for g in g_int], (1e-4, 1e-4))
+        return g_ora
+
+    masks = host_drop_masks(lp, B, 0x5EED, 3)
+    assert masks and all(0 < m.mean() < 1 for m in masks.values())
+    g = run_both(masks)
+    g_other = run_both(host_drop_masks(lp, B, 0x5EED, 4))
+    assert _rejects(g_other, g, TOL[name]), "the mask does not reach the gradient"
+
+
+@pytest.mark.parametrize("B", [7, 129])
+@pytest.mark.parametrize("name", list(DROP_MODELS))
+def test_tolerances_reject_dropout_bugs(name, B, monkeypatch):
+    """The per-step comparison rejects the oracle's gradient computed with a dropout fault the step could have, one layer
+    at a time: (a) the mask of the previous step counter, (b) the mask of another layer's stream; and in the backward of
+    every dropout layer: (c) no 1 / keep, (d) act' taken at the stored a instead of a * keep (tanh / sigmoid layers)."""
+    _, lp, _ = _model(name)
+    X, Y = _data(name, B, seed=11)
+    w = _weights(name)
+    seed, ctr = 0x2468ACE, 7
+    masks = host_drop_masks(lp, B, seed, ctr)
+    _, ref = oracle(lp, w, X, Y, emulate_bf16=True, drop_mask=masks)
+    tol = TOL[name]
+    assert not _rejects(ref, ref, tol)
+    mutants = {}
+    for i in masks:
+        prev = {**masks, i: host_drop_masks(lp, B, seed, ctr - 1)[i]}
+        mutants[f"with layer {i}'s mask of the previous counter"] = oracle(lp, w, X, Y, True, drop_mask=prev)[1]
+        other = {**masks, i: host_drop_masks(lp, B, seed, ctr, streams={i: i + 1})[i]}
+        mutants[f"with layer {i}'s mask of stream {i + 1}"] = oracle(lp, w, X, Y, True, drop_mask=other)[1]
+    faults = {"without 1 / keep in the backward": lambda a, act, keep: _dact(a * keep, act)}
+    if any(lp.layers[i].act in ("Tanh", "Sigmoid") for i in masks):
+        faults["with act' taken at the stored a"] = lambda a, act, keep: _dact(a, act) / keep
+    for what, fn in faults.items():
+        with monkeypatch.context() as m:
+            m.setitem(globals(), "_drop_dact", fn)
+            mutants[what] = oracle(lp, w, X, Y, True, drop_mask=masks)[1]
+    for what, grads in mutants.items():
+        assert _rejects(grads, ref, tol), f"{name} B={B}: the tolerance {tol} accepts the gradient {what}"
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # GPU tier: the native step
 # ------------------------------------------------------------------------------------------------------------------
@@ -528,7 +695,8 @@ def _recorded_argmax(lp, dbg, B):
 
 def _recorded_relu_mask(lp, dbg, B):
     """{layer: active ReLU units} as the step stored them: the next dense layer's input, the conv output, or the fused
-    first conv's pooled output"""
+    first conv's pooled output.  Behind a dropout the stored input is 0 at every dropped unit, active or not: the oracle
+    only checks this record on the units the dropout keeps."""
     out = {}
     dense = [i for i, l in enumerate(lp.layers) if l.kind == "dense"]
     for i, l in enumerate(lp.layers):
@@ -560,15 +728,16 @@ def _check_pools(tag, lp, dbg, pools, B):
             assert torch.equal(_pool_gather(act, l, idx), r["pooled"].to(DEV).double().reshape(B, *l.out_shape)), tag
 
 
-def _compare_step(tag, lp, w, X, Y, got, loss, dbg, tol):
+def _compare_step(tag, lp, w, X, Y, got, loss, dbg, tol, drop_mask=None, loss_tol=LOSS_TOL):
     B = X.shape[0]
     assert np.isfinite(loss), f"{tag}: loss {loss}"
-    l_ref, out, params, pools, _ = _forward(lp, w, X, Y, True, _recorded_argmax(lp, dbg, B), _recorded_relu_mask(lp, dbg, B))
+    l_ref, out, params, pools, _ = _forward(lp, w, X, Y, True, _recorded_argmax(lp, dbg, B), _recorded_relu_mask(lp, dbg, B),
+                                            drop_mask)
     _check_pools(tag, lp, dbg, pools, B)
     ref = _grads(l_ref, params)
     l_ref = float(l_ref.detach())
     l_err = abs(loss - l_ref) / max(abs(l_ref), 1e-30)
-    assert l_err <= LOSS_TOL, f"{tag}: loss {loss} vs {l_ref} (relative error {l_err:.2e})"
+    assert l_err <= loss_tol, f"{tag}: loss {loss} vs {l_ref} (relative error {l_err:.2e})"
     fro, mx = _assert_grads(tag, lp.var_order, got, ref, tol)
     print(f"[step-grad] {tag}: rel-Frobenius {fro:.2e} max-abs {mx:.2e} loss {l_err:.2e}")
     return fro, mx, l_err
