@@ -1,6 +1,6 @@
 // Elementwise / reduction kernels of the training step that are not GEMMs:
-// input cast+transpose (K11 feeder), softmax-cross-entropy (K5), MSE (K6), argmax (K7).
-// Reference semantics: tf.losses.softmax_cross_entropy / mean_squared_error with the default
+// input cast+transpose (K11 feeder), softmax-cross-entropy (K5), MSE and sigmoid-cross-entropy (K6), argmax (K7).
+// Reference semantics: tf.losses.softmax_cross_entropy / mean_squared_error / sigmoid_cross_entropy with the default
 // SUM_BY_NONZERO_WEIGHTS reduction (examples/simple_dnn.py:20, autoencoder_example.py:15).
 #include "sm90_ptx.cuh"
 #include "sf_api.h"
@@ -129,12 +129,38 @@ softmax_xent_kernel(const float* __restrict__ logits, int ld_logits, const float
 }
 
 // ---------------------------------------------------------------------------
-// MSE over all elements (32x32 tiles; transposed store through smem; column sums for dbias).
+// Element-wise losses over all elements (32x32 tiles; transposed store through smem; column sums for dbias).  The
+// head maps (network output o, target t) to a loss term and dz:
+//   MseHead          loss += mean((o - t)^2), dz = 2 (o - t) / (rows * cols) * act'(o)   (o after activation `act`)
+//   SigmoidXentHead  loss += mean(max(o, 0) - o t + log1p(exp(-|o|))), dz = (sigmoid(o) - t) / (rows * cols)  (raw logits)
 // ---------------------------------------------------------------------------
+struct MseHead {
+  static constexpr int kKid = KID_MSE;
+  __device__ static float scale(int rows, int cols) { return 2.f / (static_cast<float>(rows) * static_cast<float>(cols)); }
+  __device__ static float grad(float o, float t, int act, float scale, float& lacc) {
+    const float d = o - t;
+    lacc += d * d;
+    return d * scale * dact_from_out(o, act);
+  }
+  __device__ static float loss(float sum, float scale) { return sum * 0.5f * scale; }
+};
+
+struct SigmoidXentHead {
+  static constexpr int kKid = KID_SIGMOID_XENT;
+  __device__ static float scale(int rows, int cols) { return 1.f / (static_cast<float>(rows) * static_cast<float>(cols)); }
+  __device__ static float grad(float o, float t, int, float scale, float& lacc) {
+    float g;
+    lacc += sigmoid_xent_elem(o, t, g);
+    return g * scale;
+  }
+  __device__ static float loss(float sum, float scale) { return sum * scale; }
+};
+
+template <class Head>
 __global__ void __launch_bounds__(256)
-mse_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ target, int ld_target,
-           int act, float* __restrict__ loss, __nv_bfloat16* __restrict__ dz, int ld_dz,
-           __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias, int rows, int cols) {
+elementwise_loss_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ target, int ld_target,
+                        int act, float* __restrict__ loss, __nv_bfloat16* __restrict__ dz, int ld_dz,
+                        __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias, int rows, int cols) {
   __shared__ float tile[32][33];
   __shared__ float s_col[32];
   __shared__ float s_loss[8];
@@ -146,18 +172,14 @@ mse_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ 
   const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
   if (threadIdx.x < 32) s_col[threadIdx.x] = 0.f;
   __syncthreads();
-  const float scale = 2.f / (static_cast<float>(rows) * static_cast<float>(cols));
+  const float scale = Head::scale(rows, cols);
   float lacc = 0.f, cacc = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int r = r0 + ty + 8 * i, c = c0 + tx;
     float g = 0.f;
-    if (r < rows && c < cols) {
-      const float o = out[static_cast<size_t>(r) * ld_out + c];
-      const float d = o - target[static_cast<size_t>(r) * ld_target + c];
-      lacc += d * d;
-      g = d * scale * dact_from_out(o, act);
-    }
+    if (r < rows && c < cols)
+      g = Head::grad(out[static_cast<size_t>(r) * ld_out + c], target[static_cast<size_t>(r) * ld_target + c], act, scale, lacc);
     tile[ty + 8 * i][tx] = g;
     cacc += g;
     if (dz != nullptr && r < rows && c < ld_dz) dz[static_cast<size_t>(r) * ld_dz + c] = __float2bfloat16(g);
@@ -170,7 +192,7 @@ mse_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ 
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += s_loss[i];
-    if (t != 0.f) atomicAdd(loss, t * 0.5f * scale);
+    if (t != 0.f) atomicAdd(loss, Head::loss(t, scale));
   }
   if (dbias && threadIdx.x < 32 && c0 + threadIdx.x < cols && s_col[threadIdx.x] != 0.f)
     atomicAdd(dbias + c0 + threadIdx.x, s_col[threadIdx.x]);
@@ -181,7 +203,7 @@ mse_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ 
       if (c < cols && r < rows) dzT[static_cast<size_t>(c) * ld_t + r] = __float2bfloat16(tile[tx][ty + 8 * i]);
     }
   }
-  trace.end(KID_MSE);
+  trace.end(Head::kKid);
 }
 
 __global__ void __launch_bounds__(256)
@@ -266,13 +288,28 @@ extern "C" int sf_softmax_xent(const float* logits, int ld_logits, const float* 
                                      logits, ld_logits, labels, ld_labels, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
 }
 
+// the grid spans ld_dz columns, so the padded tail of every dz row is written (with zeros)
+template <class Head>
+static int launch_elementwise_loss(const float* out, int ld_out, const float* target, int ld_target, int act, float* loss,
+                                   __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t, float* dbias, int rows, int cols,
+                                   cudaStream_t st) {
+  const int span_c = (dz && ld_dz > cols) ? ld_dz : cols;
+  dim3 grid((span_c + 31) / 32, (rows + 31) / 32);
+  return static_cast<int>(sf::launch(sf::elementwise_loss_kernel<Head>, grid, dim3(256), 0, st, out, ld_out, target, ld_target, act,
+                                     loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
+}
+
 extern "C" int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act,
                            float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                            float* dbias, int rows, int cols, cudaStream_t st) {
-  const int span_c = (dz && ld_dz > cols) ? ld_dz : cols;
-  dim3 grid((span_c + 31) / 32, (rows + 31) / 32);
-  return static_cast<int>(sf::launch(sf::mse_kernel, grid, dim3(256), 0, st, out, ld_out, target, ld_target, act,
-                                     loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
+  return launch_elementwise_loss<sf::MseHead>(out, ld_out, target, ld_target, act, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols, st);
+}
+
+extern "C" int sf_sigmoid_xent(const float* logits, int ld_logits, const float* labels, int ld_labels, float* loss,
+                               __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t, float* dbias, int rows, int cols,
+                               cudaStream_t st) {
+  return launch_elementwise_loss<sf::SigmoidXentHead>(logits, ld_logits, labels, ld_labels, SF_ACT_NONE, loss, dz, ld_dz, dzT, ld_t,
+                                                      dbias, rows, cols, st);
 }
 
 extern "C" int sf_argmax_rows(const float* in, int ld, float* out, int rows, int cols, cudaStream_t st) {

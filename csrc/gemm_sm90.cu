@@ -17,8 +17,9 @@
 //   * fp32 store or atomic accumulate (split-K / straight into the flat gradient buffer that the
 //     push kernel consumes).
 // The generic kernel (sf_gemm_kernel) tests each of these at run time.  The training GEMMs run specialized variants
-// (sf_gemm_epi_kernel, one per SfEpi kind) that contain only their own epilogue code, a fifth to a half of the generic
-// kernel's; the DGRAD / LOSS variants also fetch their act'(aux) / label rows before the main loop.
+// (sf_gemm_epi_kernel, one per SfEpi kind, and sf_gemm_sigmoid_loss_kernel) that contain only their own epilogue code, a
+// fifth to a half of the generic kernel's; the DGRAD / loss variants also fetch their act'(aux) / label rows before the
+// main loop.
 //
 // The B operand may live in *peer* GPU memory: the tensor map simply carries the peer-mapped
 // address, and the TMA engine pulls weight tiles over NVLink while the MMA pipeline runs
@@ -116,13 +117,18 @@ template <int EPI>
 struct EpiFeatures {
   static constexpr bool kGeneric = EPI == SF_EPI_GENERIC || EPI == kEpiPair;
   static constexpr bool kAct = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS;
-  static constexpr bool kLoss = EPI == SF_EPI_GENERIC || EPI == SF_EPI_LOSS;
+  static constexpr bool kLoss = EPI == SF_EPI_GENERIC || EPI == SF_EPI_LOSS;                  // softmax-CE / MSE heads
+  // sigmoid-CE head: only in its own variant, which therefore also carries the transposed bf16 output and the fused
+  // read-your-writes wait that otherwise only the generic kernel has (so the generic kernel stays as it was)
+  static constexpr bool kSigmoidLoss = EPI == SF_EPI_SIGMOID_LOSS;
+  static constexpr bool kOutT = kGeneric || EPI == SF_EPI_SIGMOID_LOSS;
+  static constexpr bool kRyw = kGeneric || EPI == SF_EPI_SIGMOID_LOSS;
   static constexpr bool kAux = kGeneric || EPI == SF_EPI_DGRAD;
-  static constexpr bool kColsum = kGeneric || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD;
+  static constexpr bool kColsum = kGeneric || EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_DGRAD;
   static constexpr bool kF32 = kGeneric || EPI == SF_EPI_WGRAD;
-  static constexpr bool kBf16 = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD;
+  static constexpr bool kBf16 = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_DGRAD;
   // the thread's act'(aux) chunk / label row are fetched before the main loop (epi_prefetch)
-  static constexpr bool kPrefetch = EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD;
+  static constexpr bool kPrefetch = EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_DGRAD;
 };
 
 // One 32-column chunk of a thread's output row: everything between the accumulator (v, already in registers) and
@@ -201,6 +207,19 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) lrow += __shfl_xor_sync(0xffffffffu, lrow, o);
       if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow * 0.5f * scale);
+    } else if (F::kSigmoidLoss && ep.loss_mode == SF_LOSS_SIGMOID_XENT) {
+      // f holds raw logits (the host rejects an activation); the caller fetched the chunk's labels
+      const float scale = __fdividef(1.f, static_cast<float>(M) * static_cast<float>(N));
+      float lrow = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        float g = 0.f;
+        if (row_ok && col0 + j < N) lrow += sigmoid_xent_elem(f[j], tgt_pref[j], g);
+        f[j] = g * scale;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) lrow += __shfl_xor_sync(0xffffffffu, lrow, o);
+      if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow * scale);
     }
     if (tq != nullptr) tq[3] = trace_now();
     if (F::kAux && (!F::kGeneric || ep.aux != nullptr) && row_ok) {
@@ -287,7 +306,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
       }
     }
     if (tq != nullptr) tq[7] = trace_now();
-    if (F::kGeneric && ep.outT_bf16 != nullptr && row_ok) {
+    if (F::kOutT && ep.outT_bf16 != nullptr && row_ok) {
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (col0 + j < N)
@@ -444,7 +463,7 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
   // successors launch when it completes) - they must not sit on SMs that the shard applier whose acknowledgement it
   // waits for needs for its own CTAs.  A grid of several waves triggers at entry: its successor's CTAs only get SMs as
   // this grid drains.  A one-wave grid triggers after its main loop, see there.
-  if ((!F::kGeneric || ep.ryw == nullptr) && !ep.one_wave) pdl_launch_dependents();
+  if ((!F::kRyw || ep.ryw == nullptr) && !ep.one_wave) pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * BN;
@@ -471,7 +490,7 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      if (F::kGeneric && ep.ryw != nullptr) {
+      if (F::kRyw && ep.ryw != nullptr) {
         // pull fused into this GEMM: read-your-writes wait before the first weight tile is fetched (local spin)
         const SfRyw& w = *ep.ryw;
         const uint32_t posted = *w.my_posted;
@@ -531,7 +550,7 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
     // One-wave grid: the successor launches once every CTA is past its main loop, so its launch and prologue overlap
     // this epilogue.  A trigger at entry would let a chain of small GEMMs pre-launch in a cascade, and those waiting
     // CTAs (one per SM at this register / shared-memory size, 149 for the push) hold SMs the GEMMs ahead of them need.
-    if ((!F::kGeneric || ep.ryw == nullptr) && ep.one_wave) pdl_launch_dependents();
+    if ((!F::kRyw || ep.ryw == nullptr) && ep.one_wave) pdl_launch_dependents();
     // every stage has been consumed by both warpgroups: the ring holds the staged accumulator tile from here on
     float* stg = reinterpret_cast<float*>(stage_base);
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -563,6 +582,17 @@ sf_gemm_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                    const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
   static_assert(EPI != SF_EPI_GENERIC, "the generic epilogue is sf_gemm_kernel");
   gemm_cta<BN, MN, EPI>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+
+// The sigmoid cross-entropy head (SF_EPI_SIGMOID_LOSS, K-major) runs only here: as a runtime branch of the LOSS variant
+// it raised that variant's register count, and in the generic kernel it added a quarter to the code every generic GEMM
+// of the training step fetches.  It carries what a loss GEMM may need beyond the LOSS variant: the transposed dz of the
+// K-major weight-gradient path and the read-your-writes wait of a network whose only dense layer is the loss layer.
+template <int BN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_sigmoid_loss_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                            const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  gemm_cta<BN, false, SF_EPI_SIGMOID_LOSS>(tmA, tmB, ep, M, N, K, kblocks_per_split);
 }
 
 // ---------------------------------------------------------------------------
@@ -634,6 +664,12 @@ static int pick_epi(const SfGemm* g) {
   const SfGemmEpilogue& e = g->ep;
   const bool dropout = e.drop_keep > 0.f && e.drop_keep < 1.f;
   const bool aux_dropout = e.aux_keep > 0.f && e.aux_keep < 1.f;
+  if (e.loss_mode == SF_LOSS_SIGMOID_XENT) {
+    // the sigmoid head exists only in its own variant: K-major, BN 32 / 64, raw logits, bf16 dz (+ transpose)
+    const bool ok = !g->pair && !g->mn_major && !dropout && e.route == nullptr && e.aux == nullptr && e.out_f32 == nullptr &&
+                    e.out_bf16 != nullptr && e.act == SF_ACT_NONE && (g->bn == 32 || g->bn == 64);
+    return ok ? SF_EPI_SIGMOID_LOSS : SF_EPI_GENERIC;
+  }
   if (g->pair || dropout || e.route != nullptr || e.ryw != nullptr || e.outT_bf16 != nullptr) return SF_EPI_GENERIC;
   if (g->mn_major) {
     const bool wgrad = (g->bn == 64 || g->bn == 128) && e.out_f32 != nullptr && e.out_bf16 == nullptr && e.aux == nullptr &&
@@ -648,7 +684,9 @@ static int pick_epi(const SfGemm* g) {
 
 extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return -2;
+  if (g->ep.loss_mode < SF_LOSS_NONE || g->ep.loss_mode > SF_LOSS_SIGMOID_XENT) return -5;
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
+  if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->bn > 64) g->bn = 64;    // the widest tile of its variant
   if (g->split_k <= 0) g->split_k = 1;
   // large, un-split problems go to the persistent cluster-pair kernel (gemm_pair_sm90.cu): 256 x 128 tiles per CTA pair
   {
@@ -693,6 +731,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   g->ep.n_store_limit = lim;
   g->ep.one_wave = static_cast<long long>((g->N + g->bn - 1) / g->bn) * ((g->M + sf::kBM - 1) / sf::kBM) * g->split_k <= sf_num_sms();
   g->epi = g->epi == SF_EPI_GENERIC ? SF_EPI_GENERIC : pick_epi(g);
+  if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->epi != SF_EPI_SIGMOID_LOSS) return -5;
   return 0;
 }
 
@@ -701,6 +740,7 @@ static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
   using S = sf::GemmSmem<BN>;
   auto kernel = [] {
     if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
+    else if constexpr (EPI == SF_EPI_SIGMOID_LOSS) return sf::sf_gemm_sigmoid_loss_kernel<BN>;
     else return sf::sf_gemm_epi_kernel<BN, MN, EPI>;
   }();
   static bool attr_set = false;
@@ -728,6 +768,7 @@ extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
     case SF_EPI_FWD: return static_cast<int>(launch_kmajor_variant<SF_EPI_FWD>(g, st));
     case SF_EPI_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_LOSS>(g, st));
     case SF_EPI_DGRAD: return static_cast<int>(launch_kmajor_variant<SF_EPI_DGRAD>(g, st));
+    case SF_EPI_SIGMOID_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_SIGMOID_LOSS>(g, st));
     case SF_EPI_WGRAD:
       e = g->bn == 64 ? launch_bn<64, true, SF_EPI_WGRAD>(g, st) : launch_bn<128, true, SF_EPI_WGRAD>(g, st);
       return static_cast<int>(e);

@@ -941,6 +941,15 @@ PYBIND11_MODULE(_C, m) {
                                   P<float>(dbias), rows, cols, st);
              });
            })
+      .def("add_sigmoid_xent",
+           [](Plan& p, uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss,
+              uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
+             p.add("sigmoid_xent", [=](cudaStream_t st) {
+               return sf_sigmoid_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels,
+                                      P<float>(loss), P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t,
+                                      P<float>(dbias), rows, cols, st);
+             });
+           })
       .def("add_argmax",
            [](Plan& p, uintptr_t in, int ld, uintptr_t out, int rows, int cols) {
              p.add("argmax", [=](cudaStream_t st) {
@@ -1105,6 +1114,14 @@ PYBIND11_MODULE(_C, m) {
                       P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols,
                       S(stream)),
           "mse_loss");
+  });
+  m.def("sigmoid_xent", [](uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss,
+                           uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols,
+                           uintptr_t stream) {
+    ck_rc(sf_sigmoid_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss),
+                          P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols,
+                          S(stream)),
+          "sigmoid_xent");
   });
   m.def("argmax_rows", [](uintptr_t in, int ld, uintptr_t out, int rows, int cols, uintptr_t stream) {
     ck_rc(sf_argmax_rows(P<const float>(in), ld, P<float>(out), rows, cols, S(stream)), "argmax_rows");

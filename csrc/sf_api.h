@@ -64,7 +64,8 @@ struct SfGemmEpilogue {
   int a_evict_first;
   // fused loss (last dense layer): the epilogue turns the activation into dL/dz in registers, so
   // out_bf16 / outT_bf16 / colsum receive dz, dz^T and the bias gradient directly.
-  int loss_mode;                  // 0 none, 1 softmax cross-entropy (N <= 32), 2 mean squared error
+  int loss_mode;                  // SfLossMode: 0 none, 1 softmax cross-entropy (N <= 32), 2 mean squared error,
+                                  // 3 sigmoid cross-entropy (raw logits, any N)
   const float* target;            // [M, ld_target] labels (one-hot / soft) or regression targets
   int ld_target;
   float* loss;                    // scalar accumulator (mean loss)
@@ -89,7 +90,7 @@ struct SfGemmEpilogue {
   const SfRyw* ryw;               // device memory; nullptr = no wait
 };
 
-enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2 };
+enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, SF_LOSS_SIGMOID_XENT = 3 };
 
 // Epilogue variant of the one-CTA GEMM kernel.  The generic kernel carries every epilogue feature behind runtime tests;
 // each specialized variant compiles in only the features of one kind of training GEMM (sf_gemm_prepare picks it):
@@ -97,7 +98,9 @@ enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2 };
 //   LOSS  bias (+ activation) + softmax-CE / MSE head -> dz bf16, loss, optional column sum
 //   DGRAD act'(aux) -> bf16, optional column sum
 //   WGRAD fp32 store or atomic accumulate (MN-major operands)
-enum SfEpi { SF_EPI_GENERIC = 0, SF_EPI_FWD = 1, SF_EPI_LOSS = 2, SF_EPI_DGRAD = 3, SF_EPI_WGRAD = 4 };
+//   SIGMOID_LOSS  bias + sigmoid-CE head on raw logits -> dz bf16 (+ transpose), loss, optional column sum, optional
+//                 read-your-writes wait; the only kernel with this head (the generic kernel has none)
+enum SfEpi { SF_EPI_GENERIC = 0, SF_EPI_FWD = 1, SF_EPI_LOSS = 2, SF_EPI_DGRAD = 3, SF_EPI_WGRAD = 4, SF_EPI_SIGMOID_LOSS = 5 };
 
 
 struct SfGemm {
@@ -154,6 +157,11 @@ int sf_softmax_xent(const float* logits, int ld_logits, const float* labels, int
 int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act,
                 float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                 float* dbias, int rows, int cols, cudaStream_t st);
+// sigmoid cross-entropy of raw logits z against labels y in [0, 1] over all elements:
+// loss += mean(max(z, 0) - z * y + log1p(exp(-|z|))); dz = (sigmoid(z) - y) / (rows * cols)
+int sf_sigmoid_xent(const float* logits, int ld_logits, const float* labels, int ld_labels, float* loss,
+                    __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t, float* dbias, int rows, int cols,
+                    cudaStream_t st);
 int sf_argmax_rows(const float* in, int ld, float* out, int rows, int cols, cudaStream_t st);
 int sf_fill_zero(void* p, size_t bytes, cudaStream_t st);
 

@@ -45,7 +45,7 @@ __device__ unsigned int g_trace_n = 0;
 
 enum KernelId { KID_GEMM = 1, KID_CAST = 2, KID_SOFTMAX = 3, KID_MSE = 4, KID_ARGMAX = 5, KID_PUSH = 6, KID_PULL = 7,
                 KID_IM2COL = 8, KID_COL2IM = 9, KID_POOL_FWD = 10, KID_POOL_BWD = 11, KID_POOL_GEN_FWD = 12, KID_POOL_GEN_BWD = 13,
-                KID_ACT_BWD = 14,
+                KID_ACT_BWD = 14, KID_SIGMOID_XENT = 15,
                 // phase stamps (ids 100 and up): one extra record of three stamps in t0 / t1 / t2
                 KID_PUSH_LEAD = 106,      // push, block 0: grant seen, gradient loads returned, optimizer math done
                 KID_PUSH_TAIL = 107 };    // push, last CTA: stores issued, done-counter arrival returned, tail done
@@ -437,6 +437,17 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
     k.y += 0xBB67AE85u;
   }
   return c;
+}
+
+// Sigmoid cross-entropy of one raw logit z against label y (tf.nn.sigmoid_cross_entropy_with_logits), shared by the
+// fused-loss GEMM epilogue and the stand-alone loss kernel: returns max(z, 0) - z y + log1p(e) and sets g = sigmoid(z) - y,
+// with e = exp(-|z|) <= 1 on both sides of 0.  log1pf, not log(1 + e): 1 + e rounds to 1 for |z| > 17, which would drop
+// the loss of every saturated element.
+__device__ __forceinline__ float sigmoid_xent_elem(float z, float y, float& g) {
+  const float e = __expf(-fabsf(z));
+  const float r = __fdividef(1.f, 1.f + e);
+  g = (z >= 0.f ? r : e * r) - y;
+  return fmaxf(z, 0.f) - z * y + log1pf(e);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -3,7 +3,7 @@
 The reference runs whatever graph the user serialised through a TF session.  The H100 engine
 instead executes a *compiled* plan: the forward chain between ``tfInput`` and the loss is pattern-
 matched into dense / conv / pool / reshape layers with fused bias+activation, the loss into
-softmax-cross-entropy or mean-squared-error, ``tf.nn.dropout`` / ``tf.layers.dropout`` after a dense layer into a
+softmax-cross-entropy, sigmoid-cross-entropy or mean-squared-error, ``tf.nn.dropout`` / ``tf.layers.dropout`` after a dense layer into a
 fused Philox mask in that layer's epilogue, and ``tfOutput`` into "activation of layer k" (+ optional ArgMax /
 Softmax).  Graphs outside this family (custom losses, exotic ops) are reported as unsupported so the caller can use the
 generic interpreter engine instead (loudly: a RuntimeWarning names the reason).
@@ -69,7 +69,7 @@ class OutputSpec:
 @dataclass
 class LayerPlan:
     layers: List[Layer]
-    loss: Optional[str]                         # softmax_xent | mse | None (inference only)
+    loss: Optional[str]                         # softmax_xent | sigmoid_xent | mse | None (inference only)
     input_name: str
     label_name: Optional[str]                   # placeholder fed with labels; None if target is the input
     target_is_input: bool
@@ -130,6 +130,22 @@ def _const_scalar(ir: GraphIR, ref: Tuple[str, int]) -> Optional[float]:
     return None
 
 
+def _const_ones(ir: GraphIR, ref: Tuple[str, int]) -> bool:
+    """``ref`` is a Const (possibly behind Identity / PlaceholderWithDefault / Cast) whose every element is 1"""
+    node = ir.nodes[ref[0]]
+    hops = 0
+    while node.op in ("Identity", "PlaceholderWithDefault", "Cast") and node.inputs and hops < 6:
+        node = ir.nodes[node.inputs[0][0]]
+        hops += 1
+    if node.op != "Const":
+        return False
+    try:
+        v = node.attrs["value"].reshape(-1)
+        return v.size > 0 and bool((v == 1).all())
+    except Exception:
+        return False
+
+
 def _match_dropout(ir: GraphIR, node: Node) -> Optional[Tuple[Tuple[str, int], float]]:
     """``tf.nn.dropout`` sub-graph: Mul(RealDiv(x, keep), Floor(Add(keep, RandomUniform(Shape(x))))) -> (x, keep)."""
     if node.op != "Mul" or len(node.inputs) != 2:
@@ -149,6 +165,73 @@ def _match_dropout(ir: GraphIR, node: Node) -> Optional[Tuple[Tuple[str, int], f
     return None
 
 
+def _is_zeros_like(ir: GraphIR, ref: Tuple[str, int], x: Tuple[str, int]) -> bool:
+    n = ir.nodes[ref[0]]
+    return n.op == "ZerosLike" and len(n.inputs) == 1 and n.inputs[0] == x
+
+
+def _is_nonneg_cond(ir: GraphIR, ref: Tuple[str, int], x: Tuple[str, int]) -> bool:
+    """``x >= zeros_like(x)``"""
+    n = ir.nodes[ref[0]]
+    return n.op == "GreaterEqual" and len(n.inputs) == 2 and n.inputs[0] == x and _is_zeros_like(ir, n.inputs[1], x)
+
+
+def _relu_of(ir: GraphIR, ref: Tuple[str, int]) -> Optional[Tuple[str, int]]:
+    """x of ``Relu(x)`` or of TF's ``Select(x >= zeros_like(x), x, zeros_like(x))``"""
+    n = ir.nodes[ref[0]]
+    if n.op == "Relu" and len(n.inputs) == 1:
+        return n.inputs[0]
+    if n.op == "Select" and len(n.inputs) == 3:
+        x = n.inputs[1]
+        if _is_nonneg_cond(ir, n.inputs[0], x) and _is_zeros_like(ir, n.inputs[2], x):
+            return x
+    return None
+
+
+def _neg_abs_of(ir: GraphIR, ref: Tuple[str, int]) -> Optional[Tuple[str, int]]:
+    """x of ``Neg(Abs(x))`` or of TF's ``Select(x >= zeros_like(x), Neg(x), x)``"""
+    n = ir.nodes[ref[0]]
+    if n.op == "Neg" and len(n.inputs) == 1:
+        a = ir.nodes[n.inputs[0][0]]
+        return a.inputs[0] if a.op == "Abs" and len(a.inputs) == 1 else None
+    if n.op == "Select" and len(n.inputs) == 3:
+        x = n.inputs[2]
+        neg = ir.nodes[n.inputs[1][0]]
+        if _is_nonneg_cond(ir, n.inputs[0], x) and neg.op == "Neg" and neg.inputs == [x]:
+            return x
+    return None
+
+
+def _match_sigmoid_xent(ir: GraphIR, node: Node) -> Optional[Tuple[Tuple[str, int], Tuple[str, int]]]:
+    """``tf.nn.sigmoid_cross_entropy_with_logits``: Add(Sub(relu(x), Mul(x, z)), Log1p(Exp(-|x|))), with relu and -|x| in
+    the tfcompat builder's spelling (Relu, Neg(Abs)) or TF-1.x's (Select on x >= 0) -> (logits x, labels z)."""
+    if node.op not in ("Add", "AddV2") or len(node.inputs) != 2:
+        return None
+    for s_ref, l_ref in ((node.inputs[0], node.inputs[1]), (node.inputs[1], node.inputs[0])):
+        sub, log1p = ir.nodes[s_ref[0]], ir.nodes[l_ref[0]]
+        if sub.op != "Sub" or len(sub.inputs) != 2 or log1p.op != "Log1p" or len(log1p.inputs) != 1:
+            continue
+        ex = ir.nodes[log1p.inputs[0][0]]
+        if ex.op != "Exp" or len(ex.inputs) != 1:
+            continue
+        x = _relu_of(ir, sub.inputs[0])
+        mul = ir.nodes[sub.inputs[1][0]]
+        if x is None or mul.op != "Mul" or len(mul.inputs) != 2 or _neg_abs_of(ir, ex.inputs[0]) != x:
+            continue
+        if mul.inputs[0] == x:
+            return x, mul.inputs[1]
+        if mul.inputs[1] == x:
+            return x, mul.inputs[0]
+    return None
+
+
+_FLOAT_TYPES = ("DT_FLOAT", "DT_HALF", "DT_BFLOAT16", "DT_DOUBLE")
+
+
+def _float_cast(node: Node) -> bool:
+    return node.attrs.get("SrcT", "DT_FLOAT") in _FLOAT_TYPES and node.attrs.get("DstT", "DT_FLOAT") in _FLOAT_TYPES
+
+
 def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
     """Walk back from the scalar loss through reductions / scalings to the per-element loss node."""
     seen = set()
@@ -165,6 +248,8 @@ def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
             return "mse", node
         if node.op == "Square" and node.inputs and ir.nodes[node.inputs[0][0]].op == "Sub":
             return "mse", ir.nodes[node.inputs[0][0]]
+        if _match_sigmoid_xent(ir, node) is not None:
+            return "sigmoid_xent", node
         if node.op in ("Sum", "Mean", "RealDiv", "Div", "DivNoNan", "Mul", "Identity", "Select", "Reshape", "Cast"):
             # follow data inputs that are not plain constants / shape plumbing
             for src, _ in node.inputs[: 1 if node.op in ("Sum", "Mean", "Reshape") else len(node.inputs)]:
@@ -172,7 +257,7 @@ def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
                     frontier.append(src)
         else:
             continue
-    raise UnsupportedGraph(f"loss '{loss_ref}' is neither softmax-cross-entropy nor mean-squared-error")
+    raise UnsupportedGraph(f"loss '{loss_ref}' is neither softmax-cross-entropy, sigmoid-cross-entropy nor mean-squared-error")
 
 
 def _check_mean_reduction(ir: GraphIR, loss_ref: str, kind: str, core: Node) -> None:
@@ -184,6 +269,8 @@ def _check_mean_reduction(ir: GraphIR, loss_ref: str, kind: str, core: Node) -> 
     hops = 0
     while node.name != core.name and hops < 16:
         ops_on_path.append(node.op)
+        if kind == "sigmoid_xent" and node.op == "Mul" and not any(_const_ones(ir, i) for i in node.inputs):
+            raise UnsupportedGraph("weighted sigmoid cross-entropy is not covered by the compiled plan")
         nxt = None
         for src, _ in node.inputs:
             if ir.nodes[src].op not in ("Const", "Size", "Shape", "Cast") or src == core.name:
@@ -196,6 +283,9 @@ def _check_mean_reduction(ir: GraphIR, loss_ref: str, kind: str, core: Node) -> 
     if "Mean" in ops_on_path:
         if kind == "mse" and "Mul" in ops_on_path:
             raise UnsupportedGraph("scaled MSE variants are not covered by the compiled plan")
+        if kind == "sigmoid_xent" and "Sum" in ops_on_path:
+            # e.g. reduce_mean(reduce_sum(per_element, axis=1)): a sum over the labels, N times the element mean
+            raise UnsupportedGraph("a sum under a mean of sigmoid cross-entropy is not covered by the compiled plan")
         return
     if "Sum" in ops_on_path and any(o in ops_on_path for o in ("RealDiv", "Div", "DivNoNan")):
         return
@@ -223,6 +313,8 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
         a, b = core.inputs[0], core.inputs[1]
         if loss_kind == "softmax_xent":
             pred_ref, target_ref = a, b               # (features=logits, labels)
+        elif loss_kind == "sigmoid_xent":
+            pred_ref, target_ref = _match_sigmoid_xent(ir, core)
         else:
             # mean_squared_error is symmetric: the side that is a placeholder is the target
             def is_ph(ref):
@@ -406,7 +498,9 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
     label_dim = 0
     if need_loss:
         tnode = ir.nodes[target_ref[0]]
-        while tnode.op in _PASS and tnode.inputs:
+        # tf.losses.sigmoid_cross_entropy casts the labels to the logits' dtype
+        passes = _PASS + ("Cast",) if loss_kind == "sigmoid_xent" else _PASS
+        while tnode.op in passes and tnode.inputs and (tnode.op != "Cast" or _float_cast(tnode)):
             tnode = ir.nodes[tnode.inputs[0][0]]
         if tnode.name == input_node:
             target_is_input = True
@@ -421,8 +515,8 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             raise UnsupportedGraph("loss target must be a placeholder or the input itself")
         if label_dim != layers[-1].out_features:
             raise UnsupportedGraph("label width does not match the network output width")
-        if loss_kind == "softmax_xent" and layers[-1].act is not None:
-            raise UnsupportedGraph("softmax cross-entropy expects raw logits")
+        if loss_kind in ("softmax_xent", "sigmoid_xent") and layers[-1].act is not None:
+            raise UnsupportedGraph(f"{loss_kind.split('_')[0]} cross-entropy expects raw logits")
         if layers[-1].dropout_keep:
             raise UnsupportedGraph("dropout on the network output is not covered by the compiled plan")
 

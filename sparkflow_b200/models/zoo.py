@@ -11,6 +11,7 @@ Each function mirrors a model definition of the reference:
   * :func:`cnn_same`          – TensorFlow's "Deep MNIST" network (SAME-padded convs and pools)
   * :func:`cnn_strided`       – strided / SAME convs, a conv feeding a conv, an overlapping 3x3/2 pool, a conv feeding
     the flatten
+  * :func:`binary_dnn` / :func:`multilabel_dnn` – binary and multi-label classifiers trained with sigmoid cross-entropy
 """
 from __future__ import annotations
 
@@ -27,6 +28,30 @@ def simple_dnn():
     logits = tf.layers.dense(h2, 10, kernel_initializer=tf.glorot_uniform_initializer())
     tf.argmax(logits, 1, name="out")
     return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def binary_dnn():
+    """784-256-256-1 binary classifier: sigmoid cross-entropy on the logit, ``out`` = its probability"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 1], name="y")
+    h1 = tf.layers.dense(x, 256, activation=tf.nn.relu)
+    h2 = tf.layers.dense(h1, 256, activation=tf.nn.relu)
+    logits = tf.layers.dense(h2, 1)
+    tf.nn.sigmoid(logits, name="out")
+    return tf.losses.sigmoid_cross_entropy(y, logits)
+
+
+def multilabel_dnn(tags: int = 40):
+    """784-256-``tags`` multi-label classifier: one independent sigmoid cross-entropy per tag, spelled as
+    ``reduce_mean(sigmoid_cross_entropy_with_logits)`` + ``add_loss``"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, tags], name="y")
+    h = tf.layers.dense(x, 256, activation=tf.nn.relu)
+    logits = tf.layers.dense(h, tags)
+    tf.nn.sigmoid(logits, name="out")
+    loss = tf.reduce_mean(tf.nn.sigmoid_cross_entropy_with_logits(labels=y, logits=logits))
+    tf.losses.add_loss(loss)
+    return loss
 
 
 def cnn():
@@ -133,6 +158,8 @@ MODELS: Dict[str, Callable] = {
     "test_mlp": test_mlp,
     "test_autoencoder": test_autoencoder,
     "fixture_mlp": fixture_mlp,
+    "binary_dnn": binary_dnn,
+    "multilabel_dnn": multilabel_dnn,
 }
 
 

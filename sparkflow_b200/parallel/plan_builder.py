@@ -122,6 +122,16 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
     return i
 
 
+_LOSS_MODES = {"softmax_xent": 1, "mse": 2, "sigmoid_xent": 3}     # SfLossMode (csrc/sf_api.h)
+
+
+def loss_mode(kind: Optional[str]) -> int:
+    """the fused-loss GEMM epilogue's head for LayerPlan loss kind ``kind``"""
+    if kind not in _LOSS_MODES:
+        raise UnsupportedGraph(f"no fused loss head for loss kind {kind!r}")
+    return _LOSS_MODES[kind]
+
+
 def _split_k(tiles: int, kblocks: int) -> int:
     if kblocks < 16:
         return 1
@@ -364,11 +374,12 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             drop = dict(keep=float(l.dropout_keep), seed=seed, stream=i, ctr=done_dev)
         rec[i] = dict(a_in=cur["buf"], a_in_ld=cur["ld"], a_inT=cur.get("bufT"), drop=drop)
         if last:
-            fuse_loss = train and worker.fuse_loss and (lp.loss == "mse" or ks.cols <= 32)
+            # the element-wise heads take any width; the softmax row must fit one 32-column epilogue chunk
+            fuse_loss = train and worker.fuse_loss and (lp.loss != "softmax_xent" or ks.cols <= 32)
             if fuse_loss:
                 dz_last, dzT_last = zeros(B, round_up(ks.cols, 8)), (None if use_mn else zeros(ks.cols, ldB))
                 db = P(worker.grads) + bs.offset * 4 if bs else 0
-                d.update(loss_mode=1 if lp.loss == "softmax_xent" else 2, target=P(target), ld_target=target.shape[1],
+                d.update(loss_mode=loss_mode(lp.loss), target=P(target), ld_target=target.shape[1],
                          loss=P(worker.loss_acc), out_bf16=P(dz_last), ld_bf16=dz_last.shape[1], outT_bf16=P(dzT_last),
                          ld_t=ldB if dzT_last is not None else 0, colsum=db)
             else:
@@ -388,12 +399,22 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     result = None
     last_l = layers[stop_layer]
     n_out = lay.by_name(last_l.kernel).cols
+
+    def add_loss(loss, dz, ld_dz, dzT, ld_t, db):
+        """stand-alone loss kernel on the fp32 output of the last layer (pointers 0: not written)"""
+        args = (P(out_f32), n_out, P(target), target.shape[1])
+        if lp.loss == "softmax_xent":
+            plan.add_softmax_xent(*args, loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
+        elif lp.loss == "sigmoid_xent":
+            plan.add_sigmoid_xent(*args, loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
+        elif lp.loss == "mse":
+            plan.add_mse(*args, ACT_IDS[last_l.act], loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
+        else:
+            raise UnsupportedGraph(f"no loss kernel for loss kind {lp.loss!r}")
+
     if not train:
         if with_loss:
-            if lp.loss == "softmax_xent":
-                plan.add_softmax_xent(P(out_f32), n_out, P(target), target.shape[1], P(loss_out), 0, 0, 0, 0, 0, B, n_out)
-            else:
-                plan.add_mse(P(out_f32), n_out, P(target), target.shape[1], ACT_IDS[last_l.act], P(loss_out), 0, 0, 0, 0, 0, B, n_out)
+            add_loss(P(loss_out), 0, 0, 0, 0, 0)
         elif post == "ArgMax":
             result = zeros(B, dtype=f32)
             plan.add_argmax(P(out_f32), n_out, P(result), B, n_out)
@@ -407,13 +428,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     if not fuse_loss:
         dz_last, dzT_last = zeros(B, round_up(n_out, 8)), (None if use_mn else zeros(n_out, ldB))
         db = P(worker.grads) + bs_last.offset * 4 if bs_last else 0
-        ldt_last = ldB if dzT_last is not None else 0
-        if lp.loss == "softmax_xent":
-            plan.add_softmax_xent(P(out_f32), n_out, P(target), target.shape[1], P(worker.loss_acc), P(dz_last), dz_last.shape[1],
-                                  P(dzT_last), ldt_last, db, B, n_out)
-        else:
-            plan.add_mse(P(out_f32), n_out, P(target), target.shape[1], ACT_IDS[last_l.act], P(worker.loss_acc), P(dz_last),
-                         dz_last.shape[1], P(dzT_last), ldt_last, db, B, n_out)
+        add_loss(P(worker.loss_acc), P(dz_last), dz_last.shape[1], P(dzT_last), ldB if dzT_last is not None else 0, db)
 
     # ---------------- backward ----------------
     n_side = [0]

@@ -89,7 +89,7 @@ for kid, rs in by_kid.items():
         cur["end"] = max(cur["end"], r["t2"])
 summ.sort(key=lambda c: c["ready"])
 names = {1: "gemm", 2: "cast", 3: "softmax", 4: "mse", 5: "argmax", 6: "push", 7: "pull", 8: "im2col", 9: "col2im", 10: "pool_fwd", 11: "pool_bwd", 12: "pool_gen_fwd", 13: "pool_gen_bwd",
-         14: "act_bwd"}
+         14: "act_bwd", 15: "sigmoid_xent"}
 print("card:", torch.cuda.get_device_name(0), "| plan:", plan.names())
 print("%-8s %5s %9s %9s %9s %8s" % ("kernel", "ctas", "start_us", "ready_us", "end_us", "dur_us"))
 for s in summ:
