@@ -19,6 +19,8 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <tuple>
+#include <utility>
 #include <vector>
 
 #include "sf_api.h"
@@ -50,6 +52,28 @@ template <class T>
 T getd(const py::dict& d, const char* k, T dflt) {
   if (d.contains(k) && !d[k].is_none()) return d[k].cast<T>();
   return dflt;
+}
+
+// the device addresses listed under `k`, cast into `out` (more than `out` holds: `what` is the error); returns how many
+template <class T, size_t N>
+int getd_ptrs(const py::dict& d, const char* k, const char* what, T* (&out)[N]) {
+  const auto v = getd<std::vector<uintptr_t>>(d, k, {});
+  if (v.size() > N) throw std::runtime_error(what);
+  for (size_t i = 0; i < v.size(); ++i) out[i] = P<T>(v[i]);
+  return static_cast<int>(v.size());
+}
+
+// one (offset, rows, cols, w_off, w_ld, wt_off, wt_ld) row of a variable table (any other length: `what` is the error)
+void fill_seg(SfTensorSeg& sg, const std::vector<int64_t>& r, const char* what) {
+  if (r.size() != 7) throw std::runtime_error(what);
+  std::memset(&sg, 0, sizeof(sg));
+  sg.offset = r[0];
+  sg.rows = static_cast<int>(r[1]);
+  sg.cols = static_cast<int>(r[2]);
+  sg.w_off = r[3];
+  sg.w_ld = static_cast<int>(r[4]);
+  sg.wt_off = r[5];
+  sg.wt_ld = static_cast<int>(r[6]);
 }
 
 // ---------------------------------------------------------------------------
@@ -145,20 +169,11 @@ SfPushArgs parse_push(const py::dict& d) {
   std::memset(&a, 0, sizeof(a));
   a.state = P<float4>(getd<uintptr_t>(d, "state", 0));
   a.ctrl = P<uint32_t>(getd<uintptr_t>(d, "ctrl", 0));
-  auto dsts = getd<std::vector<uintptr_t>>(d, "shadow_dst", {});
-  if (dsts.size() > 8) throw std::runtime_error("push: at most 8 publish destinations");
-  a.n_shadow_dst = static_cast<int>(dsts.size());
-  for (size_t i = 0; i < dsts.size(); ++i) a.shadow_dst[i] = P<__nv_bfloat16>(dsts[i]);
-  auto vps = getd<std::vector<uintptr_t>>(d, "vec_pub", {});
-  if (vps.size() > 2) throw std::runtime_error("push: at most 2 vec_pub targets");
-  a.n_vec_pub = static_cast<int>(vps.size());
-  for (size_t i = 0; i < vps.size(); ++i) a.vec_pub[i] = P<float>(vps[i]);
+  a.n_shadow_dst = getd_ptrs(d, "shadow_dst", "push: at most 8 publish destinations", a.shadow_dst);
+  a.n_vec_pub = getd_ptrs(d, "vec_pub", "push: at most 2 vec_pub targets", a.vec_pub);
   a.vec_offset = getd<long long>(d, "vec_offset", 0);
   a.shadow_is_mc = getd<int>(d, "shadow_is_mc", 0);
-  auto vds = getd<std::vector<uintptr_t>>(d, "vec_dst", {});
-  if (vds.size() > 8) throw std::runtime_error("push: at most 8 vec_dst targets");
-  a.n_vec_dst = static_cast<int>(vds.size());
-  for (size_t i = 0; i < vds.size(); ++i) a.vec_dst[i] = P<float>(vds[i]);
+  a.n_vec_dst = getd_ptrs(d, "vec_dst", "push: at most 8 vec_dst targets", a.vec_dst);
   a.mb_zero = getd<int>(d, "mb_zero", 0);
   a.grad = P<float>(getd<uintptr_t>(d, "grad", 0));
   a.loss_acc = P<float>(getd<uintptr_t>(d, "loss_acc", 0));
@@ -181,11 +196,8 @@ SfPushArgs parse_push(const py::dict& d) {
     if (!rows.empty() && rows.size() <= SF_MAX_INLINE_SEGS) {
       int acc = 0;
       for (size_t i = 0; i < rows.size(); ++i) {
-        const auto& r = rows[i];
-        if (r.size() != 7) throw std::runtime_error("push: seg_rows entries are (offset, rows, cols, w_off, w_ld, wt_off, wt_ld)");
         SfTensorSeg& sg = a.inline_segs[i];
-        sg.offset = r[0]; sg.rows = static_cast<int>(r[1]); sg.cols = static_cast<int>(r[2]);
-        sg.w_off = r[3]; sg.w_ld = static_cast<int>(r[4]); sg.wt_off = r[5]; sg.wt_ld = static_cast<int>(r[6]);
+        fill_seg(sg, rows[i], "push: seg_rows entries are (offset, rows, cols, w_off, w_ld, wt_off, wt_ld)");
         a.tile_prefix[i] = acc;
         acc += ((sg.rows + 31) / 32) * ((sg.cols + 63) / 64);
       }
@@ -266,11 +278,9 @@ SfPostFlagsArgs parse_post_flags(const py::dict& d) {
   a.n_shards = getd<int>(d, "n_shards", 0);
   if (a.n_shards < 1 || a.n_shards > SF_MAX_SHARDS) throw std::runtime_error("post_flags: n_shards in [1, 8]");
   fill_bounds(d, a.n_shards, a.bounds);
-  auto posted = getd<std::vector<uintptr_t>>(d, "posted", {});
-  auto mbs = getd<std::vector<uintptr_t>>(d, "mailbox", {});
-  if (static_cast<int>(posted.size()) != a.n_shards || static_cast<int>(mbs.size()) != a.n_shards)
-    throw std::runtime_error("post_flags: one posted word and one mailbox per shard");
-  for (int i = 0; i < a.n_shards; ++i) { a.posted[i] = P<uint32_t>(posted[i]); a.mailbox[i] = P<float>(mbs[i]); }
+  const char* per_shard = "post_flags: one posted word and one mailbox per shard";
+  if (getd_ptrs(d, "posted", per_shard, a.posted) != a.n_shards || getd_ptrs(d, "mailbox", per_shard, a.mailbox) != a.n_shards)
+    throw std::runtime_error(per_shard);
   a.grad = P<float>(getd<uintptr_t>(d, "grad", 0));
   a.vec_tiles = P<const long long>(getd<uintptr_t>(d, "vec_tiles", 0));
   a.n_vec_tiles = getd<int>(d, "n_vec_tiles", 0);
@@ -736,25 +746,20 @@ class Applier {
     args_.tile_begin = getd<int>(shard, "tile_begin", 0);
     args_.tile_end = getd<int>(shard, "tile_end", 0);
     {
-      auto acks = getd<std::vector<uintptr_t>>(shard, "ack", {});
-      if (acks.size() > 8) throw std::runtime_error("applier: at most 8 ack words");
-      if (!acks.empty() && static_cast<int>(acks.size()) != n_workers) throw std::runtime_error("applier: one ack word per worker, or none");
-      for (size_t i = 0; i < acks.size(); ++i) {
-        if (!acks[i]) throw std::runtime_error("applier: ack words must be non-null");
-        args_.ack[i] = P<uint32_t>(acks[i]);
-      }
-      auto vb = getd<std::vector<uintptr_t>>(shard, "ver_begin", {});
-      auto ve = getd<std::vector<uintptr_t>>(shard, "ver_end", {});
-      if (vb.size() != ve.size() || vb.size() > 8) throw std::runtime_error("applier: ver_begin / ver_end lists must match (<= 8)");
-      args_.n_ver = static_cast<int>(vb.size());
-      for (size_t i = 0; i < vb.size(); ++i) { args_.ver_begin[i] = P<uint32_t>(vb[i]); args_.ver_end[i] = P<uint32_t>(ve[i]); }
+      const int n_ack = getd_ptrs(shard, "ack", "applier: at most 8 ack words", args_.ack);
+      if (n_ack && n_ack != n_workers) throw std::runtime_error("applier: one ack word per worker, or none");
+      for (int i = 0; i < n_ack; ++i)
+        if (!args_.ack[i]) throw std::runtime_error("applier: ack words must be non-null");
+      const char* ver = "applier: ver_begin / ver_end lists must match (<= 8)";
+      args_.n_ver = getd_ptrs(shard, "ver_begin", ver, args_.ver_begin);
+      if (getd_ptrs(shard, "ver_end", ver, args_.ver_end) != args_.n_ver) throw std::runtime_error(ver);
       args_.ver_mc = getd<int>(shard, "ver_mc", 0);
       args_.stats = P<unsigned long long>(getd<uintptr_t>(shard, "stats", 0));
       args_.linger = getd<int>(shard, "linger", 0);
       args_.ver_local = P<const uint32_t>(getd<uintptr_t>(shard, "ver_local", 0));
       args_.slot_off_bf16 = getd<long long>(shard, "slot_off_bf16", 0);
       args_.slot_off_f32 = getd<long long>(shard, "slot_off_f32", 0);
-      if (args_.n_ver > 0 && (acks.empty() || !args_.ver_local || !args_.slot_off_bf16 || !args_.slot_off_f32))
+      if (args_.n_ver > 0 && (!n_ack || !args_.ver_local || !args_.slot_off_bf16 || !args_.slot_off_f32))
         throw std::runtime_error("applier: seqlock stamps need ack words, ver_local and both slot offsets");
     }
     ck(cudaGetDevice(&device_), "cudaGetDevice");
@@ -855,20 +860,163 @@ bool enable_peer_access(int peer) {
 py::bytes pack_segs(const std::vector<std::vector<int64_t>>& rows) {
   std::vector<SfTensorSeg> v(rows.size());
   for (size_t i = 0; i < rows.size(); ++i) {
-    const auto& r = rows[i];
-    if (r.size() != 7) throw std::runtime_error("pack_segs: (offset, rows, cols, w_off, w_ld, wt_off, wt_ld)");
-    std::memset(&v[i], 0, sizeof(SfTensorSeg));
-    v[i].offset = r[0];
-    v[i].rows = static_cast<int>(r[1]);
-    v[i].cols = static_cast<int>(r[2]);
-    v[i].w_off = r[3];
-    v[i].w_ld = static_cast<int>(r[4]);
-    v[i].wt_off = r[5];
-    v[i].wt_ld = static_cast<int>(r[6]);
+    fill_seg(v[i], rows[i], "pack_segs: (offset, rows, cols, w_off, w_ld, wt_off, wt_ld)");
     if (v[i].w_off >= 0 && ((v[i].w_ld % 8) || (v[i].w_off % 8))) throw std::runtime_error("pack_segs: w_ld / w_off must be multiples of 8");
     if (v[i].wt_off >= 0 && ((v[i].wt_ld % 8) || (v[i].wt_off % 8))) throw std::runtime_error("pack_segs: wt_ld / wt_off must be multiples of 8");
   }
   return py::bytes(reinterpret_cast<const char*>(v.data()), v.size() * sizeof(SfTensorSeg));
+}
+
+// ---------------------------------------------------------------------------
+// Kernel launchers: each takes a kernel's Python-facing arguments (device addresses, sizes; the dict-driven ops parse
+// and check their dict here, once) and returns the launch as a callable of the stream that returns the sf_* rc.  A plan
+// keeps the callable and calls it on every run; the direct entry point calls it right away (see def_kernel).
+// ---------------------------------------------------------------------------
+namespace launch {
+
+auto cast_transpose(uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, int rows, int cols) {
+  return [=](cudaStream_t st) {
+    return idx ? sf_gather_cast_transpose(P<const float>(in), ld_in, P<const int32_t>(idx), P<__nv_bfloat16>(out), ld_out,
+                                          P<__nv_bfloat16>(outT), ld_t, rows, cols, st)
+               : sf_cast_transpose(P<const float>(in), ld_in, P<__nv_bfloat16>(out), ld_out, P<__nv_bfloat16>(outT), ld_t, rows, cols, st);
+  };
+}
+auto softmax_xent(uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss, uintptr_t dz, int ld_dz,
+                  uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
+  return [=](cudaStream_t st) {
+    return sf_softmax_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss), P<__nv_bfloat16>(dz),
+                           ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
+  };
+}
+auto mse(uintptr_t out, int ld_out, uintptr_t target, int ld_target, int act, uintptr_t loss, uintptr_t dz, int ld_dz, uintptr_t dzT,
+         int ld_t, uintptr_t dbias, int rows, int cols) {
+  return [=](cudaStream_t st) {
+    return sf_mse_loss(P<const float>(out), ld_out, P<const float>(target), ld_target, act, P<float>(loss), P<__nv_bfloat16>(dz), ld_dz,
+                       P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
+  };
+}
+auto sigmoid_xent(uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss, uintptr_t dz, int ld_dz,
+                  uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
+  return [=](cudaStream_t st) {
+    return sf_sigmoid_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss), P<__nv_bfloat16>(dz),
+                           ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
+  };
+}
+auto argmax(uintptr_t in, int ld, uintptr_t out, int rows, int cols) {
+  return [=](cudaStream_t st) { return sf_argmax_rows(P<const float>(in), ld, P<float>(out), rows, cols, st); };
+}
+auto im2col(uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, int sh, int sw,
+            int pad_top, int pad_left, int out_h, int out_w) {
+  return [=](cudaStream_t st) {
+    return sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w, P<__nv_bfloat16>(out),
+                          ld_out, P<__nv_bfloat16>(outT), ld_t, st);
+  };
+}
+auto col2im(uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din, int sh, int sw, int pad_top,
+            int pad_left, int out_h, int out_w) {
+  return [=](cudaStream_t st) {
+    return sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                          P<__nv_bfloat16>(din), st);
+  };
+}
+auto maxpool_fwd(uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintptr_t argmax, uintptr_t outT, int ld_t) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool2_fwd(P<const __nv_bfloat16>(in), n, h, w, c, P<__nv_bfloat16>(out), P<uint8_t>(argmax), P<__nv_bfloat16>(outT), ld_t, st);
+  };
+}
+auto maxpool_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz,
+                 uintptr_t dzT, int ld_t, uintptr_t dbias) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool2_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, P<const __nv_bfloat16>(act_out), act,
+                           P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), st);
+  };
+}
+auto maxpool_gen_fwd(uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
+                     int out_w, uintptr_t out, uintptr_t argmax) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool_fwd(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w, P<__nv_bfloat16>(out),
+                          P<uint8_t>(argmax), st);
+  };
+}
+auto maxpool_gen_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
+                     int pad_left, int out_h, int out_w, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h,
+                          out_w, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
+  };
+}
+auto act_bwd_bias(uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+  return [=](cudaStream_t st) {
+    return sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz,
+                           P<float>(dbias), st);
+  };
+}
+auto conv_first_fwd(uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act,
+                    uintptr_t pooled, uintptr_t argmax, int pad_top, int pad_left, int out_h, int out_w) {
+  return [=](cudaStream_t st) {
+    return sf_conv_first_fwd(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(wT), ld_w, P<const float>(bias),
+                             act, P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), pad_top, pad_left, out_h, out_w, st);
+  };
+}
+auto conv_first_wgrad(uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t g_pool, uintptr_t pooled,
+                      uintptr_t argmax, int act, uintptr_t dW, uintptr_t db, int pad_top, int pad_left, int out_h, int out_w) {
+  return [=](cudaStream_t st) {
+    return sf_conv_first_wgrad(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(g_pool),
+                               P<const __nv_bfloat16>(pooled), P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), pad_top, pad_left,
+                               out_h, out_w, st);
+  };
+}
+auto push(const py::dict& d, uintptr_t local_sync, int grid) {
+  const SfPushArgs a = parse_push(d);
+  return [=](cudaStream_t st) { return sf_push_launch(&a, P<uint32_t>(local_sync), grid, st); };
+}
+auto post(const py::dict& d, uintptr_t local_sync, int grid) {
+  const SfPostArgs a = parse_post(d);
+  return [=](cudaStream_t st) { return sf_post_launch(&a, P<uint32_t>(local_sync), grid, st); };
+}
+auto pull(const py::dict& d, uintptr_t local_sync, int grid) {
+  const SfPullArgs a = parse_pull(d);
+  return [=](cudaStream_t st) { return sf_pull_launch(&a, P<uint32_t>(local_sync), grid, st); };
+}
+auto sync_pull(const py::dict& d) {
+  const SfSyncPullArgs a = parse_sync_pull(d);
+  return [=](cudaStream_t st) { return sf_sync_pull_launch(&a, st); };
+}
+auto post_flags(const py::dict& d) {
+  const SfPostFlagsArgs a = parse_post_flags(d);
+  return [=](cudaStream_t st) { return sf_post_flags_launch(&a, st); };
+}
+
+}  // namespace launch
+
+// the direct entry point of `launch`: its arguments with the stream inserted before the last sizeof...(J) of them
+template <class L, class... A, size_t... I, size_t... J>
+auto direct_entry(const char* name, L (*launch)(A...), std::index_sequence<I...>, std::index_sequence<J...>) {
+  using Args = std::tuple<A...>;
+  return [name, launch](std::tuple_element_t<I, Args>... lead, uintptr_t stream,
+                        std::tuple_element_t<sizeof...(I) + J, Args>... trail) { ck_rc(launch(lead..., trail...)(S(stream)), name); };
+}
+
+// Binds one kernel's launcher twice: as the plan op Plan.add_<plan_name>(args...) and as the direct entry point
+// <direct_name>(args..., stream), which launches at once and raises if the launch fails.  `names` are the keyword names
+// of the leading arguments and `defaults` those of the trailing defaulted ones; the direct form takes its stream between
+// the two.  Bound without them, the arguments are positional and the stream comes last.
+template <class L, class... A, class... N, class... D>
+void def_kernel(py::module_& m, py::class_<Plan>& plan, const char* plan_name, const char* direct_name, L (*launch)(A...),
+                std::tuple<N...> names, std::tuple<D...> defaults) {
+  auto add = [plan_name, launch](Plan& p, A... a) { p.add(plan_name, launch(a...)); };
+  auto now = direct_entry(direct_name, launch, std::make_index_sequence<sizeof...(A) - sizeof...(D)>(),
+                          std::make_index_sequence<sizeof...(D)>());
+  const std::string add_name = std::string("add_") + plan_name;
+  std::apply([&](const auto&... x) { plan.def(add_name.c_str(), add, x...); }, std::tuple_cat(names, defaults));
+  if constexpr (sizeof...(N) + sizeof...(D) == 0)
+    m.def(direct_name, now);
+  else
+    std::apply([&](const auto&... x) { m.def(direct_name, now, x...); }, std::tuple_cat(names, std::make_tuple(py::arg("stream")), defaults));
+}
+template <class L, class... A>
+void def_kernel(py::module_& m, py::class_<Plan>& plan, const char* plan_name, const char* direct_name, L (*launch)(A...)) {
+  def_kernel(m, plan, plan_name, direct_name, launch, std::tuple<>(), std::tuple<>());
 }
 
 }  // namespace
@@ -892,8 +1040,8 @@ PYBIND11_MODULE(_C, m) {
       .def("mn_major", &Gemm::mn_major)
       .def_property_readonly("grid", &Gemm::grid);
 
-  py::class_<Plan>(m, "Plan")
-      .def(py::init<>())
+  py::class_<Plan> plan(m, "Plan");
+  plan.def(py::init<>())
       .def("__len__", &Plan::size)
       .def("names", &Plan::names)
       .def("run", &Plan::run)
@@ -906,163 +1054,49 @@ PYBIND11_MODULE(_C, m) {
       .def("join", &Plan::join)
       .def("graph_nodes", &Plan::graph_nodes)
       .def("add_gemm", &Plan::add_gemm, py::arg("gemm"), py::arg("name") = "gemm")
-      .def("add_cast_transpose",
-           [](Plan& p, uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, uintptr_t outT,
-              int ld_t, int rows, int cols) {
-             p.add("cast_transpose", [=](cudaStream_t st) {
-               return idx ? sf_gather_cast_transpose(P<const float>(in), ld_in, P<const int32_t>(idx),
-                                                     P<__nv_bfloat16>(out), ld_out, P<__nv_bfloat16>(outT),
-                                                     ld_t, rows, cols, st)
-                          : sf_cast_transpose(P<const float>(in), ld_in, P<__nv_bfloat16>(out), ld_out,
-                                              P<__nv_bfloat16>(outT), ld_t, rows, cols, st);
-             });
-           })
       .def("add_gather_rows",
            [](Plan& p, uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, int rows, int cols) {
              p.add("gather_rows", [=](cudaStream_t st) {
                return sf_gather_rows_f32(P<const float>(in), ld_in, P<const int32_t>(idx), P<float>(out), ld_out, rows, cols, st);
              });
-           })
-      .def("add_softmax_xent",
-           [](Plan& p, uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss,
-              uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
-             p.add("softmax_xent", [=](cudaStream_t st) {
-               return sf_softmax_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels,
-                                      P<float>(loss), P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t,
-                                      P<float>(dbias), rows, cols, st);
-             });
-           })
-      .def("add_mse",
-           [](Plan& p, uintptr_t out, int ld_out, uintptr_t target, int ld_target, int act, uintptr_t loss,
-              uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
-             p.add("mse", [=](cudaStream_t st) {
-               return sf_mse_loss(P<const float>(out), ld_out, P<const float>(target), ld_target, act,
-                                  P<float>(loss), P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t,
-                                  P<float>(dbias), rows, cols, st);
-             });
-           })
-      .def("add_sigmoid_xent",
-           [](Plan& p, uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss,
-              uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
-             p.add("sigmoid_xent", [=](cudaStream_t st) {
-               return sf_sigmoid_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels,
-                                      P<float>(loss), P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t,
-                                      P<float>(dbias), rows, cols, st);
-             });
-           })
-      .def("add_argmax",
-           [](Plan& p, uintptr_t in, int ld, uintptr_t out, int rows, int cols) {
-             p.add("argmax", [=](cudaStream_t st) {
-               return sf_argmax_rows(P<const float>(in), ld, P<float>(out), rows, cols, st);
-             });
-           })
-      .def("add_im2col",
-           [](Plan& p, uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, int sh,
-              int sw, int pad_top, int pad_left, int out_h, int out_w) {
-             p.add("im2col", [=](cudaStream_t st) {
-               return sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
-                                     P<__nv_bfloat16>(out), ld_out, P<__nv_bfloat16>(outT), ld_t, st);
-             });
-           },
-           py::arg("in"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("out"), py::arg("ld_out"),
-           py::arg("outT"), py::arg("ld_t"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0,
-           py::arg("out_h") = 0, py::arg("out_w") = 0)
-      .def("add_col2im",
-           [](Plan& p, uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din, int sh, int sw, int pad_top,
-              int pad_left, int out_h, int out_w) {
-             p.add("col2im", [=](cudaStream_t st) {
-               return sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
-                                     P<__nv_bfloat16>(din), st);
-             });
-           },
-           py::arg("dcols"), py::arg("ld_cols"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"),
-           py::arg("din"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0, py::arg("out_h") = 0,
-           py::arg("out_w") = 0)
-      .def("add_maxpool_fwd",
-           [](Plan& p, uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintptr_t argmax, uintptr_t outT, int ld_t) {
-             p.add("maxpool_fwd", [=](cudaStream_t st) {
-               return sf_maxpool2_fwd(P<const __nv_bfloat16>(in), n, h, w, c, P<__nv_bfloat16>(out), P<uint8_t>(argmax),
-                                      P<__nv_bfloat16>(outT), ld_t, st);
-             });
-           })
-      .def("add_maxpool_bwd",
-           [](Plan& p, uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, uintptr_t act_out, int act, uintptr_t dz,
-              int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias) {
-             p.add("maxpool_bwd", [=](cudaStream_t st) {
-               return sf_maxpool2_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c,
-                                      P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT),
-                                      ld_t, P<float>(dbias), st);
-             });
-           })
-      .def("add_maxpool_gen_fwd",
-           [](Plan& p, uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
-              int out_w, uintptr_t out, uintptr_t argmax) {
-             p.add("maxpool_gen_fwd", [=](cudaStream_t st) {
-               return sf_maxpool_fwd(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
-                                     P<__nv_bfloat16>(out), P<uint8_t>(argmax), st);
-             });
-           })
-      .def("add_maxpool_gen_bwd",
-           [](Plan& p, uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
-              int pad_left, int out_h, int out_w, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
-             p.add("maxpool_gen_bwd", [=](cudaStream_t st) {
-               return sf_maxpool_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top,
-                                     pad_left, out_h, out_w, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz,
-                                     P<float>(dbias), st);
-             });
-           })
-      .def("add_act_bwd_bias",
-           [](Plan& p, uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
-             p.add("act_bwd_bias", [=](cudaStream_t st) {
-               return sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act,
-                                      P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
-             });
-           })
-      .def("add_conv_first_fwd",
-           [](Plan& p, uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act,
-              uintptr_t pooled, uintptr_t argmax, int pad_top, int pad_left, int out_h, int out_w) {
-             p.add("conv_first_fwd", [=](cudaStream_t st) {
-               return sf_conv_first_fwd(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(wT), ld_w, P<const float>(bias),
-                                        act, P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), pad_top, pad_left, out_h, out_w, st);
-             });
-           },
-           py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"), py::arg("wT"),
-           py::arg("ld_w"), py::arg("bias"), py::arg("act"), py::arg("pooled"), py::arg("argmax"), py::arg("pad_top") = 0,
-           py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0)
-      .def("add_conv_first_wgrad",
-           [](Plan& p, uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t g_pool, uintptr_t pooled, uintptr_t argmax,
-              int act, uintptr_t dW, uintptr_t db, int pad_top, int pad_left, int out_h, int out_w) {
-             p.add("conv_first_wgrad", [=](cudaStream_t st) {
-               return sf_conv_first_wgrad(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(g_pool),
-                                          P<const __nv_bfloat16>(pooled), P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), pad_top,
-                                          pad_left, out_h, out_w, st);
-             });
-           },
-           py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"),
-           py::arg("g_pool"), py::arg("pooled"), py::arg("argmax"), py::arg("act"), py::arg("dW"), py::arg("db"), py::arg("pad_top") = 0,
-           py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0)
-      .def("add_push",
-           [](Plan& p, const py::dict& d, uintptr_t local_sync, int grid) {
-             const SfPushArgs a = parse_push(d);
-             p.add("push", [=](cudaStream_t st) { return sf_push_launch(&a, P<uint32_t>(local_sync), grid, st); });
-           })
-      .def("add_post",
-           [](Plan& p, const py::dict& d, uintptr_t local_sync, int grid) {
-             const SfPostArgs a = parse_post(d);
-             p.add("post", [=](cudaStream_t st) { return sf_post_launch(&a, P<uint32_t>(local_sync), grid, st); });
-           })
-      .def("add_sync_pull", [](Plan& p, const py::dict& d) {
-        const SfSyncPullArgs a = parse_sync_pull(d);
-        p.add("sync_pull", [=](cudaStream_t st) { return sf_sync_pull_launch(&a, st); });
-      })
-      .def("add_post_flags", [](Plan& p, const py::dict& d) {
-        const SfPostFlagsArgs a = parse_post_flags(d);
-        p.add("post_flags", [=](cudaStream_t st) { return sf_post_flags_launch(&a, st); });
-      })
-      .def("add_pull", [](Plan& p, const py::dict& d, uintptr_t local_sync, int grid) {
-        const SfPullArgs a = parse_pull(d);
-        p.add("pull", [=](cudaStream_t st) { return sf_pull_launch(&a, P<uint32_t>(local_sync), grid, st); });
-      });
+           });
+
+  // every kernel below is a plan op (Plan.add_<first name>) and a direct entry point (_C.<second name>, used by tests and
+  // the eager paths)
+  def_kernel(m, plan, "cast_transpose", "cast_transpose", launch::cast_transpose);
+  def_kernel(m, plan, "softmax_xent", "softmax_xent", launch::softmax_xent);
+  def_kernel(m, plan, "mse", "mse_loss", launch::mse);
+  def_kernel(m, plan, "sigmoid_xent", "sigmoid_xent", launch::sigmoid_xent);
+  def_kernel(m, plan, "argmax", "argmax_rows", launch::argmax);
+  def_kernel(m, plan, "maxpool_fwd", "maxpool_fwd", launch::maxpool_fwd);
+  def_kernel(m, plan, "maxpool_bwd", "maxpool_bwd", launch::maxpool_bwd);
+  def_kernel(m, plan, "maxpool_gen_fwd", "maxpool_gen_fwd", launch::maxpool_gen_fwd);
+  def_kernel(m, plan, "maxpool_gen_bwd", "maxpool_gen_bwd", launch::maxpool_gen_bwd);
+  def_kernel(m, plan, "act_bwd_bias", "act_bwd_bias", launch::act_bwd_bias);
+  def_kernel(m, plan, "push", "push", launch::push);
+  def_kernel(m, plan, "post", "post", launch::post);
+  def_kernel(m, plan, "pull", "pull", launch::pull);
+  def_kernel(m, plan, "sync_pull", "sync_pull", launch::sync_pull);
+  def_kernel(m, plan, "post_flags", "post_flags", launch::post_flags);
+  // conv geometry (stride, pad_top / pad_left, output size) trails the stream argument; the defaults are VALID stride 1
+  const auto pads = std::make_tuple(py::arg("pad_top") = 0, py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0);
+  const auto geometry = std::tuple_cat(std::make_tuple(py::arg("sh") = 1, py::arg("sw") = 1), pads);
+  def_kernel(m, plan, "im2col", "im2col", launch::im2col,
+             std::make_tuple(py::arg("in"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("out"),
+                             py::arg("ld_out"), py::arg("outT"), py::arg("ld_t")),
+             geometry);
+  def_kernel(m, plan, "col2im", "col2im", launch::col2im,
+             std::make_tuple(py::arg("dcols"), py::arg("ld_cols"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"),
+                             py::arg("kw"), py::arg("din")),
+             geometry);
+  def_kernel(m, plan, "conv_first_fwd", "conv_first_fwd", launch::conv_first_fwd,
+             std::make_tuple(py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"),
+                             py::arg("wT"), py::arg("ld_w"), py::arg("bias"), py::arg("act"), py::arg("pooled"), py::arg("argmax")),
+             pads);
+  def_kernel(m, plan, "conv_first_wgrad", "conv_first_wgrad", launch::conv_first_wgrad,
+             std::make_tuple(py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"),
+                             py::arg("g_pool"), py::arg("pooled"), py::arg("argmax"), py::arg("act"), py::arg("dW"), py::arg("db")),
+             pads);
 
   py::class_<Applier>(m, "Applier")
       .def(py::init<const py::dict&, uintptr_t, size_t, uintptr_t, int, uintptr_t, double, int, int, int, uintptr_t, uintptr_t, const py::dict&>(), py::arg("push"), py::arg("mailboxes"),
@@ -1074,10 +1108,6 @@ PYBIND11_MODULE(_C, m) {
       .def("stop", &Applier::stop);
   m.attr("MB_WORDS") = static_cast<int>(SF_MB_WORDS);
   m.attr("MB_APPLIED") = static_cast<int>(SF_MB_APPLIED);
-  m.def("post", [](const py::dict& d, uintptr_t local_sync, int grid, uintptr_t stream) {
-    const SfPostArgs a = parse_post(d);
-    ck_rc(sf_post_launch(&a, P<uint32_t>(local_sync), grid, S(stream)), "post");
-  });
 
   py::class_<StepDriver>(m, "StepDriver")
       .def(py::init<uintptr_t, uintptr_t, uintptr_t, size_t, uintptr_t, size_t, uintptr_t, int>())
@@ -1090,125 +1120,9 @@ PYBIND11_MODULE(_C, m) {
       .def("host_ns", &StepDriver::host_ns)
       .def("probe", &StepDriver::probe);
 
-  // direct (un-planned) entry points, used by tests and the eager paths
-  m.def("cast_transpose", [](uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, uintptr_t outT,
-                             int ld_t, int rows, int cols, uintptr_t stream) {
-    ck_rc(idx ? sf_gather_cast_transpose(P<const float>(in), ld_in, P<const int32_t>(idx), P<__nv_bfloat16>(out),
-                                         ld_out, P<__nv_bfloat16>(outT), ld_t, rows, cols, S(stream))
-              : sf_cast_transpose(P<const float>(in), ld_in, P<__nv_bfloat16>(out), ld_out,
-                                  P<__nv_bfloat16>(outT), ld_t, rows, cols, S(stream)),
-          "cast_transpose");
-  });
-  m.def("softmax_xent", [](uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss,
-                           uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols,
-                           uintptr_t stream) {
-    ck_rc(sf_softmax_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss),
-                          P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols,
-                          S(stream)),
-          "softmax_xent");
-  });
-  m.def("mse_loss", [](uintptr_t out, int ld_out, uintptr_t target, int ld_target, int act, uintptr_t loss,
-                       uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols,
-                       uintptr_t stream) {
-    ck_rc(sf_mse_loss(P<const float>(out), ld_out, P<const float>(target), ld_target, act, P<float>(loss),
-                      P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols,
-                      S(stream)),
-          "mse_loss");
-  });
-  m.def("sigmoid_xent", [](uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss,
-                           uintptr_t dz, int ld_dz, uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols,
-                           uintptr_t stream) {
-    ck_rc(sf_sigmoid_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss),
-                          P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols,
-                          S(stream)),
-          "sigmoid_xent");
-  });
-  m.def("argmax_rows", [](uintptr_t in, int ld, uintptr_t out, int rows, int cols, uintptr_t stream) {
-    ck_rc(sf_argmax_rows(P<const float>(in), ld, P<float>(out), rows, cols, S(stream)), "argmax_rows");
-  });
-  m.def("push", [](const py::dict& d, uintptr_t local_sync, int grid, uintptr_t stream) {
-    const SfPushArgs a = parse_push(d);
-    ck_rc(sf_push_launch(&a, P<uint32_t>(local_sync), grid, S(stream)), "push");
-  });
-  m.def("pull", [](const py::dict& d, uintptr_t local_sync, int grid, uintptr_t stream) {
-    const SfPullArgs a = parse_pull(d);
-    ck_rc(sf_pull_launch(&a, P<uint32_t>(local_sync), grid, S(stream)), "pull");
-  });
   m.def("lock_op", [](uintptr_t ctrl, int op, uintptr_t stream) {
     ck_rc(sf_lock_test(P<uint32_t>(ctrl), op, S(stream)), "lock_op");
   });
-  // conv geometry (stride, pad_top / pad_left, output size) trails the stream argument; the defaults are VALID stride 1
-  m.def(
-      "im2col",
-      [](uintptr_t in, int n, int h, int w, int c, int kh, int kw, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, uintptr_t stream, int sh,
-         int sw, int pad_top, int pad_left, int out_h, int out_w) {
-        ck_rc(sf_im2col_nhwc(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w, P<__nv_bfloat16>(out),
-                             ld_out, P<__nv_bfloat16>(outT), ld_t, S(stream)),
-              "im2col");
-      },
-      py::arg("in"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("out"), py::arg("ld_out"),
-      py::arg("outT"), py::arg("ld_t"), py::arg("stream"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0,
-      py::arg("out_h") = 0, py::arg("out_w") = 0);
-  m.def(
-      "col2im",
-      [](uintptr_t dcols, int ld_cols, int n, int h, int w, int c, int kh, int kw, uintptr_t din, uintptr_t stream, int sh, int sw, int pad_top,
-         int pad_left, int out_h, int out_w) {
-        ck_rc(sf_col2im_nhwc(P<const __nv_bfloat16>(dcols), ld_cols, n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
-                             P<__nv_bfloat16>(din), S(stream)),
-              "col2im");
-      },
-      py::arg("dcols"), py::arg("ld_cols"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("c"), py::arg("kh"), py::arg("kw"), py::arg("din"),
-      py::arg("stream"), py::arg("sh") = 1, py::arg("sw") = 1, py::arg("pad_top") = 0, py::arg("pad_left") = 0, py::arg("out_h") = 0,
-      py::arg("out_w") = 0);
-  m.def("maxpool_fwd", [](uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintptr_t argmax, uintptr_t outT, int ld_t, uintptr_t stream) {
-    ck_rc(sf_maxpool2_fwd(P<const __nv_bfloat16>(in), n, h, w, c, P<__nv_bfloat16>(out), P<uint8_t>(argmax), P<__nv_bfloat16>(outT), ld_t, S(stream)), "maxpool_fwd");
-  });
-  m.def("maxpool_bwd", [](uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz,
-                          uintptr_t dzT, int ld_t, uintptr_t dbias, uintptr_t stream) {
-    ck_rc(sf_maxpool2_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, P<const __nv_bfloat16>(act_out), act,
-                          P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), S(stream)), "maxpool_bwd");
-  });
-  m.def("maxpool_gen_fwd", [](uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
-                              int out_w, uintptr_t out, uintptr_t argmax, uintptr_t stream) {
-    ck_rc(sf_maxpool_fwd(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w, P<__nv_bfloat16>(out),
-                         P<uint8_t>(argmax), S(stream)),
-          "maxpool_gen_fwd");
-  });
-  m.def("maxpool_gen_bwd", [](uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
-                              int pad_left, int out_h, int out_w, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias,
-                              uintptr_t stream) {
-    ck_rc(sf_maxpool_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
-                         P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), S(stream)),
-          "maxpool_gen_bwd");
-  });
-  m.def("act_bwd_bias", [](uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias,
-                           uintptr_t stream) {
-    ck_rc(sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz,
-                          P<float>(dbias), S(stream)),
-          "act_bwd_bias");
-  });
-  m.def(
-      "conv_first_fwd",
-      [](uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act, uintptr_t pooled,
-         uintptr_t argmax, uintptr_t stream, int pad_top, int pad_left, int out_h, int out_w) {
-        ck_rc(sf_conv_first_fwd(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(wT), ld_w, P<const float>(bias), act,
-                                P<__nv_bfloat16>(pooled), P<uint8_t>(argmax), pad_top, pad_left, out_h, out_w, S(stream)),
-              "conv_first_fwd");
-      },
-      py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"), py::arg("wT"),
-      py::arg("ld_w"), py::arg("bias"), py::arg("act"), py::arg("pooled"), py::arg("argmax"), py::arg("stream"), py::arg("pad_top") = 0,
-      py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0);
-  m.def(
-      "conv_first_wgrad",
-      [](uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t g_pool, uintptr_t pooled, uintptr_t argmax, int act,
-         uintptr_t dW, uintptr_t db, uintptr_t stream, int pad_top, int pad_left, int out_h, int out_w) {
-        ck_rc(sf_conv_first_wgrad(P<const __nv_bfloat16>(x), n, h, w, cin, kh, kw, cout, P<const __nv_bfloat16>(g_pool), P<const __nv_bfloat16>(pooled),
-                                  P<const uint8_t>(argmax), act, P<float>(dW), P<float>(db), pad_top, pad_left, out_h, out_w, S(stream)),
-              "conv_first_wgrad");
-      },
-      py::arg("x"), py::arg("n"), py::arg("h"), py::arg("w"), py::arg("cin"), py::arg("kh"), py::arg("kw"), py::arg("cout"), py::arg("g_pool"),
-      py::arg("pooled"), py::arg("argmax"), py::arg("act"), py::arg("dW"), py::arg("db"), py::arg("stream"), py::arg("pad_top") = 0,
-      py::arg("pad_left") = 0, py::arg("out_h") = 0, py::arg("out_w") = 0);
   m.def("gemm_pick_bn", &sf_gemm_pick_bn);
   m.def("set_pdl", &sf_set_pdl);
   m.def("trace_enable", [](uintptr_t buf, unsigned int cap) { ck_rc(sf_trace_enable(P<void>(buf), cap), "trace_enable"); });
@@ -1225,14 +1139,6 @@ PYBIND11_MODULE(_C, m) {
   m.def("pack_route", &pack_route);
   m.def("pack_ryw", &pack_ryw);
   m.attr("MAX_SHARDS") = static_cast<int>(SF_MAX_SHARDS);
-  m.def("sync_pull", [](const py::dict& d, uintptr_t stream) {
-    const SfSyncPullArgs a = parse_sync_pull(d);
-    ck_rc(sf_sync_pull_launch(&a, S(stream)), "sync_pull");
-  });
-  m.def("post_flags", [](const py::dict& d, uintptr_t stream) {
-    const SfPostFlagsArgs a = parse_post_flags(d);
-    ck_rc(sf_post_flags_launch(&a, S(stream)), "post_flags");
-  });
   // symmetric (VMM) memory + NVSwitch multicast
   m.def("vmm_granularity", &sfvmm::granularity, py::arg("device"), py::arg("multicast") = false, py::arg("n_devices") = 1);
   m.def("vmm_multicast_supported", &sfvmm::multicast_supported);
