@@ -241,7 +241,7 @@ maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __rest
   const int oh = h / 2, ow = w / 2;
   const int M = n * h * w;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const int c0 = blockIdx.x * 32, m0 = blockIdx.y * 32;
+  const int m0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   if (threadIdx.x < 32) s_col[threadIdx.x] = 0.f;
   __syncthreads();
   float cacc = 0.f;
@@ -458,7 +458,7 @@ extern "C" int sf_maxpool2_bwd(const __nv_bfloat16* dout, const uint8_t* argmax,
                                float* dbias, cudaStream_t st) {
   const int M = n * h * w;
   const int span_c = (dz && ld_dz > c) ? ld_dz : c;
-  dim3 grid((span_c + 31) / 32, (M + 31) / 32);
+  dim3 grid((M + 31) / 32, (span_c + 31) / 32);     // rows on grid.x: a large batch outgrows grid.y's 65535 blocks
   return static_cast<int>(sf::launch(sf::maxpool_bwd_kernel, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, act_out, act, dz,
                                      ld_dz, dzT, ld_t, dbias));
 }

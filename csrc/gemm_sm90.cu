@@ -688,10 +688,11 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->bn > 64) g->bn = 64;    // the widest tile of its variant
   if (g->split_k <= 0) g->split_k = 1;
-  // large, un-split problems go to the persistent cluster-pair kernel (gemm_pair_sm90.cu): 256 x 128 tiles per CTA pair
+  // large, un-split problems go to the persistent cluster-pair kernel (gemm_pair_sm90.cu): 256 x 128 tiles per CTA pair.
+  // A GEMM that carries the fused read-your-writes wait stays on the one-CTA kernel, the only one that implements it.
   {
     const long long pair_tiles = static_cast<long long>((g->M + 255) / 256) * ((g->N + sf::kPairBN - 1) / sf::kPairBN);
-    const bool eligible = g->split_k == 1 && g->ep.loss_mode == SF_LOSS_NONE && g->M >= 256 && g->N >= 256;
+    const bool eligible = g->split_k == 1 && g->ep.loss_mode == SF_LOSS_NONE && g->ep.ryw == nullptr && g->M >= 256 && g->N >= 256;
     const char* env = getenv("SPARKFLOW_GEMM_PAIR");
     int want = g->pair;
     if (env != nullptr && want < 0) want = atoi(env);
@@ -699,6 +700,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
     g->pair = (want > 0 && eligible && !g->mn_major) ? 1 : 0;
     if (g->pair) g->bn = sf::kPairBN;
   }
+  if (!g->pair && (g->M + sf::kBM - 1) / sf::kBM > 65535) return -2;     // the one-CTA grid puts M tiles on grid.y
   int rc;
   if (g->mn_major) {
     // a is [K, lda] (M contiguous), b is [K, ldb] (N contiguous): boxes of {64 MN elements, 64 K rows}

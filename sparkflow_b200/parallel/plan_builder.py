@@ -387,13 +387,14 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 d.update(out_f32=P(out_f32), ld_f32=ks.cols)
             g = C.Gemm(d)
             emit(g, f"fwd{i}" + ("+loss" if fuse_loss else ""))
-            rec[i]["N"] = ks.cols
+            rec[i].update(N=ks.cols, fwd=g)
             break
         nxt = zeros(B, round_up(ks.cols, 8))
         nxtT = zeros(ks.cols, ldB) if (train and not use_mn) else None
         d.update(out_bf16=P(nxt), ld_bf16=nxt.shape[1], outT_bf16=P(nxtT), ld_t=ldB if nxtT is not None else 0)
         g = C.Gemm(d)
         emit(g, f"fwd{i}")
+        rec[i]["fwd"] = g
         cur = dict(kind="flat", buf=nxt, bufT=nxtT, feat=ks.cols, ld=nxt.shape[1])
 
     result = None
@@ -478,6 +479,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                           colsum=P(worker.grads) + pb.offset * 4 if pb else 0)
                 dg = C.Gemm(dd)
                 emit(dg, f"dgrad{i}")
+                r["dgrad"] = dg
                 g_dz, g_dzT = ndz, ndzT
             else:                                  # flatten over an image: gradient wrt the pooled tensor / the conv activation
                 g_img = zeros(B, ks.rows)

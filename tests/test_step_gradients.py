@@ -40,6 +40,11 @@ MODELS = {
     "cnn_same": ({}, "onehot"),
     "cnn_strided": ({}, "onehot"),
 }
+# larger configurations of zoo models, run only at the large batch sizes below: name -> (zoo name, zoo kwargs, label kind)
+LARGE_MODELS = {
+    "wide_dnn_1024": ("wide_dnn", dict(width=1024, depth=2, classes=100), "onehot"),
+    "wide_dnn_bench": ("wide_dnn", {}, "onehot"),          # bench.py's flagship: 4096 x 4, 1000 classes
+}
 DENSE = [m for m in MODELS if not m.startswith("cnn")]
 CNNS = [m for m in MODELS if m.startswith("cnn")]
 
@@ -111,6 +116,10 @@ TOL = {                                  # measured: per-step test; delivered-gr
     "test_autoencoder": (1e-5, 1e-5),    # 1.6e-6, 1.7e-6
     "fixture_mlp": (1e-5, 1e-5),         # 1.1e-6, 1.1e-6
     "wide_dnn": (2.5e-3, 9e-3),          # 7.8e-4, 2.9e-3
+    # the large-batch cases, measured on an H100 80GB HBM3 (700 W power limit): the 1024-wide model at B = 4353 (step,
+    # sharded delivery), the benchmark's 4096 x 4 model at B = 300 and 1025
+    "wide_dnn_1024": (6e-4, 9e-4),       # 1.8e-4, 2.3e-4; 1.9e-4, 2.8e-4
+    "wide_dnn_bench": (9e-3, 1e-2),      # 3.0e-3, 3.1e-3
     "cnn": (7e-4, 2.5e-3),               # 2.2e-4, 7.6e-4
     "cnn_same": (2.5e-3, 7e-3),          # 7.8e-4, 2.1e-3
     "cnn_strided": (6e-4, 1.5e-3),       # 1.8e-4, 4.8e-4; 4.2e-4, 9.7e-4
@@ -143,8 +152,8 @@ def _model(name):
             fn, kind = DROP_MODELS[name]
             ir = GraphIR.from_metagraph(build_graph(fn))
         else:
-            kw, kind = MODELS[name]
-            ir = GraphIR.from_metagraph(zoo.build(name, **kw))
+            zname, kw, kind = LARGE_MODELS[name] if name in LARGE_MODELS else (name, *MODELS[name])
+            ir = GraphIR.from_metagraph(zoo.build(zname, **kw))
         label = "y:0" if kind else None
         _MODEL_CACHE[name] = (ir, compile_graph(ir, "x:0", label), label)
     return _MODEL_CACHE[name]
@@ -152,7 +161,7 @@ def _model(name):
 
 def _data(name, n, seed):
     _, lp, _ = _model(name)
-    kind = (DROP_MODELS if name in DROP_MODELS else MODELS)[name][1]
+    kind = LARGE_MODELS[name][2] if name in LARGE_MODELS else (DROP_MODELS if name in DROP_MODELS else MODELS)[name][1]
     rng = np.random.default_rng(seed)
     X = rng.random((n, lp.input_dim), dtype=np.float32)
     if kind == "onehot":
@@ -714,18 +723,26 @@ def _recorded_relu_mask(lp, dbg, B):
 
 def _check_pools(tag, lp, dbg, pools, B):
     """Each recorded winner holds its window's maximum: exactly on the step's own bf16 conv output where the plan keeps
-    it, and up to fp32 accumulation order on the oracle's activation (the fused first conv never stores it)."""
+    it, and on the oracle's activation up to fp32 accumulation order (the fused first conv never stores it) plus, where
+    the oracle's activation is its own bf16 store, one bf16 rounding step of it (a near-tie the two roundings order
+    differently: at B = 3700 cnn meets two such windows among 5.9 million)."""
     for i, (a, idx) in pools.items():
         l = lp.layers[i]
+        r = dbg[i]
         win = _pool_gather(a, l, idx)
         best = _pool_gather(a, l, _pool_argmax(a, l))
-        slack = 1e-4 * max(1.0, float(best.abs().max()))
-        assert bool((win >= best - slack).all()), f"{tag}: pool layer {i} routes a gradient to a cell below its window maximum"
-        r = dbg[i]
+        slack = torch.full_like(best, 1e-4 * max(1.0, float(best.abs().max())))
         if not r.get("fused"):
             act = dbg[r["conv"]]["act_out"].to(DEV).double().reshape(B, *l.in_shape)
             assert torch.equal(idx, _pool_argmax(act, l)), f"{tag}: pool layer {i} did not pick the first maximum of its window"
             assert torch.equal(_pool_gather(act, l, idx), r["pooled"].to(DEV).double().reshape(B, *l.out_shape)), tag
+            step = torch.ldexp((best != 0).to(best.dtype), torch.frexp(best)[1] - 8)      # one bf16 step at |best|
+            slack = torch.maximum(slack, step)
+        below = best - win
+        k = int(below.argmax())
+        assert bool((below <= slack).all()), (f"{tag}: pool layer {i} routes a gradient to a cell below its window maximum: "
+                                              f"{float(below.flatten()[k]):.3e} below {float(best.flatten()[k]):.6e} "
+                                              f"({int((below > slack).sum())} windows), slack {float(slack.flatten()[k]):.1e}")
 
 
 def _compare_step(tag, lp, w, X, Y, got, loss, dbg, tol, drop_mask=None, loss_tol=LOSS_TOL):
@@ -1092,3 +1109,143 @@ def test_delivered_gradients_match_oracle(name, mode):
         master.close()
     if name in CNNS:
         assert split == {False, True}, f"{name}/{mode}: the batch sizes must switch the split-K conv weight gradient on and off"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# large batches: the size-dependent kernel choices the batch sizes above never reach
+# ------------------------------------------------------------------------------------------------------------------
+def _first_pair_batch(width, sms):
+    """the smallest B at which sf_gemm_prepare sends a B x width x width GEMM (K >= 512) to the cluster-pair kernel:
+    sf_gemm_pick_bn picks 256 columns (ceil(B / 128) * ceil(width / 256) >= SMs) and there are at least SMs / 2 pair
+    tiles of 256 x 128"""
+    B = 1
+    while -(-B // 128) * -(-width // 256) < sms or -(-B // 256) * -(-width // 128) < sms // 2:
+        B += 1
+    return B
+
+
+def _dense_gemms(lp, dbg, kind):
+    return [dbg[i][kind] for i, l in enumerate(lp.layers) if l.kind == "dense" and kind in dbg[i]]
+
+
+def _assert_pair_gemms(tag, lp, dbg):
+    """at least one forward and one dgrad GEMM of the step ran on the cluster-pair kernel"""
+    assert any(g.pair for g in _dense_gemms(lp, dbg, "fwd")), f"{tag}: no forward GEMM on the pair kernel"
+    assert any(g.pair for g in _dense_gemms(lp, dbg, "dgrad")), f"{tag}: no dgrad GEMM on the pair kernel"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant", ["default", "unfused_loss"])
+def test_large_batch_wide_step_matches_oracle(variant, monkeypatch):
+    """A 1024-wide, 2-deep, 100-class MLP at B = 32 * SMs + 129: its 1024 x 1024 forward and dgrad GEMMs run on the
+    cluster-pair kernel, the last pair tile row holds 1 row (rank 1 of it entirely out of bounds) on 132 SMs, and the
+    stand-alone softmax cross-entropy has more rows than its capped grid has warps (the grid-stride loop)."""
+    from sparkflow_b200.ops import native
+
+    for k, v in VARIANTS[variant].items():
+        monkeypatch.setenv(k, v)
+    name = "wide_dnn_1024"
+    _, lp, _ = _model(name)
+    w = _weights(name)
+    B = 32 * native.num_sms() + 129
+    master, worker = _worker(name, w)
+    try:
+        X, Y = _data(name, B, seed=B)
+        got, loss, dbg, names = _run_step(worker, B, X, Y, "staged")
+        _expected_kernels(name, variant, names, dbg, lp)
+        assert "softmax_xent" in [n.split("@")[0] for n in names]
+        _assert_pair_gemms(f"{name} B={B}", lp, dbg)
+        _compare_step(f"{name}/{variant} B={B}", lp, w, X, Y, got, loss, dbg, TOL[name])
+    finally:
+        master.close()
+
+
+@pytest.mark.gpu
+def test_benchmark_wide_dnn_step_matches_oracle():
+    """bench.py's flagship model (4096 x 4, 1000 classes: K = 4096 GEMMs, an N = 1000 weight-gradient tail, a 1000-class
+    softmax) at the benchmark's batch of 300 and at the smallest batch whose 4096-wide GEMMs run on the pair kernel
+    (1025 on 132 SMs: the last pair tile holds one row)."""
+    from sparkflow_b200.ops import native
+
+    name = "wide_dnn_bench"
+    _, lp, _ = _model(name)
+    w = _weights(name)
+    B_pair = _first_pair_batch(4096, native.num_sms())
+    master, worker = _worker(name, w)
+    try:
+        for B in (300, B_pair):
+            X, Y = _data(name, B, seed=B)
+            got, loss, dbg, names = _run_step(worker, B, X, Y, "staged")
+            _expected_kernels(name, "default", names, dbg, lp)
+            if B == B_pair:
+                _assert_pair_gemms(f"{name} B={B}", lp, dbg)
+            _compare_step(f"{name} B={B}", lp, w, X, Y, got, loss, dbg, TOL[name])
+    finally:
+        master.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,variant,B", [("cnn", "lowered_conv1", 3700), ("cnn", "kmajor_wgrad", 3700), ("cnn_same", "lowered_conv1", 2700)])
+def test_large_batch_cnn_step_matches_oracle(name, variant, B, monkeypatch):
+    """The first 2x2 max-pool of a lowered first conv with more than 65535 * 32 rows: its backward has more 32-row blocks
+    than a grid's y dimension holds."""
+    for k, v in VARIANTS[variant].items():
+        monkeypatch.setenv(k, v)
+    _, lp, _ = _model(name)
+    pool = min(i for i, l in enumerate(lp.layers) if l.kind == "pool")
+    h, w_, _ = lp.layers[pool].in_shape
+    assert B * h * w_ > 65535 * 32, (B, h, w_)
+    w = _weights(name)
+    master, worker = _worker(name, w)
+    try:
+        X, Y = _data(name, B, seed=B)
+        got, loss, dbg, names = _run_step(worker, B, X, Y, "staged")
+        _expected_kernels(name, variant, names, dbg, lp)
+        assert "maxpool_bwd" in [n.split("@")[0] for n in names], names
+        _compare_step(f"{name}/{variant} B={B}", lp, w, X, Y, got, loss, dbg, TOL[name])
+    finally:
+        master.close()
+
+
+@pytest.mark.gpu
+def test_sharded_hogwild_step_keeps_its_wait_off_the_pair_kernel():
+    """3 Hogwild shards, where the read-your-writes wait rides in the step's first GEMM.  At B = 32 * SMs + 129 the
+    1024-wide model's fwd0 (which carries the wait) and fwd1 have the same shape, so fwd1 on the pair kernel and fwd0 on
+    the one-CTA kernel shows that the wait alone kept fwd0 off it (the pair kernel has no wait).  Then one delivered step:
+    within the model's tolerance of the oracle and within DELIVERY_TOL of the same step without push."""
+    from sparkflow_b200.ops import native
+
+    name = "wide_dnn_1024"
+    cfg = TAP_MODES["sharded3"]
+    _, lp, _ = _model(name)
+    w = _weights(name)
+    B = 32 * native.num_sms() + 129
+    X, Y = _data(name, B, seed=61)
+    master, worker = _worker(name, w)
+    try:
+        plain = _run_step(worker, B, X, Y, "in_graph")[0]
+    finally:
+        master.close()
+    spec = OptimizerSpec.from_tf_kwargs("momentum", dict(learning_rate=0.0, momentum=0.0))
+    master, worker = _worker(name, w, spec, **cfg)
+    try:
+        plan, bufs = worker.build_plan(B, 0, with_pull=True, with_push=True)
+        dbg, names = worker.last_debug, worker.last_plan_names()
+        _check_tap_coverage(f"{name}/sharded3", name, lp, master, worker, names, cfg)
+        f0, f1 = _dense_gemms(lp, dbg, "fwd")[:2]
+        assert lp.layers[0].kind == "dense" and lp.input_dim == lp.layers[0].out_shape[0], "fwd0 and fwd1 must have one shape"
+        assert f1.pair == 1, "the shape must be pair-eligible"
+        assert f0.pair == 0, "the GEMM carrying the read-your-writes wait went to the pair kernel"
+        with torch.cuda.stream(worker.stream):
+            bufs.x_stage.copy_(torch.from_numpy(X))
+            bufs.y_stage.copy_(torch.from_numpy(Y))
+            plan.run(worker.stream.cuda_stream)
+        worker.drain()
+        assert wait_pushes(master, 1) == 1
+        got = master.slot_arrays()[0]
+        _compare_step(f"{name}/sharded3 B={B}", lp, w, X, Y, got, float(bufs.loss_out[0]), dbg, TOL[name])
+        delivery = max(_errors(g, r)[0] for g, r in zip(got, plain))
+        print(f"[step-grad] {name}/sharded3 B={B}: against the same step without push: rel-Frobenius {delivery:.2e}")
+        assert delivery <= DELIVERY_TOL, f"the delivered gradient differs from the step's own by {delivery:.2e}"
+    finally:
+        master.close()
