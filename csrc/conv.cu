@@ -227,11 +227,18 @@ __device__ __forceinline__ float pool_dact(float a, int act) {
     default: return 1.f;
   }
 }
+// EXT: the backward kernels' twins for the extended activations (SfAct 4-9, alpha = a leaky ReLU's slope); the launchers
+// pick a twin exactly when act is one of them, so the ReLU / sigmoid / tanh kernels keep their code.
+template <bool EXT>
+__device__ __forceinline__ float pool_dact(float a, int act, float alpha) {
+  return EXT ? act_ext_dact(a, act, alpha) : pool_dact(a, act);
+}
 
-__global__ void __launch_bounds__(256)
-maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c,
-                   const __nv_bfloat16* __restrict__ act_out, int act, __nv_bfloat16* __restrict__ dz, int ld_dz,
-                   __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias) {
+template <bool EXT>
+__device__ __forceinline__ void maxpool_bwd_tile(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h,
+                                                 int w, int c, const __nv_bfloat16* __restrict__ act_out, int act, float alpha,
+                                                 __nv_bfloat16* __restrict__ dz, int ld_dz, __nv_bfloat16* __restrict__ dzT, int ld_t,
+                                                 float* __restrict__ dbias) {
   __shared__ __nv_bfloat16 tile[32][34];
   __shared__ float s_col[32];
   TraceScope trace;
@@ -256,7 +263,7 @@ maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __rest
       if (py < oh && px < ow) {
         const size_t o = ((static_cast<size_t>(b) * oh + py) * ow + px) * c + cc;
         if (argmax[o] == ((y & 1) * 2 + (x & 1)))
-          g = __bfloat162float(dout[o]) * pool_dact(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act);
+          g = __bfloat162float(dout[o]) * pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha);
       }
     }
     const __nv_bfloat16 gb = __float2bfloat16(g);
@@ -276,6 +283,19 @@ maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __rest
     }
   }
   trace.end(KID_POOL_BWD);
+}
+
+__global__ void __launch_bounds__(256)
+maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c,
+                   const __nv_bfloat16* __restrict__ act_out, int act, __nv_bfloat16* __restrict__ dz, int ld_dz,
+                   __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias) {
+  maxpool_bwd_tile<false>(dout, argmax, n, h, w, c, act_out, act, 0.f, dz, ld_dz, dzT, ld_t, dbias);
+}
+__global__ void __launch_bounds__(256)
+maxpool_bwd_ext_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c,
+                       const __nv_bfloat16* __restrict__ act_out, int act, float alpha, __nv_bfloat16* __restrict__ dz, int ld_dz,
+                       __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias) {
+  maxpool_bwd_tile<true>(dout, argmax, n, h, w, c, act_out, act, alpha, dz, ld_dz, dzT, ld_t, dbias);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -324,10 +344,11 @@ maxpool_gen_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w
 //                    of dout[b, py, px, c]
 // (overlapping windows: a position collects the gradient of every window it won).  Row-major dz [M, ld_dz] and the
 // column sums over M into dbias[C]; one 32(m) x 32(c) tile per CTA, M tiles on x.
-__global__ void __launch_bounds__(256)
-maxpool_gen_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c, int kh, int kw,
-                       int sh, int sw, int pt, int pl, int oh, int ow, const __nv_bfloat16* __restrict__ act_out, int act,
-                       __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+template <bool EXT>
+__device__ __forceinline__ void maxpool_gen_bwd_tile(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n,
+                                                     int h, int w, int c, int kh, int kw, int sh, int sw, int pt, int pl, int oh, int ow,
+                                                     const __nv_bfloat16* __restrict__ act_out, int act, float alpha,
+                                                     __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
   __shared__ float s_col[32];
   TraceScope trace;
   pdl_launch_dependents();
@@ -357,7 +378,7 @@ maxpool_gen_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __
           if (argmax[o] == dy * kw + (xp - px * sw)) g += __bfloat162float(dout[o]);
         }
       }
-      if (g != 0.f) g *= pool_dact(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act);
+      if (g != 0.f) g *= pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha);
     }
     cacc += g;
     if (dz != nullptr && m < M && cc < ld_dz) dz[static_cast<size_t>(m) * ld_dz + cc] = __float2bfloat16(g);
@@ -369,14 +390,29 @@ maxpool_gen_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __
   trace.end(KID_POOL_GEN_BWD);
 }
 
+__global__ void __launch_bounds__(256)
+maxpool_gen_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c, int kh, int kw,
+                       int sh, int sw, int pt, int pl, int oh, int ow, const __nv_bfloat16* __restrict__ act_out, int act,
+                       __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+  maxpool_gen_bwd_tile<false>(dout, argmax, n, h, w, c, kh, kw, sh, sw, pt, pl, oh, ow, act_out, act, 0.f, dz, ld_dz, dbias);
+}
+// (256, 4): under the plain bound ptxas kept this twin at 32 registers and spilled 48 bytes; it needs 52
+__global__ void __launch_bounds__(256, 4)
+maxpool_gen_bwd_ext_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c, int kh,
+                           int kw, int sh, int sw, int pt, int pl, int oh, int ow, const __nv_bfloat16* __restrict__ act_out, int act,
+                           float alpha, __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+  maxpool_gen_bwd_tile<true>(dout, argmax, n, h, w, c, kh, kw, sh, sw, pt, pl, oh, ow, act_out, act, alpha, dz, ld_dz, dbias);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Activation gradient of a conv with no pool after it: dz[m, c] = g[m, c] * act'(a[m, c]) written row-major [M, ld_dz], and
 // the column sums over M added into dbias[C].  g is the gradient wrt the conv's activation output: col2im of the next conv
 // or the flatten dgrad of the dense layer above.  Same 32(m) x 32(c) tile and s_col reduction as maxpool_bwd_kernel.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-act_bwd_bias_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c, const __nv_bfloat16* __restrict__ act_out, int act,
-                    __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+template <bool EXT>
+__device__ __forceinline__ void act_bwd_bias_tile(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c,
+                                                  const __nv_bfloat16* __restrict__ act_out, int act, float alpha,
+                                                  __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
   __shared__ float s_col[32];
   TraceScope trace;
   pdl_launch_dependents();
@@ -392,7 +428,8 @@ act_bwd_bias_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c,
     const int m = m0 + ty + 8 * i, cc = c0 + tx;
     float v = 0.f;
     if (m < M && cc < c)
-      v = __bfloat162float(g[static_cast<size_t>(m) * ld_g + cc]) * pool_dact(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act);
+      v = __bfloat162float(g[static_cast<size_t>(m) * ld_g + cc]) *
+          pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha);
     cacc += v;
     if (dz != nullptr && m < M && cc < ld_dz) dz[static_cast<size_t>(m) * ld_dz + cc] = __float2bfloat16(v);
   }
@@ -401,6 +438,17 @@ act_bwd_bias_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c,
   if (dbias != nullptr && threadIdx.x < 32 && c0 + threadIdx.x < c && s_col[threadIdx.x] != 0.f)
     atomicAdd(dbias + c0 + threadIdx.x, s_col[threadIdx.x]);
   trace.end(KID_ACT_BWD);
+}
+
+__global__ void __launch_bounds__(256)
+act_bwd_bias_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c, const __nv_bfloat16* __restrict__ act_out, int act,
+                    __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+  act_bwd_bias_tile<false>(g, ld_g, M, c, act_out, act, 0.f, dz, ld_dz, dbias);
+}
+__global__ void __launch_bounds__(256)
+act_bwd_bias_ext_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c, const __nv_bfloat16* __restrict__ act_out, int act,
+                        float alpha, __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+  act_bwd_bias_tile<true>(g, ld_g, M, c, act_out, act, alpha, dz, ld_dz, dbias);
 }
 
 }  // namespace sf
@@ -454,11 +502,14 @@ extern "C" int sf_maxpool2_fwd(const __nv_bfloat16* in, int n, int h, int w, int
 }
 
 extern "C" int sf_maxpool2_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c,
-                               const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
-                               float* dbias, cudaStream_t st) {
+                               const __nv_bfloat16* act_out, int act, float act_alpha, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT,
+                               int ld_t, float* dbias, cudaStream_t st) {
   const int M = n * h * w;
   const int span_c = (dz && ld_dz > c) ? ld_dz : c;
   dim3 grid((M + 31) / 32, (span_c + 31) / 32);     // rows on grid.x: a large batch outgrows grid.y's 65535 blocks
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::maxpool_bwd_ext_kernel, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, act_out, act, act_alpha,
+                                       dz, ld_dz, dzT, ld_t, dbias));
   return static_cast<int>(sf::launch(sf::maxpool_bwd_kernel, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, act_out, act, dz,
                                      ld_dz, dzT, ld_t, dbias));
 }
@@ -473,21 +524,27 @@ extern "C" int sf_maxpool_fwd(const __nv_bfloat16* in, int n, int h, int w, int 
 }
 
 extern "C" int sf_maxpool_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw,
-                              int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz,
-                              int ld_dz, float* dbias, cudaStream_t st) {
+                              int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, float act_alpha,
+                              __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st) {
   if (kh < 1 || kw < 1 || kh > 4 || kw > 4 || sh < 1 || sw < 1) return -8;
   conv_out_size(h, w, kh, kw, sh, sw, out_h, out_w);
   const int M = n * h * w;
   const int span_c = (dz && ld_dz > c) ? ld_dz : c;
   dim3 grid((M + 31) / 32, (span_c + 31) / 32);
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::maxpool_gen_bwd_ext_kernel, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, kh, kw, sh, sw,
+                                       pad_top, pad_left, out_h, out_w, act_out, act, act_alpha, dz, ld_dz, dbias));
   return static_cast<int>(sf::launch(sf::maxpool_gen_bwd_kernel, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, kh, kw, sh, sw, pad_top,
                                      pad_left, out_h, out_w, act_out, act, dz, ld_dz, dbias));
 }
 
-extern "C" int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz,
-                               int ld_dz, float* dbias, cudaStream_t st) {
+extern "C" int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, float act_alpha,
+                               __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st) {
   const int span_c = (dz && ld_dz > c) ? ld_dz : c;
   dim3 grid((rows + 31) / 32, (span_c + 31) / 32);
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::act_bwd_bias_ext_kernel, grid, dim3(256), 0, st, g, ld_g, rows, c, act_out, act, act_alpha, dz,
+                                       ld_dz, dbias));
   return static_cast<int>(sf::launch(sf::act_bwd_bias_kernel, grid, dim3(256), 0, st, g, ld_g, rows, c, act_out, act, dz, ld_dz, dbias));
 }
 

@@ -26,6 +26,10 @@ __device__ __forceinline__ float dact_from_out(float a, int act) {
     default: return 1.f;
   }
 }
+// with the extended set (SfAct 4-9)
+__device__ __forceinline__ float dact_from_out(float a, int act, float alpha) {
+  return act >= SF_ACT_ELU ? act_ext_dact(a, act, alpha) : dact_from_out(a, act);
+}
 
 // ---------------------------------------------------------------------------
 // fp32 -> bf16 cast with optional row gather and transposed copy.  32x32 tiles through smem so
@@ -133,11 +137,13 @@ softmax_xent_kernel(const float* __restrict__ logits, int ld_logits, const float
 // head maps (network output o, target t) to a loss term and dz:
 //   MseHead          loss += mean((o - t)^2), dz = 2 (o - t) / (rows * cols) * act'(o)   (o after activation `act`)
 //   SigmoidXentHead  loss += mean(max(o, 0) - o t + log1p(exp(-|o|))), dz = (sigmoid(o) - t) / (rows * cols)  (raw logits)
+//   MseExtHead       MseHead for the extended activations (SfAct 4-9; alpha: a leaky ReLU's slope), its own kernel so
+//                    that the MSE kernel of ReLU / sigmoid / tanh outputs keeps its code
 // ---------------------------------------------------------------------------
 struct MseHead {
   static constexpr int kKid = KID_MSE;
   __device__ static float scale(int rows, int cols) { return 2.f / (static_cast<float>(rows) * static_cast<float>(cols)); }
-  __device__ static float grad(float o, float t, int act, float scale, float& lacc) {
+  __device__ static float grad(float o, float t, int act, float, float scale, float& lacc) {
     const float d = o - t;
     lacc += d * d;
     return d * scale * dact_from_out(o, act);
@@ -145,10 +151,21 @@ struct MseHead {
   __device__ static float loss(float sum, float scale) { return sum * 0.5f * scale; }
 };
 
+struct MseExtHead {
+  static constexpr int kKid = KID_MSE;
+  __device__ static float scale(int rows, int cols) { return 2.f / (static_cast<float>(rows) * static_cast<float>(cols)); }
+  __device__ static float grad(float o, float t, int act, float alpha, float scale, float& lacc) {
+    const float d = o - t;
+    lacc += d * d;
+    return d * scale * dact_from_out(o, act, alpha);
+  }
+  __device__ static float loss(float sum, float scale) { return sum * 0.5f * scale; }
+};
+
 struct SigmoidXentHead {
   static constexpr int kKid = KID_SIGMOID_XENT;
   __device__ static float scale(int rows, int cols) { return 1.f / (static_cast<float>(rows) * static_cast<float>(cols)); }
-  __device__ static float grad(float o, float t, int, float scale, float& lacc) {
+  __device__ static float grad(float o, float t, int, float, float scale, float& lacc) {
     float g;
     lacc += sigmoid_xent_elem(o, t, g);
     return g * scale;
@@ -157,10 +174,10 @@ struct SigmoidXentHead {
 };
 
 template <class Head>
-__global__ void __launch_bounds__(256)
-elementwise_loss_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ target, int ld_target,
-                        int act, float* __restrict__ loss, __nv_bfloat16* __restrict__ dz, int ld_dz,
-                        __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias, int rows, int cols) {
+__device__ __forceinline__ void elementwise_loss_tile(const float* __restrict__ out, int ld_out, const float* __restrict__ target,
+                                                      int ld_target, int act, float act_alpha, float* __restrict__ loss,
+                                                      __nv_bfloat16* __restrict__ dz, int ld_dz, __nv_bfloat16* __restrict__ dzT, int ld_t,
+                                                      float* __restrict__ dbias, int rows, int cols) {
   __shared__ float tile[32][33];
   __shared__ float s_col[32];
   __shared__ float s_loss[8];
@@ -179,7 +196,8 @@ elementwise_loss_kernel(const float* __restrict__ out, int ld_out, const float* 
     const int r = r0 + ty + 8 * i, c = c0 + tx;
     float g = 0.f;
     if (r < rows && c < cols)
-      g = Head::grad(out[static_cast<size_t>(r) * ld_out + c], target[static_cast<size_t>(r) * ld_target + c], act, scale, lacc);
+      g = Head::grad(out[static_cast<size_t>(r) * ld_out + c], target[static_cast<size_t>(r) * ld_target + c], act, act_alpha, scale,
+                     lacc);
     tile[ty + 8 * i][tx] = g;
     cacc += g;
     if (dz != nullptr && r < rows && c < ld_dz) dz[static_cast<size_t>(r) * ld_dz + c] = __float2bfloat16(g);
@@ -204,6 +222,21 @@ elementwise_loss_kernel(const float* __restrict__ out, int ld_out, const float* 
     }
   }
   trace.end(Head::kKid);
+}
+
+template <class Head>
+__global__ void __launch_bounds__(256)
+elementwise_loss_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ target, int ld_target,
+                        int act, float* __restrict__ loss, __nv_bfloat16* __restrict__ dz, int ld_dz,
+                        __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias, int rows, int cols) {
+  elementwise_loss_tile<Head>(out, ld_out, target, ld_target, act, 0.f, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols);
+}
+// MSE of an output with an extended activation (MseExtHead); act_alpha: a leaky ReLU's slope
+__global__ void __launch_bounds__(256)
+mse_ext_loss_kernel(const float* __restrict__ out, int ld_out, const float* __restrict__ target, int ld_target, int act, float act_alpha,
+                    float* __restrict__ loss, __nv_bfloat16* __restrict__ dz, int ld_dz, __nv_bfloat16* __restrict__ dzT, int ld_t,
+                    float* __restrict__ dbias, int rows, int cols) {
+  elementwise_loss_tile<MseExtHead>(out, ld_out, target, ld_target, act, act_alpha, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols);
 }
 
 __global__ void __launch_bounds__(256)
@@ -289,19 +322,24 @@ extern "C" int sf_softmax_xent(const float* logits, int ld_logits, const float* 
 }
 
 // the grid spans ld_dz columns, so the padded tail of every dz row is written (with zeros)
+static dim3 elementwise_loss_grid(__nv_bfloat16* dz, int ld_dz, int rows, int cols) {
+  const int span_c = (dz && ld_dz > cols) ? ld_dz : cols;
+  return dim3((span_c + 31) / 32, (rows + 31) / 32);
+}
 template <class Head>
 static int launch_elementwise_loss(const float* out, int ld_out, const float* target, int ld_target, int act, float* loss,
                                    __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t, float* dbias, int rows, int cols,
                                    cudaStream_t st) {
-  const int span_c = (dz && ld_dz > cols) ? ld_dz : cols;
-  dim3 grid((span_c + 31) / 32, (rows + 31) / 32);
-  return static_cast<int>(sf::launch(sf::elementwise_loss_kernel<Head>, grid, dim3(256), 0, st, out, ld_out, target, ld_target, act,
-                                     loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
+  return static_cast<int>(sf::launch(sf::elementwise_loss_kernel<Head>, elementwise_loss_grid(dz, ld_dz, rows, cols), dim3(256), 0, st, out,
+                                     ld_out, target, ld_target, act, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
 }
 
-extern "C" int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act,
+extern "C" int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act, float act_alpha,
                            float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                            float* dbias, int rows, int cols, cudaStream_t st) {
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::mse_ext_loss_kernel, elementwise_loss_grid(dz, ld_dz, rows, cols), dim3(256), 0, st, out, ld_out,
+                                       target, ld_target, act, act_alpha, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
   return launch_elementwise_loss<sf::MseHead>(out, ld_out, target, ld_target, act, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols, st);
 }
 

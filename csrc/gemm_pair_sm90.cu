@@ -38,9 +38,10 @@ __device__ __forceinline__ void pair_tile_coords(int t, int tiles_m, int tiles_n
   tn = r / gm;
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-sf_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const SfGemmEpilogue ep,
-                    int M, int N, int K, int tiles_m, int tiles_n, int group_m) {
+// One CTA of the pair kernel.  EXT: the extended activations (SfAct 4-9) are compiled into the epilogue.
+template <bool EXT>
+__device__ __forceinline__ void pair_cta(const CUtensorMap& tmA, const CUtensorMap& tmB, const SfGemmEpilogue& ep, int M, int N, int K,
+                                         int tiles_m, int tiles_n, int group_m) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
@@ -112,7 +113,7 @@ sf_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       if (ct < kPairBN) s_bias[ct] = (ep.bias != nullptr && n0 + ct < N) ? ep.bias[n0 + ct] : 0.f;
       stage_acc<kPairBN>(stg, acc, ct);
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      epilogue_tile<kPairBN, kEpiPair>(ep, stg, s_bias, m0, n0, M, N, ct);
+      epilogue_tile<kPairBN, kEpiPair, EXT>(ep, stg, s_bias, m0, n0, M, N, ct);
     }
   }
 
@@ -121,12 +122,27 @@ sf_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   trace.end(KID_GEMM);
 }
 
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
+sf_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const SfGemmEpilogue ep,
+                    int M, int N, int K, int tiles_m, int tiles_n, int group_m) {
+  pair_cta<false>(tmA, tmB, ep, M, N, K, tiles_m, tiles_n, group_m);
+}
+
+// the twin that carries the extended activations (a large layer with ELU, SELU, ...; see sf_gemm_ext_kernel)
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
+sf_gemm_pair_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const SfGemmEpilogue ep,
+                        int M, int N, int K, int tiles_m, int tiles_n, int group_m) {
+  pair_cta<true>(tmA, tmB, ep, M, N, K, tiles_m, tiles_n, group_m);
+}
+
 }  // namespace sf
 
-extern "C" int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st) {
+template <bool EXT>
+static int pair_launch(const SfGemm* g, cudaStream_t st) {
+  const auto kernel = EXT ? sf::sf_gemm_pair_ext_kernel : sf::sf_gemm_pair_kernel;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(sf::sf_gemm_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sf::kPairSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sf::kPairSmemBytes);
     if (e != cudaSuccess) return static_cast<int>(e);
     attr_set = true;
   }
@@ -150,6 +166,10 @@ extern "C" int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = sf::pdl_enabled() ? 1 : 0;
-  return static_cast<int>(cudaLaunchKernelEx(&cfg, sf::sf_gemm_pair_kernel, g->tmA, g->tmB, g->ep, g->M, g->N, g->K, tiles_m, tiles_n,
-                                             group_m));
+  return static_cast<int>(cudaLaunchKernelEx(&cfg, kernel, g->tmA, g->tmB, g->ep, g->M, g->N, g->K, tiles_m, tiles_n, group_m));
+}
+
+extern "C" int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st) {
+  const bool ext = g->ep.act >= SF_ACT_ELU || g->ep.aux_act >= SF_ACT_ELU;
+  return ext ? pair_launch<true>(g, st) : pair_launch<false>(g, st);
 }

@@ -60,9 +60,61 @@ __device__ __forceinline__ float act_bwd_from_out(float a, int act) {
     default: return 1.f;
   }
 }
-// whole-chunk forms: ONE (uniform) branch on the activation kind instead of one per element
-__device__ __forceinline__ void act_fwd32(float (&f)[32], int act) {
-  if (act == SF_ACT_RELU) {
+// Whole-chunk forms of the extended activations (SfAct 4-9): one loop per kind, so the kind is tested once per chunk.
+template <int ACT>
+__device__ __forceinline__ void act_ext_fwd_chunk(float (&f)[32], float alpha) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) f[j] = act_ext_fwd(f[j], ACT, alpha);
+}
+template <int ACT>
+__device__ __forceinline__ void act_ext_bwd_chunk(float (&f)[32], const float (&a)[32], float keep, float alpha) {
+  if (keep > 0.f && keep < 1.f) {
+    const float ik = __fdividef(1.f, keep);
+    if constexpr (ACT == SF_ACT_RELU6) {
+      // saturation is decided in stored units: a saturated unit holds bf16(6 * ik), rounded exactly as the forward
+      // epilogue rounded it, and a * keep of that value is not 6 for most keep (keep 0.9: 6.65625 * 0.9 = 5.9906)
+      const float sat = __bfloat162float(__float2bfloat16(6.f * ik));
+#pragma unroll
+      for (int j = 0; j < 32; ++j) f[j] *= (a[j] > 0.f && a[j] < sat) ? ik : 0.f;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) f[j] *= a[j] != 0.f ? act_ext_dact(a[j] * keep, ACT, alpha) * ik : 0.f;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) f[j] *= act_ext_dact(a[j], ACT, alpha);
+  }
+}
+__device__ __forceinline__ void act_ext_fwd32(float (&f)[32], int act, float alpha) {
+  switch (act) {
+    case SF_ACT_ELU: act_ext_fwd_chunk<SF_ACT_ELU>(f, alpha); break;
+    case SF_ACT_SELU: act_ext_fwd_chunk<SF_ACT_SELU>(f, alpha); break;
+    case SF_ACT_SOFTPLUS: act_ext_fwd_chunk<SF_ACT_SOFTPLUS>(f, alpha); break;
+    case SF_ACT_SOFTSIGN: act_ext_fwd_chunk<SF_ACT_SOFTSIGN>(f, alpha); break;
+    case SF_ACT_LEAKY_RELU: act_ext_fwd_chunk<SF_ACT_LEAKY_RELU>(f, alpha); break;
+    case SF_ACT_RELU6: act_ext_fwd_chunk<SF_ACT_RELU6>(f, alpha); break;
+    default: break;
+  }
+}
+__device__ __forceinline__ void act_ext_bwd32(float (&f)[32], const float (&a)[32], int act, float keep, float alpha) {
+  switch (act) {
+    case SF_ACT_ELU: act_ext_bwd_chunk<SF_ACT_ELU>(f, a, keep, alpha); break;
+    case SF_ACT_SELU: act_ext_bwd_chunk<SF_ACT_SELU>(f, a, keep, alpha); break;
+    case SF_ACT_SOFTPLUS: act_ext_bwd_chunk<SF_ACT_SOFTPLUS>(f, a, keep, alpha); break;
+    case SF_ACT_SOFTSIGN: act_ext_bwd_chunk<SF_ACT_SOFTSIGN>(f, a, keep, alpha); break;
+    case SF_ACT_LEAKY_RELU: act_ext_bwd_chunk<SF_ACT_LEAKY_RELU>(f, a, keep, alpha); break;
+    case SF_ACT_RELU6: act_ext_bwd_chunk<SF_ACT_RELU6>(f, a, keep, alpha); break;
+    default: break;
+  }
+}
+
+// whole-chunk forms: ONE (uniform) branch on the activation kind instead of one per element.  EXT: the kernel is a twin
+// that also carries the extended set (act >= SF_ACT_ELU); without it these are the ReLU / sigmoid / tanh code alone.
+template <bool EXT>
+__device__ __forceinline__ void act_fwd32(float (&f)[32], int act, float alpha) {
+  if (EXT && act >= SF_ACT_ELU) {
+    act_ext_fwd32(f, act, alpha);
+  } else if (act == SF_ACT_RELU) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
   } else if (act == SF_ACT_SIGMOID) {
@@ -74,8 +126,11 @@ __device__ __forceinline__ void act_fwd32(float (&f)[32], int act) {
   }
 }
 // f[j] *= act'(a[j]) (a = activation output); keep in (0, 1): a = act(z) * mask / keep (fused dropout), mask = a != 0
-__device__ __forceinline__ void act_bwd32(float (&f)[32], const float (&a)[32], int act, float keep) {
-  if (keep > 0.f && keep < 1.f) {
+template <bool EXT>
+__device__ __forceinline__ void act_bwd32(float (&f)[32], const float (&a)[32], int act, float keep, float alpha) {
+  if (EXT && act >= SF_ACT_ELU) {
+    act_ext_bwd32(f, a, act, keep, alpha);
+  } else if (keep > 0.f && keep < 1.f) {
     const float ik = __fdividef(1.f, keep);
 #pragma unroll
     for (int j = 0; j < 32; ++j) f[j] *= a[j] != 0.f ? act_bwd_from_out(a[j] * keep, act) * ik : 0.f;
@@ -133,8 +188,8 @@ struct EpiFeatures {
 
 // One 32-column chunk of a thread's output row: everything between the accumulator (v, already in registers) and
 // global memory.  `aux_pref` / `tgt_pref` are the act'(a) operand / label row of this chunk when the caller fetched
-// them before the accumulator wait (nullptr: read here).
-template <int EPI>
+// them before the accumulator wait (nullptr: read here).  EXT: the extended activations (twin kernels only).
+template <int EPI, bool EXT>
 __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32_t (&v)[32], const float* s_bias32, int row, bool row_ok,
                                           int col0, int M, int N, int lane, const uint4* aux_pref, const float* tgt_pref,
                                           unsigned long long* tq = nullptr) {
@@ -143,7 +198,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
 #pragma unroll
     for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]) * ep.alpha + s_bias32[j];
     if (tq != nullptr) tq[0] = trace_now();
-    if (F::kAct) act_fwd32(f, ep.act);
+    if (F::kAct) act_fwd32<EXT>(f, ep.act, ep.act_alpha);
     if (tq != nullptr) tq[1] = trace_now();
     if (F::kGeneric && ep.drop_keep > 0.f && ep.drop_keep < 1.f) {
       // fused dropout: keep with probability drop_keep, scale the survivors by 1 / drop_keep
@@ -203,7 +258,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
           f[j] = 0.f;
         }
       }
-      act_bwd32(f, a_out, ep.act, 0.f);
+      act_bwd32<EXT>(f, a_out, ep.act, 0.f, ep.act_alpha);
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) lrow += __shfl_xor_sync(0xffffffffu, lrow, o);
       if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow * 0.5f * scale);
@@ -237,7 +292,7 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
           a32[g * 8 + 2 * t + 1] = a2.y;
         }
       }
-      act_bwd32(f, a32, ep.aux_act, F::kGeneric ? ep.aux_keep : 0.f);
+      act_bwd32<EXT>(f, a32, ep.aux_act, F::kGeneric ? ep.aux_keep : 0.f, ep.aux_act_alpha);
     }
     if (tq != nullptr) tq[4] = trace_now();
     // padded columns / rows contribute exact zeros everywhere below
@@ -409,7 +464,7 @@ __device__ __forceinline__ void epi_prefetch(const SfGemmEpilogue& ep, uint4 (&a
 // Epilogue of one 128 x BN tile from the staged accumulator, by the 256 consumer threads: warp q owns rows
 // 32 * (q % 4) .. + 32 (one row per lane) and every other 32-column chunk starting at chunk q / 4.  aux_pref / tgt_pref:
 // the thread's chunk fetched by epi_prefetch (variants with EpiFeatures::kPrefetch only).
-template <int BN, int EPI>
+template <int BN, int EPI, bool EXT>
 __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const float* stg, const float* s_bias, int m0, int n0, int M,
                                               int N, int ct, const uint4* aux_pref = nullptr, const float* tgt_pref = nullptr) {
   using F = EpiFeatures<EPI>;
@@ -426,7 +481,7 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(srow[c * 32 + j]);
     if constexpr (F::kPrefetch) {
-      epi_chunk<EPI>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, aux_pref, tgt_pref);
+      epi_chunk<EPI, EXT>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, aux_pref, tgt_pref);
     } else {
       float tgt[32];
       if (F::kLoss && ep.loss_mode != SF_LOSS_NONE) {
@@ -434,7 +489,7 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 #pragma unroll
         for (int j = 0; j < 32; ++j) tgt[j] = (row_ok && col0 + j < N) ? tp[j] : 0.f;
       }
-      epi_chunk<EPI>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, nullptr, F::kLoss ? tgt : nullptr);
+      epi_chunk<EPI, EXT>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, nullptr, F::kLoss ? tgt : nullptr);
     }
   }
 }
@@ -443,8 +498,9 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 // run the wgmma main loop for 64 rows of the tile and then, together, the epilogue.
 // MN: both operands MN-major (D = a^T . b with a [K, M], b [K, N] row-major): the stage buffers have the same size, but a
 // stage is filled with {64 MN elements, 64 K rows} boxes and described to the tensor core as MN-major.
-// EPI: epilogue feature set (SfEpi); only the generic kernel handles the fused read-your-writes wait.
-template <int BN, bool MN, int EPI>
+// EPI: epilogue feature set (SfEpi); only the generic kernel handles the fused read-your-writes wait.  EXT: the extended
+// activations are compiled in (the twin kernels below).
+template <int BN, bool MN, int EPI, bool EXT = false>
 __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorMap& tmB, const SfGemmEpilogue& ep, int M, int N,
                                          int K, int kblocks_per_split) {
   static_assert(!MN || BN % 64 == 0, "MN-major B needs whole 64-element swizzle atoms");
@@ -558,9 +614,9 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
     asm volatile("bar.sync 1, 256;" ::: "memory");
     asm volatile("bar.sync 2, 352;" ::: "memory");      // bias tile in shared memory
     if constexpr (F::kPrefetch) {
-      epilogue_tile<BN, EPI>(ep, stg, s_bias, m0, n0, M, N, ct, aux_pref, tgt_pref);
+      epilogue_tile<BN, EPI, EXT>(ep, stg, s_bias, m0, n0, M, N, ct, aux_pref, tgt_pref);
     } else {
-      epilogue_tile<BN, EPI>(ep, stg, s_bias, m0, n0, M, N, ct);
+      epilogue_tile<BN, EPI, EXT>(ep, stg, s_bias, m0, n0, M, N, ct);
     }
   }
   trace.end(KID_GEMM);
@@ -593,6 +649,23 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 sf_gemm_sigmoid_loss_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                             const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
   gemm_cta<BN, false, SF_EPI_SIGMOID_LOSS>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+
+// Twins of the generic kernel (K-major) and of the FWD / LOSS / DGRAD variants that also carry the extended activations
+// (SfAct 4-9): their code would otherwise sit in every ReLU / sigmoid / tanh GEMM's epilogue, which is instruction-fetch
+// bound.  sf_gemm_launch picks a twin exactly when ep.act or ep.aux_act is one of them.
+template <int BN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  gemm_cta<BN, false, SF_EPI_GENERIC, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+template <int BN, int EPI>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_epi_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  static_assert(EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD, "only these variants apply an activation");
+  gemm_cta<BN, false, EPI, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
 }
 
 // ---------------------------------------------------------------------------
@@ -682,8 +755,13 @@ static int pick_epi(const SfGemm* g) {
   return e.colsum == nullptr ? SF_EPI_FWD : SF_EPI_GENERIC;
 }
 
+// the epilogue applies (or differentiates) one of the extended activations: the GEMM runs on a twin kernel
+static bool uses_ext_act(const SfGemmEpilogue& e) { return e.act >= SF_ACT_ELU || e.aux_act >= SF_ACT_ELU; }
+
 extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return -2;
+  if (g->ep.act < SF_ACT_NONE || g->ep.act > SF_ACT_RELU6 || g->ep.aux_act < SF_ACT_NONE || g->ep.aux_act > SF_ACT_RELU6) return -5;
+  if (g->mn_major && uses_ext_act(g->ep)) return -7;     // no MN-major twin: the weight-gradient GEMMs apply no activation
   if (g->ep.loss_mode < SF_LOSS_NONE || g->ep.loss_mode > SF_LOSS_SIGMOID_XENT) return -5;
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->bn > 64) g->bn = 64;    // the widest tile of its variant
@@ -737,11 +815,13 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   return 0;
 }
 
-template <int BN, bool MN = false, int EPI = SF_EPI_GENERIC>
+template <int BN, bool MN = false, int EPI = SF_EPI_GENERIC, bool EXT = false>
 static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
   using S = sf::GemmSmem<BN>;
   auto kernel = [] {
-    if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
+    if constexpr (EXT && EPI == SF_EPI_GENERIC) return sf::sf_gemm_ext_kernel<BN>;
+    else if constexpr (EXT) return sf::sf_gemm_epi_ext_kernel<BN, EPI>;
+    else if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
     else if constexpr (EPI == SF_EPI_SIGMOID_LOSS) return sf::sf_gemm_sigmoid_loss_kernel<BN>;
     else return sf::sf_gemm_epi_kernel<BN, MN, EPI>;
   }();
@@ -757,13 +837,35 @@ static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
 }
 
 // K-major epilogue variants exist at BN 32 and 64 (pick_epi)
-template <int EPI>
+template <int EPI, bool EXT = false>
 static cudaError_t launch_kmajor_variant(const SfGemm* g, cudaStream_t st) {
-  return g->bn == 32 ? launch_bn<32, false, EPI>(g, st) : launch_bn<64, false, EPI>(g, st);
+  return g->bn == 32 ? launch_bn<32, false, EPI, EXT>(g, st) : launch_bn<64, false, EPI, EXT>(g, st);
+}
+
+// the twins of the extended activations (K-major only, see sf_gemm_prepare)
+static int launch_ext(const SfGemm* g, cudaStream_t st) {
+  cudaError_t e;
+  switch (g->epi) {
+    case SF_EPI_GENERIC: break;
+    case SF_EPI_FWD: return static_cast<int>(launch_kmajor_variant<SF_EPI_FWD, true>(g, st));
+    case SF_EPI_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_LOSS, true>(g, st));
+    case SF_EPI_DGRAD: return static_cast<int>(launch_kmajor_variant<SF_EPI_DGRAD, true>(g, st));
+    default: return -3;
+  }
+  if (g->mn_major) return -3;
+  switch (g->bn) {
+    case 32: e = launch_bn<32, false, SF_EPI_GENERIC, true>(g, st); break;
+    case 64: e = launch_bn<64, false, SF_EPI_GENERIC, true>(g, st); break;
+    case 128: e = launch_bn<128, false, SF_EPI_GENERIC, true>(g, st); break;
+    case 256: e = launch_bn<256, false, SF_EPI_GENERIC, true>(g, st); break;
+    default: return -3;
+  }
+  return static_cast<int>(e);
 }
 
 extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
   if (g->pair) return sf_gemm_pair_launch(g, st);
+  if (uses_ext_act(g->ep)) return launch_ext(g, st);
   cudaError_t e;
   switch (g->epi) {
     case SF_EPI_GENERIC: break;

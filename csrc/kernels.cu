@@ -54,6 +54,23 @@ extern "C" int sf_preload_kernels() {
   SF_PRELOAD(sf::im2col_kernel); SF_PRELOAD(sf::col2im_kernel); SF_PRELOAD(sf::maxpool_fwd_kernel); SF_PRELOAD(sf::maxpool_bwd_kernel);
   SF_PRELOAD(sf::im2col_vec8_kernel); SF_PRELOAD(sf::col2im_vec8_kernel);
   SF_PRELOAD(sf::maxpool_gen_fwd_kernel); SF_PRELOAD(sf::maxpool_gen_bwd_kernel); SF_PRELOAD(sf::act_bwd_bias_kernel);
+  // the twins of the extended activations (SfAct 4-9)
+  SF_SMEM_ATTR(sf::sf_gemm_ext_kernel<32>, sf::GemmSmem<32>::kBytes); SF_SMEM_ATTR(sf::sf_gemm_ext_kernel<64>, sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR(sf::sf_gemm_ext_kernel<128>, sf::GemmSmem<128>::kBytes); SF_SMEM_ATTR(sf::sf_gemm_ext_kernel<256>, sf::GemmSmem<256>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_ext_kernel<32, SF_EPI_FWD>), sf::GemmSmem<32>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_ext_kernel<64, SF_EPI_FWD>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_ext_kernel<32, SF_EPI_LOSS>), sf::GemmSmem<32>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_ext_kernel<64, SF_EPI_LOSS>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_ext_kernel<32, SF_EPI_DGRAD>), sf::GemmSmem<32>::kBytes);
+  SF_SMEM_ATTR((sf::sf_gemm_epi_ext_kernel<64, SF_EPI_DGRAD>), sf::GemmSmem<64>::kBytes);
+  SF_SMEM_ATTR(sf::sf_gemm_pair_ext_kernel, sf::kPairSmemBytes);
+  SF_PRELOAD(sf::sf_gemm_ext_kernel<32>); SF_PRELOAD(sf::sf_gemm_ext_kernel<64>); SF_PRELOAD(sf::sf_gemm_ext_kernel<128>);
+  SF_PRELOAD(sf::sf_gemm_ext_kernel<256>); SF_PRELOAD(sf::sf_gemm_pair_ext_kernel);
+  SF_PRELOAD((sf::sf_gemm_epi_ext_kernel<32, SF_EPI_FWD>)); SF_PRELOAD((sf::sf_gemm_epi_ext_kernel<64, SF_EPI_FWD>));
+  SF_PRELOAD((sf::sf_gemm_epi_ext_kernel<32, SF_EPI_LOSS>)); SF_PRELOAD((sf::sf_gemm_epi_ext_kernel<64, SF_EPI_LOSS>));
+  SF_PRELOAD((sf::sf_gemm_epi_ext_kernel<32, SF_EPI_DGRAD>)); SF_PRELOAD((sf::sf_gemm_epi_ext_kernel<64, SF_EPI_DGRAD>));
+  SF_PRELOAD(sf::mse_ext_loss_kernel);
+  SF_PRELOAD(sf::maxpool_bwd_ext_kernel); SF_PRELOAD(sf::maxpool_gen_bwd_ext_kernel); SF_PRELOAD(sf::act_bwd_bias_ext_kernel);
   SF_PRELOAD((sf::conv_first_fwd_kernel<5, 5, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<5, 5, 1>));
   SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 1>));
   SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 3>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 3>));

@@ -120,6 +120,8 @@ struct Gemm {
     g.ep.drop_stream = getd<unsigned int>(d, "drop_stream", 0u);
     g.ep.drop_ctr = P<const unsigned int>(getd<uintptr_t>(d, "drop_ctr", 0));
     g.ep.aux_keep = getd<float>(d, "aux_keep", 0.0f);
+    g.ep.act_alpha = getd<float>(d, "act_alpha", 0.0f);
+    g.ep.aux_act_alpha = getd<float>(d, "aux_act_alpha", 0.0f);
     g.ep.ryw = P<const SfRyw>(getd<uintptr_t>(d, "ryw", 0));
     g.ep.route = P<const SfRoute>(getd<uintptr_t>(d, "route", 0));
     g.ep.route_tile0 = getd<int>(d, "route_tile0", 0);
@@ -874,6 +876,16 @@ py::bytes pack_segs(const std::vector<std::vector<int64_t>>& rows) {
 // ---------------------------------------------------------------------------
 namespace launch {
 
+// The `act` argument of the stand-alone backward / loss kernels: the SfAct in its low 32 bits and, for a leaky ReLU, the
+// fp32 bits of its slope in the high 32 (0 otherwise), so these bindings keep their signatures.
+int act_kind(long long act) { return static_cast<int>(act & 0xffffffffLL); }
+float act_alpha(long long act) {
+  const uint32_t bits = static_cast<uint32_t>(static_cast<unsigned long long>(act) >> 32);
+  float a;
+  std::memcpy(&a, &bits, sizeof(a));
+  return a;
+}
+
 auto cast_transpose(uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int ld_out, uintptr_t outT, int ld_t, int rows, int cols) {
   return [=](cudaStream_t st) {
     return idx ? sf_gather_cast_transpose(P<const float>(in), ld_in, P<const int32_t>(idx), P<__nv_bfloat16>(out), ld_out,
@@ -888,10 +900,10 @@ auto softmax_xent(uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labe
                            ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
   };
 }
-auto mse(uintptr_t out, int ld_out, uintptr_t target, int ld_target, int act, uintptr_t loss, uintptr_t dz, int ld_dz, uintptr_t dzT,
+auto mse(uintptr_t out, int ld_out, uintptr_t target, int ld_target, long long act, uintptr_t loss, uintptr_t dz, int ld_dz, uintptr_t dzT,
          int ld_t, uintptr_t dbias, int rows, int cols) {
   return [=](cudaStream_t st) {
-    return sf_mse_loss(P<const float>(out), ld_out, P<const float>(target), ld_target, act, P<float>(loss), P<__nv_bfloat16>(dz), ld_dz,
+    return sf_mse_loss(P<const float>(out), ld_out, P<const float>(target), ld_target, act_kind(act), act_alpha(act), P<float>(loss), P<__nv_bfloat16>(dz), ld_dz,
                        P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
   };
 }
@@ -924,11 +936,11 @@ auto maxpool_fwd(uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintpt
     return sf_maxpool2_fwd(P<const __nv_bfloat16>(in), n, h, w, c, P<__nv_bfloat16>(out), P<uint8_t>(argmax), P<__nv_bfloat16>(outT), ld_t, st);
   };
 }
-auto maxpool_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz,
+auto maxpool_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, uintptr_t act_out, long long act, uintptr_t dz, int ld_dz,
                  uintptr_t dzT, int ld_t, uintptr_t dbias) {
   return [=](cudaStream_t st) {
-    return sf_maxpool2_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, P<const __nv_bfloat16>(act_out), act,
-                           P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), st);
+    return sf_maxpool2_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, P<const __nv_bfloat16>(act_out), act_kind(act),
+                           act_alpha(act), P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), st);
   };
 }
 auto maxpool_gen_fwd(uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
@@ -939,15 +951,17 @@ auto maxpool_gen_fwd(uintptr_t in, int n, int h, int w, int c, int kh, int kw, i
   };
 }
 auto maxpool_gen_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
-                     int pad_left, int out_h, int out_w, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+                     int pad_left, int out_h, int out_w, uintptr_t act_out, long long act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
   return [=](cudaStream_t st) {
     return sf_maxpool_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h,
-                          out_w, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
+                          out_w, P<const __nv_bfloat16>(act_out), act_kind(act), act_alpha(act), P<__nv_bfloat16>(dz), ld_dz,
+                          P<float>(dbias), st);
   };
 }
-auto act_bwd_bias(uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, int act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+auto act_bwd_bias(uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, long long act, uintptr_t dz, int ld_dz, uintptr_t dbias) {
   return [=](cudaStream_t st) {
-    return sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act, P<__nv_bfloat16>(dz), ld_dz,
+    return sf_act_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act_kind(act), act_alpha(act),
+                           P<__nv_bfloat16>(dz), ld_dz,
                            P<float>(dbias), st);
   };
 }

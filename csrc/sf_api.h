@@ -5,7 +5,21 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-enum SfAct { SF_ACT_NONE = 0, SF_ACT_RELU = 1, SF_ACT_SIGMOID = 2, SF_ACT_TANH = 3 };
+// 4-9: the extended set.  Each derivative is a function of the activation's output a = act(z), which is all the backward
+// pass stores; LeakyRelu takes its slope from the epilogue's act_alpha / aux_act_alpha (the kernels' alpha argument).  The
+// GEMMs run them on twins of their kernels (gemm_sm90.cu), so the kernels of ReLU / sigmoid / tanh models are unchanged.
+enum SfAct {
+  SF_ACT_NONE = 0,
+  SF_ACT_RELU = 1,
+  SF_ACT_SIGMOID = 2,
+  SF_ACT_TANH = 3,
+  SF_ACT_ELU = 4,          // x > 0 ? x : exp(x) - 1                           act' = a > 0 ? 1 : a + 1
+  SF_ACT_SELU = 5,         // lambda * (x > 0 ? x : alpha (exp(x) - 1))         act' = a > 0 ? lambda : a + lambda alpha
+  SF_ACT_SOFTPLUS = 6,     // max(x, 0) + log1p(exp(-|x|))                     act' = 1 - exp(-a)
+  SF_ACT_SOFTSIGN = 7,     // x / (1 + |x|)                                    act' = (1 - |a|)^2
+  SF_ACT_LEAKY_RELU = 8,   // x > 0 ? x : alpha x, alpha > 0                    act' = a > 0 ? 1 : alpha
+  SF_ACT_RELU6 = 9,        // min(max(x, 0), 6)                                 act' = 0 < a < 6 ? 1 : 0
+};
 
 enum SfOptimizer {
   SF_OPT_SGD = 0,
@@ -88,6 +102,8 @@ struct SfGemmEpilogue {
   const unsigned int* drop_ctr;   // device word that changes every step (nullptr: 0)
   float aux_keep;                 // dgrad: keep probability of the dropout that produced aux (0 = none)
   const SfRyw* ryw;               // device memory; nullptr = no wait
+  // slope of a leaky ReLU `act` / `aux_act` (SF_ACT_LEAKY_RELU); appended last so every field above keeps its offset
+  float act_alpha, aux_act_alpha;
 };
 
 enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, SF_LOSS_SIGMOID_XENT = 3 };
@@ -152,9 +168,9 @@ int sf_gather_cast_transpose(const float* in, int ld_in, const int32_t* idx, __n
 int sf_softmax_xent(const float* logits, int ld_logits, const float* labels, int ld_labels,
                     float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                     float* dbias, int rows, int cols, cudaStream_t st);
-// mean squared error over all elements of out (after activation `act`, out is post-activation):
-// loss += mean((out-target)^2); dz = 2*(out-target)/(rows*cols) * act'(out)
-int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act,
+// mean squared error over all elements of out (after activation `act`, out is post-activation; act_alpha: the slope of a
+// leaky ReLU): loss += mean((out-target)^2); dz = 2*(out-target)/(rows*cols) * act'(out)
+int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act, float act_alpha,
                 float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                 float* dbias, int rows, int cols, cudaStream_t st);
 // sigmoid cross-entropy of raw logits z against labels y in [0, 1] over all elements:
@@ -175,18 +191,18 @@ int sf_col2im_nhwc(const __nv_bfloat16* dcols, int ld_cols, int n, int h, int w,
 int sf_maxpool2_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, __nv_bfloat16* out,
                     uint8_t* argmax, __nv_bfloat16* outT, int ld_t, cudaStream_t st);
 int sf_maxpool2_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c,
-                    const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz, int ld_dz,
+                    const __nv_bfloat16* act_out, int act, float act_alpha, __nv_bfloat16* dz, int ld_dz,
                     __nv_bfloat16* dzT, int ld_t, float* dbias, cudaStream_t st);
 // general max-pool: kh x kw <= 4x4 window, any stride, VALID or SAME (argmax = dy * kw + dx of the winner); the backward
 // pass is fused with act'(a) of the pooled conv output and the bias gradient and writes row-major dz [M, ld_dz]
 int sf_maxpool_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left,
                    int out_h, int out_w, __nv_bfloat16* out, uint8_t* argmax, cudaStream_t st);
 int sf_maxpool_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw,
-                   int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz,
-                   int ld_dz, float* dbias, cudaStream_t st);
+                   int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, float act_alpha,
+                   __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st);
 // activation gradient of a conv with no pool after it: dz = g * act'(a) [rows, ld_dz], dbias += column sums
-int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, __nv_bfloat16* dz,
-                    int ld_dz, float* dbias, cudaStream_t st);
+int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, float act_alpha,
+                    __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st);
 
 // first convolution of a network (K = kh * kw * cin <= 64, cout in {8, 16, 32, 64}) fused with bias, activation and the
 // 2x2 max-pool that follows it: direct CUDA-core kernels, one CTA per image, nothing but the pooled tensor is written.

@@ -10,6 +10,7 @@
 #include <cuda_bf16.h>
 #include <cuda.h>
 #include <stdint.h>
+#include "sf_api.h"
 
 namespace sf {
 
@@ -448,6 +449,41 @@ __device__ __forceinline__ float sigmoid_xent_elem(float z, float y, float& g) {
   const float r = __fdividef(1.f, 1.f + e);
   g = (z >= 0.f ? r : e * r) - y;
   return fmaxf(z, 0.f) - z * y + log1pf(e);
+}
+
+// The extended activations (SfAct 4-9), shared by the GEMM epilogue twins and the stand-alone backward / loss kernels.
+// act_ext_dact takes the derivative from the stored output a = act(z), never from z.  Softplus: 1 - exp(-a) = -expm1(-a),
+// below a = 1/4 from its series (1 - exp(-a) would cancel there; the series' first omitted term is a^6 / 720 <= 1.5e-6 a),
+// so the kernels need no expm1f (its slow path gave the general pool-backward kernel a stack frame).  ReLU6 passes no
+// gradient at a = 0 or a = 6 (TF's Relu6Grad).
+constexpr float kSeluLambda = 1.0507009873554805f;
+constexpr float kSeluAlpha = 1.6732632423543772f;
+__device__ __forceinline__ float act_ext_fwd(float x, int act, float alpha) {
+  switch (act) {
+    case SF_ACT_ELU: return x > 0.f ? x : expm1f(x);
+    case SF_ACT_SELU: return kSeluLambda * (x > 0.f ? x : kSeluAlpha * expm1f(x));
+    case SF_ACT_SOFTPLUS: return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x)));
+    case SF_ACT_SOFTSIGN: return __fdividef(x, 1.f + fabsf(x));
+    case SF_ACT_LEAKY_RELU: return x > 0.f ? x : alpha * x;
+    case SF_ACT_RELU6: return fminf(fmaxf(x, 0.f), 6.f);
+    default: return x;
+  }
+}
+__device__ __forceinline__ float act_ext_dact(float a, int act, float alpha) {
+  switch (act) {
+    case SF_ACT_ELU: return a > 0.f ? 1.f : a + 1.f;
+    case SF_ACT_SELU: return a > 0.f ? kSeluLambda : a + kSeluLambda * kSeluAlpha;
+    case SF_ACT_SOFTPLUS:
+      if (a < 0.25f) return a * (1.f - a * (0.5f - a * (1.f / 6.f - a * (1.f / 24.f - a * (1.f / 120.f)))));
+      return 1.f - __expf(-a);
+    case SF_ACT_SOFTSIGN: {
+      const float t = 1.f - fabsf(a);
+      return t * t;
+    }
+    case SF_ACT_LEAKY_RELU: return a > 0.f ? 1.f : alpha;
+    case SF_ACT_RELU6: return (a > 0.f && a < 6.f) ? 1.f : 0.f;
+    default: return 1.f;
+  }
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -22,7 +22,12 @@ from typing import Dict, List, Optional, Tuple
 
 from ..graph.ir import GraphIR, Node, split_ref
 
-ACT_IDS = {None: 0, "Relu": 1, "Sigmoid": 2, "Tanh": 3}
+# SfAct (csrc/sf_api.h).  Every activation here has a derivative that is a function of its output, which is all the step
+# stores: act'(z) is recomputed from a = act(z) in the backward kernels and the fused dropout recovers its mask from a.
+ACT_IDS = {None: 0, "Relu": 1, "Sigmoid": 2, "Tanh": 3, "Elu": 4, "Selu": 5, "Softplus": 6, "Softsign": 7, "LeakyRelu": 8, "Relu6": 9}
+ACT_OPS = tuple(a for a in ACT_IDS if a is not None)
+# activations whose derivative needs the pre-activation, which the step does not keep
+_PREACT_ACTS = ("Swish", "Gelu")
 
 
 class UnsupportedGraph(ValueError):
@@ -34,7 +39,8 @@ class Layer:
     kind: str                                   # dense | conv | pool | reshape
     kernel: Optional[str] = None                # variable node names
     bias: Optional[str] = None
-    act: Optional[str] = None                   # Relu | Sigmoid | Tanh | None
+    act: Optional[str] = None                   # an ACT_OPS name or None
+    act_alpha: float = 0.0                      # LeakyRelu: the slope for x < 0 (0 for every other activation)
     in_shape: Tuple[int, ...] = ()              # per-sample shape (no batch dim)
     out_shape: Tuple[int, ...] = ()
     ksize: Tuple[int, int] = (0, 0)            # conv: filter taps; pool: window
@@ -232,6 +238,55 @@ def _float_cast(node: Node) -> bool:
     return node.attrs.get("SrcT", "DT_FLOAT") in _FLOAT_TYPES and node.attrs.get("DstT", "DT_FLOAT") in _FLOAT_TYPES
 
 
+def _preact_reason(what: str) -> str:
+    return (f"{what} is not covered by the compiled plan: its derivative is not a function of its output, and the step "
+            "keeps only activation outputs")
+
+
+def _match_leaky_maximum(ir: GraphIR, node: Node) -> Optional[Tuple[Tuple[str, int], float]]:
+    """TF 1.4-1.12's ``tf.nn.leaky_relu``: Maximum(Mul(alpha, x), x), operands of both ops in either order -> (x, alpha)"""
+    if node.op != "Maximum" or len(node.inputs) != 2:
+        return None
+    for m_ref, x in ((node.inputs[0], node.inputs[1]), (node.inputs[1], node.inputs[0])):
+        mul = ir.nodes[m_ref[0]]
+        if mul.op != "Mul" or len(mul.inputs) != 2 or x not in mul.inputs:
+            continue
+        c = mul.inputs[1] if mul.inputs[0] == x else mul.inputs[0]
+        alpha = _const_scalar(ir, c)
+        if alpha is None:
+            raise UnsupportedGraph(f"leaky ReLU '{node.name}': alpha is not a constant, so it is not covered by the compiled plan")
+        if not 0.0 <= alpha <= 1.0:
+            raise UnsupportedGraph(f"Maximum(alpha * x, x) '{node.name}' with alpha {alpha} outside [0, 1] is not a leaky ReLU and is not "
+                                   "covered by the compiled plan")
+        return x, alpha
+    return None
+
+
+def _match_activation(ir: GraphIR, node: Node) -> Optional[Tuple[str, float, Tuple[str, int]]]:
+    """(activation, act_alpha, input) when ``node`` is an activation the compiled plan fuses into its layer"""
+    if node.op in _PREACT_ACTS:
+        raise UnsupportedGraph(_preact_reason(f"activation '{node.op}' ({node.name})"))
+    if node.op == "Mul" and len(node.inputs) == 2:
+        for x, s in ((node.inputs[0], node.inputs[1]), (node.inputs[1], node.inputs[0])):
+            sig = ir.nodes[s[0]]
+            if sig.op == "Sigmoid" and sig.inputs == [x]:
+                raise UnsupportedGraph(_preact_reason(f"swish x * sigmoid(x) ('{node.name}')"))
+        return None
+    leaky = _match_leaky_maximum(ir, node)
+    if leaky is not None:
+        x, alpha = leaky
+        return ("Relu", 0.0, x) if alpha == 0.0 else ("LeakyRelu", float(alpha), x)
+    if node.op not in ACT_OPS or len(node.inputs) != 1:
+        return None
+    if node.op == "LeakyRelu":
+        alpha = float(node.attrs.get("alpha", 0.2))
+        if alpha < 0.0:
+            # the sign of the output would no longer tell the backward pass which branch the unit took
+            raise UnsupportedGraph(f"leaky ReLU '{node.name}' with a negative alpha ({alpha}) is not covered by the compiled plan")
+        return ("Relu", 0.0, node.inputs[0]) if alpha == 0.0 else ("LeakyRelu", alpha, node.inputs[0])
+    return node.op, 0.0, node.inputs[0]
+
+
 def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
     """Walk back from the scalar loss through reductions / scalings to the per-element loss node."""
     seen = set()
@@ -345,7 +400,7 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
     # ---- walk the forward chain backwards -------------------------------------------------------
     layers_rev: List[Layer] = []
     cur = chain_end
-    pending_act: Optional[Tuple[str, str]] = None      # (act, tensor name)
+    pending_act: Optional[Tuple[str, str, float]] = None   # (act, tensor name, act_alpha)
     pending_bias: Optional[Tuple[str, str]] = None     # (var, tensor name)
     pending_drop: Optional[Tuple[float, str]] = None   # (keep_prob, tensor name) of a dropout above the next layer found
     guard = 0
@@ -372,11 +427,12 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
                 pending_drop = (drop[1], tname)
             cur = drop[0]
             continue
-        if node.op in ("Relu", "Sigmoid", "Tanh"):
+        act = _match_activation(ir, node)
+        if act is not None:
             if pending_act or pending_bias:
                 raise UnsupportedGraph(f"activation '{node.name}' is not directly on top of a linear layer")
-            pending_act = (node.op, tname)
-            cur = node.inputs[0]
+            pending_act = (act[0], tname, act[1])
+            cur = act[2]
             continue
         if node.op == "BiasAdd" or (node.op in ("Add", "AddV2") and _var_of(ir, node.inputs[1]) is not None):
             if pending_bias:
@@ -402,7 +458,8 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             if pending_drop:
                 tensors["dropout"] = pending_drop[1]
             layers_rev.append(Layer("dense", kernel=kvar, bias=pending_bias[0] if pending_bias else None,
-                                    act=pending_act[0] if pending_act else None, in_shape=(kin,), out_shape=(kout,), tensors=tensors,
+                                    act=pending_act[0] if pending_act else None, act_alpha=pending_act[2] if pending_act else 0.0,
+                                    in_shape=(kin,), out_shape=(kout,), tensors=tensors,
                                     dropout_keep=pending_drop[0] if pending_drop else 0.0))
             pending_act = pending_bias = pending_drop = None
             cur = node.inputs[0]
@@ -425,7 +482,8 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             if pending_act:
                 tensors["act"] = pending_act[1]
             layers_rev.append(Layer("conv", kernel=kvar, bias=pending_bias[0] if pending_bias else None,
-                                    act=pending_act[0] if pending_act else None, in_shape=(-1, -1, cin), out_shape=(-1, -1, cout),
+                                    act=pending_act[0] if pending_act else None, act_alpha=pending_act[2] if pending_act else 0.0,
+                                    in_shape=(-1, -1, cin), out_shape=(-1, -1, cout),
                                     ksize=(kh, kw), strides=(strides[1], strides[2]), padding=_padding(node), tensors=tensors))
             pending_act = pending_bias = None
             cur = node.inputs[0]

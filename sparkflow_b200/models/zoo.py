@@ -12,6 +12,7 @@ Each function mirrors a model definition of the reference:
   * :func:`cnn_strided`       – strided / SAME convs, a conv feeding a conv, an overlapping 3x3/2 pool, a conv feeding
     the flatten
   * :func:`binary_dnn` / :func:`multilabel_dnn` – binary and multi-label classifiers trained with sigmoid cross-entropy
+  * :func:`selu_dnn` / :func:`leaky_cnn` / :func:`softplus_autoencoder` – SELU, leaky ReLU + ELU and softplus networks
 """
 from __future__ import annotations
 
@@ -93,6 +94,42 @@ def cnn_strided():
     return tf.losses.softmax_cross_entropy(y, logits)
 
 
+def selu_dnn():
+    """784-256-256-10 self-normalising classifier: SELU hidden layers, softmax-CE"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    h1 = tf.layers.dense(x, 256, activation=tf.nn.selu)
+    h2 = tf.layers.dense(h1, 256, activation=tf.nn.selu)
+    logits = tf.layers.dense(h2, 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def leaky_cnn():
+    """cnn_same with leaky ReLU (alpha 0.1) convs and an ELU dense layer"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+
+    def leaky(t):
+        return tf.nn.leaky_relu(t, alpha=0.1)
+
+    c1 = tf.layers.max_pooling2d(tf.layers.conv2d(img, 32, 5, padding="same", activation=leaky), 2, 2, padding="same")
+    c2 = tf.layers.max_pooling2d(tf.layers.conv2d(c1, 64, 5, padding="same", activation=leaky), 2, 2, padding="same")
+    h = tf.layers.dense(tf.layers.flatten(c2), 1024, activation=tf.nn.elu)
+    logits = tf.layers.dense(h, 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def softplus_autoencoder():
+    """784-128-784 auto-encoder: softplus code, sigmoid reconstruction, MSE against the input"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    code = tf.layers.dense(x, 128, activation=tf.nn.softplus, name="out")
+    rec = tf.layers.dense(code, 784, activation=tf.nn.sigmoid)
+    return tf.losses.mean_squared_error(rec, x)
+
+
 def autoencoder():
     x = tf.placeholder("float", shape=[None, 784], name="x")
     e1 = tf.layers.dense(x, 256, activation=tf.nn.relu)
@@ -160,6 +197,9 @@ MODELS: Dict[str, Callable] = {
     "fixture_mlp": fixture_mlp,
     "binary_dnn": binary_dnn,
     "multilabel_dnn": multilabel_dnn,
+    "selu_dnn": selu_dnn,
+    "leaky_cnn": leaky_cnn,
+    "softplus_autoencoder": softplus_autoencoder,
 }
 
 

@@ -27,6 +27,7 @@ from dataclasses import dataclass, field
 from typing import Any, Dict, List, Optional
 
 import os
+import struct
 
 import torch
 
@@ -88,7 +89,7 @@ def check_grammar(lp: LayerPlan) -> None:
         if l.kind == "conv":
             if l.out_shape[2] % 8:
                 raise UnsupportedGraph("conv output channels must be a multiple of 8")
-            if l.act not in (None, "Relu", "Sigmoid", "Tanh"):
+            if l.act not in ACT_IDS:
                 raise UnsupportedGraph(f"conv activation {l.act}")
     if saw_conv and lp.input_dim % 8:
         raise UnsupportedGraph("image inputs need a feature count that is a multiple of 8")
@@ -120,6 +121,12 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
     if (l.out_shape[0] + l.ksize[0] - 1) * (l.out_shape[1] + l.ksize[1] - 1) * cin * 4 > 64 * 1024:
         return None
     return i
+
+
+def act_arg(l: Layer) -> int:
+    """The ``act`` argument of the stand-alone backward / loss kernels for layer ``l``: its SfAct in the low 32 bits and
+    the fp32 bits of a leaky ReLU's alpha in the high 32 (csrc/runtime.cpp, launch::act_kind / act_alpha)."""
+    return ACT_IDS[l.act] | (struct.unpack("<I", struct.pack("<f", l.act_alpha))[0] << 32)
 
 
 _LOSS_MODES = {"softmax_xent": 1, "mse": 2, "sigmoid_xent": 3}     # SfLossMode (csrc/sf_api.h)
@@ -336,7 +343,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             ks, bs = lay.by_name(l.kernel), (lay.by_name(l.bias) if l.bias else None)
             act_out = zeros(M, cout)
             g = C.Gemm(dict(a=P(patches), lda=ldK, b=P(wsrc) + ks.wt_off * 2, ldb=ks.wt_ld, M=M, N=cout, K=K,
-                            bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], out_bf16=P(act_out), ld_bf16=cout,
+                            bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], act_alpha=l.act_alpha, out_bf16=P(act_out), ld_bf16=cout,
                             a_evict_first=1, **ryw_args()))
             gemms.append(g)
             plan.add_gemm(g, f"conv{i}")
@@ -363,7 +370,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         ks, bs = lay.by_name(l.kernel), (lay.by_name(l.bias) if l.bias else None)
         last = i == stop_layer
         d = dict(a=P(cur["buf"]), lda=cur["ld"], b=P(wsrc) + ks.wt_off * 2, ldb=ks.wt_ld, M=B, N=ks.cols, K=ks.rows,
-                 bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], **ryw_args())
+                 bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], act_alpha=l.act_alpha, **ryw_args())
         drop = None
         if l.dropout_keep:
             # fused Philox dropout: the mask is a function of (row, column, step counter of this plan, layer) under a
@@ -409,7 +416,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         elif lp.loss == "sigmoid_xent":
             plan.add_sigmoid_xent(*args, loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
         elif lp.loss == "mse":
-            plan.add_mse(*args, ACT_IDS[last_l.act], loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
+            plan.add_mse(*args, act_arg(last_l), loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
         else:
             raise UnsupportedGraph(f"no loss kernel for loss kind {lp.loss!r}")
 
@@ -474,7 +481,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 pb = lay.by_name(prev.bias) if prev.bias else None
                 ndz, ndzT = zeros(B, r["a_in_ld"]), (None if use_mn else zeros(ks.rows, ldB))
                 dd = dict(a=P(g_dz), lda=g_dz.shape[1], b=P(wsrc) + ks.w_off * 2, ldb=ks.w_ld, M=B, N=ks.rows, K=ks.cols,
-                          aux=P(r["a_in"]), ld_aux=r["a_in_ld"], aux_act=ACT_IDS[prev.act], aux_keep=float(prev.dropout_keep or 0.0), out_bf16=P(ndz),
+                          aux=P(r["a_in"]), ld_aux=r["a_in_ld"], aux_act=ACT_IDS[prev.act], aux_act_alpha=prev.act_alpha, aux_keep=float(prev.dropout_keep or 0.0), out_bf16=P(ndz),
                           ld_bf16=ndz.shape[1], outT_bf16=P(ndzT), ld_t=ldB if ndzT is not None else 0,
                           colsum=P(worker.grads) + pb.offset * 4 if pb else 0)
                 dg = C.Gemm(dd)
@@ -511,11 +518,11 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             dzc = zeros(cr["M"], c) if need_dz else None
             dzcT = None if use_mn else zeros(c, cr["ldM"])
             if pool_fast_path(l):
-                plan.add_maxpool_bwd(P(g_img), P(r["argmax"]), B, h, w, c, P(cr["act_out"]), ACT_IDS[conv_l.act], P(dzc), c if need_dz else 0,
+                plan.add_maxpool_bwd(P(g_img), P(r["argmax"]), B, h, w, c, P(cr["act_out"]), act_arg(conv_l), P(dzc), c if need_dz else 0,
                                      P(dzcT), cr["ldM"] if dzcT is not None else 0, P(worker.grads) + cb.offset * 4 if cb else 0)
             else:                                   # check_grammar keeps general pools off the K-major path: dz is row-major only
                 plan.add_maxpool_gen_bwd(P(g_img), P(r["argmax"]), B, h, w, c, l.ksize[0], l.ksize[1], l.strides[0], l.strides[1], l.pads[0],
-                                         l.pads[2], l.out_shape[0], l.out_shape[1], P(cr["act_out"]), ACT_IDS[conv_l.act], P(dzc), c,
+                                         l.pads[2], l.out_shape[0], l.out_shape[1], P(cr["act_out"]), act_arg(conv_l), P(dzc), c,
                                          P(worker.grads) + cb.offset * 4 if cb else 0)
             rec[ci]["dz"], rec[ci]["dzT"] = dzc, dzcT
             continue
@@ -527,7 +534,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 # flatten dgrad); dz = g * act'(a) and the bias gradient come from one kernel
                 cb = lay.by_name(l.bias) if l.bias else None
                 dzc = zeros(r["M"], ks.cols)
-                plan.add_act_bwd_bias(P(g_img), ks.cols, r["M"], ks.cols, P(r["act_out"]), ACT_IDS[l.act], P(dzc), ks.cols,
+                plan.add_act_bwd_bias(P(g_img), ks.cols, r["M"], ks.cols, P(r["act_out"]), act_arg(l), P(dzc), ks.cols,
                                       P(worker.grads) + cb.offset * 4 if cb else 0)
                 r["dz"], r["dzT"] = dzc, None
             kblocks = (r["M"] + 63) // 64
