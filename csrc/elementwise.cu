@@ -1,5 +1,6 @@
 // Elementwise / reduction kernels of the training step that are not GEMMs:
-// input cast+transpose (K11 feeder), softmax-cross-entropy (K5), MSE and sigmoid-cross-entropy (K6), argmax (K7).
+// input cast+transpose (K11 feeder), softmax-cross-entropy against one-hot / soft labels or class indices (K5), MSE and
+// sigmoid-cross-entropy (K6), argmax (K7).
 // Reference semantics: tf.losses.softmax_cross_entropy / mean_squared_error / sigmoid_cross_entropy with the default
 // SUM_BY_NONZERO_WEIGHTS reduction (examples/simple_dnn.py:20, autoencoder_example.py:15).
 #include "sm90_ptx.cuh"
@@ -130,6 +131,64 @@ softmax_xent_kernel(const float* __restrict__ logits, int ld_logits, const float
     for (int c = threadIdx.x; c < cols; c += blockDim.x)
       if (s_db[c] != 0.f) atomicAdd(dbias + c, s_db[c]);
   trace.end(KID_SOFTMAX);
+}
+
+// ---------------------------------------------------------------------------
+// Sparse softmax cross-entropy: one warp per row, one class index per row (labels[r * ld_labels], truncated toward zero).
+//   loss  += (lse - z_label) / B
+//   dz_j   = (softmax_j - [j == label]) / B
+// The label is compared with the column index inside the column loops and never used as an address.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+sparse_softmax_xent_kernel(const float* __restrict__ logits, int ld_logits, const float* __restrict__ labels,
+                           int ld_labels, float* __restrict__ loss, __nv_bfloat16* __restrict__ dz, int ld_dz,
+                           __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias, int rows,
+                           int cols) {
+  extern __shared__ float s_db[];   // [cols]
+  TraceScope trace;
+  pdl_launch_dependents();
+  pdl_wait();
+  trace.mark();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warps_per_block = blockDim.x >> 5;
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) s_db[c] = 0.f;
+  __syncthreads();
+  const float inv_b = 1.f / static_cast<float>(rows);
+  float loss_acc = 0.f;
+  for (int r = blockIdx.x * warps_per_block + warp; r < rows; r += gridDim.x * warps_per_block) {
+    const float* z = logits + static_cast<size_t>(r) * ld_logits;
+    float mx = -INFINITY;
+    for (int c = lane; c < cols; c += 32) mx = fmaxf(mx, z[c]);
+    mx = warp_max(mx);
+    // truncation toward zero; loaded after the max pass (loaded before it, the kernel keeps a 16-byte stack frame)
+    const int label = static_cast<int>(labels[static_cast<size_t>(r) * ld_labels]);
+    float se = 0.f, zl = 0.f;
+    for (int c = lane; c < cols; c += 32) {
+      const float zc = z[c];
+      se += __expf(zc - mx);
+      zl += c == label ? zc : 0.f;
+    }
+    se = warp_sum(se);
+    zl = warp_sum(zl);
+    loss_acc += mx + __logf(se) - zl;
+    const float inv_se = 1.f / se;
+    for (int c = lane; c < cols; c += 32) {
+      const float p = __expf(z[c] - mx) * inv_se;
+      const float g = (p - (c == label ? 1.f : 0.f)) * inv_b;
+      if (dz) dz[static_cast<size_t>(r) * ld_dz + c] = __float2bfloat16(g);
+      if (dzT) dzT[static_cast<size_t>(c) * ld_t + r] = __float2bfloat16(g);
+      if (dbias) atomicAdd(&s_db[c], g);
+    }
+    // zero the padded tail of the row so the K-major GEMM operand is clean
+    if (dz)
+      for (int c = cols + lane; c < ld_dz; c += 32) dz[static_cast<size_t>(r) * ld_dz + c] = __float2bfloat16(0.f);
+  }
+  if (lane == 0 && loss_acc != 0.f) atomicAdd(loss, loss_acc * inv_b);
+  __syncthreads();
+  if (dbias)
+    for (int c = threadIdx.x; c < cols; c += blockDim.x)
+      if (s_db[c] != 0.f) atomicAdd(dbias + c, s_db[c]);
+  trace.end(KID_SPARSE_SOFTMAX);
 }
 
 // ---------------------------------------------------------------------------
@@ -318,6 +377,15 @@ extern "C" int sf_softmax_xent(const float* logits, int ld_logits, const float* 
   int blocks = (rows + 7) / 8;
   if (blocks > sf_num_sms() * 4) blocks = sf_num_sms() * 4;
   return static_cast<int>(sf::launch(sf::softmax_xent_kernel, dim3(blocks), dim3(256), cols * sizeof(float), st,
+                                     logits, ld_logits, labels, ld_labels, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
+}
+
+extern "C" int sf_sparse_softmax_xent(const float* logits, int ld_logits, const float* labels, int ld_labels,
+                                      float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
+                                      float* dbias, int rows, int cols, cudaStream_t st) {
+  int blocks = (rows + 7) / 8;
+  if (blocks > sf_num_sms() * 4) blocks = sf_num_sms() * 4;
+  return static_cast<int>(sf::launch(sf::sparse_softmax_xent_kernel, dim3(blocks), dim3(256), cols * sizeof(float), st,
                                      logits, ld_logits, labels, ld_labels, loss, dz, ld_dz, dzT, ld_t, dbias, rows, cols));
 }
 

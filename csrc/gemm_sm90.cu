@@ -17,7 +17,7 @@
 //   * fp32 store or atomic accumulate (split-K / straight into the flat gradient buffer that the
 //     push kernel consumes).
 // The generic kernel (sf_gemm_kernel) tests each of these at run time.  The training GEMMs run specialized variants
-// (sf_gemm_epi_kernel, one per SfEpi kind, and sf_gemm_sigmoid_loss_kernel) that contain only their own epilogue code, a
+// (sf_gemm_epi_kernel, one per SfEpi kind, sf_gemm_sigmoid_loss_kernel and sf_gemm_sparse_loss_kernel) that contain only their own epilogue code, a
 // fifth to a half of the generic kernel's; the DGRAD / loss variants also fetch their act'(aux) / label rows before the
 // main loop.
 //
@@ -176,14 +176,18 @@ struct EpiFeatures {
   // sigmoid-CE head: only in its own variant, which therefore also carries the transposed bf16 output and the fused
   // read-your-writes wait that otherwise only the generic kernel has (so the generic kernel stays as it was)
   static constexpr bool kSigmoidLoss = EPI == SF_EPI_SIGMOID_LOSS;
-  static constexpr bool kOutT = kGeneric || EPI == SF_EPI_SIGMOID_LOSS;
-  static constexpr bool kRyw = kGeneric || EPI == SF_EPI_SIGMOID_LOSS;
+  // sparse softmax-CE head (one class index per row): likewise only in its own variant, with the same extras
+  static constexpr bool kSparseLoss = EPI == SF_EPI_SPARSE_LOSS;
+  static constexpr bool kOutT = kGeneric || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_SPARSE_LOSS;
+  static constexpr bool kRyw = kGeneric || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_SPARSE_LOSS;
   static constexpr bool kAux = kGeneric || EPI == SF_EPI_DGRAD;
-  static constexpr bool kColsum = kGeneric || EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_DGRAD;
+  static constexpr bool kColsum = kGeneric || EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_SPARSE_LOSS ||
+                                  EPI == SF_EPI_DGRAD;
   static constexpr bool kF32 = kGeneric || EPI == SF_EPI_WGRAD;
-  static constexpr bool kBf16 = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_DGRAD;
-  // the thread's act'(aux) chunk / label row are fetched before the main loop (epi_prefetch)
-  static constexpr bool kPrefetch = EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_DGRAD;
+  static constexpr bool kBf16 = kGeneric || EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS ||
+                                EPI == SF_EPI_SPARSE_LOSS || EPI == SF_EPI_DGRAD;
+  // the thread's act'(aux) chunk / label row / class index are fetched before the main loop (epi_prefetch)
+  static constexpr bool kPrefetch = EPI == SF_EPI_LOSS || EPI == SF_EPI_SIGMOID_LOSS || EPI == SF_EPI_SPARSE_LOSS || EPI == SF_EPI_DGRAD;
 };
 
 // One 32-column chunk of a thread's output row: everything between the accumulator (v, already in registers) and
@@ -275,6 +279,31 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) lrow += __shfl_xor_sync(0xffffffffu, lrow, o);
       if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow * scale);
+    } else if (F::kSparseLoss && ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT) {
+      // whole row in this thread (N <= 32, raw logits); tgt_pref[0] is the row's class index, truncated toward zero like
+      // TF's Cast.  It is only compared with column indices, so a label outside [0, N) reads nothing out of bounds.
+      const int label = static_cast<int>(tgt_pref[0]);
+      const int nvalid = row_ok ? (N - col0 < 32 ? N - col0 : 32) : 0;
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) mx = fmaxf(mx, j < nvalid ? f[j] : -INFINITY);
+      float se = 0.f, zl = 0.f;
+      float ex[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const bool ok = j < nvalid;
+        ex[j] = ok ? __expf(f[j] - mx) : 0.f;
+        se += ex[j];
+        zl += ok && col0 + j == label ? f[j] : 0.f;
+      }
+      const float inv_b = __fdividef(1.f, static_cast<float>(M));
+      float lrow = row_ok ? (mx + __logf(se) - zl) * inv_b : 0.f;
+      const float inv_se = row_ok ? __fdividef(1.f, se) : 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) f[j] = j < nvalid ? (ex[j] * inv_se - (col0 + j == label ? 1.f : 0.f)) * inv_b : 0.f;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) lrow += __shfl_xor_sync(0xffffffffu, lrow, o);
+      if (lane == 0 && lrow != 0.f) atomicAdd(ep.loss, lrow);
     }
     if (tq != nullptr) tq[3] = trace_now();
     if (F::kAux && (!F::kGeneric || ep.aux != nullptr) && row_ok) {
@@ -438,7 +467,8 @@ __device__ __forceinline__ void stage_acc(float* stg, const float (&acc)[BN / 2]
   for (int j = 0; j < BN / 2; ++j) stg[(r0 + 8 * ((j >> 1) & 1)) * (BN + 1) + 8 * (j >> 2) + c0 + (j & 1)] = acc[j];
 }
 
-// The act'(aux) chunk (DGRAD) or label row (LOSS) that consumer thread ct's epilogue reads, fetched before the main loop
+// The act'(aux) chunk (DGRAD), label row (LOSS) or class index (SPARSE_LOSS, into tgt[0]) that consumer thread ct's
+// epilogue reads, fetched before the main loop
 // so that the load's latency hides under it.  Earlier launches wrote both, and everything upstream of this grid is
 // complete once pdl_wait has returned.  BN <= 64: a thread owns at most one chunk (c = q / 4, see epilogue_tile).
 template <int BN, int EPI>
@@ -454,6 +484,8 @@ __device__ __forceinline__ void epi_prefetch(const SfGemmEpilogue& ep, uint4 (&a
 #pragma unroll
     for (int g = 0; g < 4; ++g)
       aux[g] = (live && col0 + g * 8 < ep.ld_aux) ? *reinterpret_cast<const uint4*>(ap + g * 8) : make_uint4(0u, 0u, 0u, 0u);
+  } else if constexpr (EPI == SF_EPI_SPARSE_LOSS) {
+    tgt[0] = live ? ep.target[static_cast<size_t>(row) * ep.ld_target] : 0.f;     // the row's class index
   } else {
     const float* tp = ep.target + static_cast<size_t>(live ? row : 0) * ep.ld_target + col0;
 #pragma unroll
@@ -651,6 +683,14 @@ sf_gemm_sigmoid_loss_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   gemm_cta<BN, false, SF_EPI_SIGMOID_LOSS>(tmA, tmB, ep, M, N, K, kblocks_per_split);
 }
 
+// The sparse softmax cross-entropy head (SF_EPI_SPARSE_LOSS, K-major, BN 32: the row fits one chunk) runs only here, so
+// that the LOSS variant and the generic kernel keep their code; it carries the same extras as the sigmoid kernel.
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_sparse_loss_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                           const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  gemm_cta<32, false, SF_EPI_SPARSE_LOSS>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+
 // Twins of the generic kernel (K-major) and of the FWD / LOSS / DGRAD variants that also carry the extended activations
 // (SfAct 4-9): their code would otherwise sit in every ReLU / sigmoid / tanh GEMM's epilogue, which is instruction-fetch
 // bound.  sf_gemm_launch picks a twin exactly when ep.act or ep.aux_act is one of them.
@@ -743,6 +783,12 @@ static int pick_epi(const SfGemm* g) {
                     e.out_bf16 != nullptr && e.act == SF_ACT_NONE && (g->bn == 32 || g->bn == 64);
     return ok ? SF_EPI_SIGMOID_LOSS : SF_EPI_GENERIC;
   }
+  if (e.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT) {
+    // likewise the sparse softmax head: K-major, BN 32, raw logits, bf16 dz (+ transpose)
+    const bool ok = !g->pair && !g->mn_major && !dropout && e.route == nullptr && e.aux == nullptr && e.out_f32 == nullptr &&
+                    e.out_bf16 != nullptr && e.act == SF_ACT_NONE && g->bn == 32;
+    return ok ? SF_EPI_SPARSE_LOSS : SF_EPI_GENERIC;
+  }
   if (g->pair || dropout || e.route != nullptr || e.ryw != nullptr || e.outT_bf16 != nullptr) return SF_EPI_GENERIC;
   if (g->mn_major) {
     const bool wgrad = (g->bn == 64 || g->bn == 128) && e.out_f32 != nullptr && e.out_bf16 == nullptr && e.aux == nullptr &&
@@ -762,7 +808,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return -2;
   if (g->ep.act < SF_ACT_NONE || g->ep.act > SF_ACT_RELU6 || g->ep.aux_act < SF_ACT_NONE || g->ep.aux_act > SF_ACT_RELU6) return -5;
   if (g->mn_major && uses_ext_act(g->ep)) return -7;     // no MN-major twin: the weight-gradient GEMMs apply no activation
-  if (g->ep.loss_mode < SF_LOSS_NONE || g->ep.loss_mode > SF_LOSS_SIGMOID_XENT) return -5;
+  if (g->ep.loss_mode < SF_LOSS_NONE || g->ep.loss_mode > SF_LOSS_SPARSE_SOFTMAX_XENT) return -5;
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->bn > 64) g->bn = 64;    // the widest tile of its variant
   if (g->split_k <= 0) g->split_k = 1;
@@ -800,7 +846,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   g->kblocks_per_split = (total_kb + g->split_k - 1) / g->split_k;
   g->split_k = (total_kb + g->kblocks_per_split - 1) / g->kblocks_per_split;
   if (g->split_k > 1) g->ep.accumulate = 1;
-  if (g->ep.loss_mode == SF_LOSS_SOFTMAX_XENT) {
+  if (g->ep.loss_mode == SF_LOSS_SOFTMAX_XENT || g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT) {
     if (g->N > 32 || g->split_k > 1) return -5;     // the row must fit one epilogue chunk
     g->bn = 32;
   }
@@ -812,6 +858,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   g->ep.one_wave = static_cast<long long>((g->N + g->bn - 1) / g->bn) * ((g->M + sf::kBM - 1) / sf::kBM) * g->split_k <= sf_num_sms();
   g->epi = g->epi == SF_EPI_GENERIC ? SF_EPI_GENERIC : pick_epi(g);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->epi != SF_EPI_SIGMOID_LOSS) return -5;
+  if (g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT && g->epi != SF_EPI_SPARSE_LOSS) return -5;
   return 0;
 }
 
@@ -823,6 +870,7 @@ static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
     else if constexpr (EXT) return sf::sf_gemm_epi_ext_kernel<BN, EPI>;
     else if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
     else if constexpr (EPI == SF_EPI_SIGMOID_LOSS) return sf::sf_gemm_sigmoid_loss_kernel<BN>;
+    else if constexpr (EPI == SF_EPI_SPARSE_LOSS) return sf::sf_gemm_sparse_loss_kernel;
     else return sf::sf_gemm_epi_kernel<BN, MN, EPI>;
   }();
   static bool attr_set = false;
@@ -873,6 +921,7 @@ extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
     case SF_EPI_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_LOSS>(g, st));
     case SF_EPI_DGRAD: return static_cast<int>(launch_kmajor_variant<SF_EPI_DGRAD>(g, st));
     case SF_EPI_SIGMOID_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_SIGMOID_LOSS>(g, st));
+    case SF_EPI_SPARSE_LOSS: return static_cast<int>(launch_bn<32, false, SF_EPI_SPARSE_LOSS>(g, st));
     case SF_EPI_WGRAD:
       e = g->bn == 64 ? launch_bn<64, true, SF_EPI_WGRAD>(g, st) : launch_bn<128, true, SF_EPI_WGRAD>(g, st);
       return static_cast<int>(e);

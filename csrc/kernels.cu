@@ -44,12 +44,13 @@ extern "C" int sf_preload_kernels() {
   SF_PRELOAD((sf::sf_gemm_epi_kernel<32, false, SF_EPI_FWD>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<64, false, SF_EPI_FWD>));
   SF_PRELOAD((sf::sf_gemm_epi_kernel<32, false, SF_EPI_LOSS>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<64, false, SF_EPI_LOSS>));
   SF_PRELOAD(sf::sf_gemm_sigmoid_loss_kernel<32>); SF_PRELOAD(sf::sf_gemm_sigmoid_loss_kernel<64>);
+  SF_SMEM_ATTR(sf::sf_gemm_sparse_loss_kernel, sf::GemmSmem<32>::kBytes); SF_PRELOAD(sf::sf_gemm_sparse_loss_kernel);
   SF_PRELOAD((sf::sf_gemm_epi_kernel<32, false, SF_EPI_DGRAD>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<64, false, SF_EPI_DGRAD>));
   SF_PRELOAD((sf::sf_gemm_epi_kernel<64, true, SF_EPI_WGRAD>)); SF_PRELOAD((sf::sf_gemm_epi_kernel<128, true, SF_EPI_WGRAD>));
   SF_SMEM_ATTR(sf::sf_gemm_pair_kernel, sf::kPairSmemBytes);
   SF_PRELOAD(sf::sf_gemm_kernel<32>); SF_PRELOAD(sf::sf_gemm_kernel<64>); SF_PRELOAD(sf::sf_gemm_kernel<128>); SF_PRELOAD(sf::sf_gemm_kernel<256>); SF_PRELOAD(sf::sf_gemm_pair_kernel);
   SF_PRELOAD(sf::gather_rows_f32_kernel); SF_PRELOAD(sf::cast_transpose_kernel<false>); SF_PRELOAD(sf::cast_transpose_kernel<true>);
-  SF_PRELOAD(sf::softmax_xent_kernel); SF_PRELOAD(sf::elementwise_loss_kernel<sf::MseHead>);
+  SF_PRELOAD(sf::softmax_xent_kernel); SF_PRELOAD(sf::sparse_softmax_xent_kernel); SF_PRELOAD(sf::elementwise_loss_kernel<sf::MseHead>);
   SF_PRELOAD(sf::elementwise_loss_kernel<sf::SigmoidXentHead>); SF_PRELOAD(sf::argmax_rows_kernel);
   SF_PRELOAD(sf::im2col_kernel); SF_PRELOAD(sf::col2im_kernel); SF_PRELOAD(sf::maxpool_fwd_kernel); SF_PRELOAD(sf::maxpool_bwd_kernel);
   SF_PRELOAD(sf::im2col_vec8_kernel); SF_PRELOAD(sf::col2im_vec8_kernel);

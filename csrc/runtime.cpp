@@ -893,9 +893,15 @@ auto cast_transpose(uintptr_t in, int ld_in, uintptr_t idx, uintptr_t out, int l
                : sf_cast_transpose(P<const float>(in), ld_in, P<__nv_bfloat16>(out), ld_out, P<__nv_bfloat16>(outT), ld_t, rows, cols, st);
   };
 }
+// softmax_xent takes one-hot / soft label rows, or one class index per row: a label row narrower than the logits row
+// (ld_labels < cols) cannot be a distribution over the classes, so it is read as one class index per row, at stride
+// ld_labels (sf_sparse_softmax_xent), and this binding keeps its signature.
 auto softmax_xent(uintptr_t logits, int ld_logits, uintptr_t labels, int ld_labels, uintptr_t loss, uintptr_t dz, int ld_dz,
                   uintptr_t dzT, int ld_t, uintptr_t dbias, int rows, int cols) {
   return [=](cudaStream_t st) {
+    if (ld_labels < cols)
+      return sf_sparse_softmax_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss),
+                                    P<__nv_bfloat16>(dz), ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
     return sf_softmax_xent(P<const float>(logits), ld_logits, P<const float>(labels), ld_labels, P<float>(loss), P<__nv_bfloat16>(dz),
                            ld_dz, P<__nv_bfloat16>(dzT), ld_t, P<float>(dbias), rows, cols, st);
   };

@@ -79,8 +79,9 @@ struct SfGemmEpilogue {
   // fused loss (last dense layer): the epilogue turns the activation into dL/dz in registers, so
   // out_bf16 / outT_bf16 / colsum receive dz, dz^T and the bias gradient directly.
   int loss_mode;                  // SfLossMode: 0 none, 1 softmax cross-entropy (N <= 32), 2 mean squared error,
-                                  // 3 sigmoid cross-entropy (raw logits, any N)
-  const float* target;            // [M, ld_target] labels (one-hot / soft) or regression targets
+                                  // 3 sigmoid cross-entropy (raw logits, any N), 4 sparse softmax cross-entropy (N <= 32)
+  const float* target;            // [M, ld_target] labels (one-hot / soft) or regression targets; loss mode 4: one class
+                                  // index per row in column 0
   int ld_target;
   float* loss;                    // scalar accumulator (mean loss)
   // sharded push fused into a wgrad epilogue: when `route` is set the fp32 output element (row, col) is stored to
@@ -106,7 +107,7 @@ struct SfGemmEpilogue {
   float act_alpha, aux_act_alpha;
 };
 
-enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, SF_LOSS_SIGMOID_XENT = 3 };
+enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, SF_LOSS_SIGMOID_XENT = 3, SF_LOSS_SPARSE_SOFTMAX_XENT = 4 };
 
 // Epilogue variant of the one-CTA GEMM kernel.  The generic kernel carries every epilogue feature behind runtime tests;
 // each specialized variant compiles in only the features of one kind of training GEMM (sf_gemm_prepare picks it):
@@ -116,7 +117,10 @@ enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, S
 //   WGRAD fp32 store or atomic accumulate (MN-major operands)
 //   SIGMOID_LOSS  bias + sigmoid-CE head on raw logits -> dz bf16 (+ transpose), loss, optional column sum, optional
 //                 read-your-writes wait; the only kernel with this head (the generic kernel has none)
-enum SfEpi { SF_EPI_GENERIC = 0, SF_EPI_FWD = 1, SF_EPI_LOSS = 2, SF_EPI_DGRAD = 3, SF_EPI_WGRAD = 4, SF_EPI_SIGMOID_LOSS = 5 };
+//   SPARSE_LOSS   bias + softmax-CE head on raw logits against one class index per row (N <= 32, BN 32) -> the same
+//                 outputs as SIGMOID_LOSS; the only kernel with this head
+enum SfEpi { SF_EPI_GENERIC = 0, SF_EPI_FWD = 1, SF_EPI_LOSS = 2, SF_EPI_DGRAD = 3, SF_EPI_WGRAD = 4, SF_EPI_SIGMOID_LOSS = 5,
+             SF_EPI_SPARSE_LOSS = 6 };
 
 
 struct SfGemm {
@@ -168,6 +172,12 @@ int sf_gather_cast_transpose(const float* in, int ld_in, const int32_t* idx, __n
 int sf_softmax_xent(const float* logits, int ld_logits, const float* labels, int ld_labels,
                     float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
                     float* dbias, int rows, int cols, cudaStream_t st);
+// softmax cross-entropy against one class index per row, labels[r * ld_labels] (a float, truncated toward zero like TF's
+// Cast): mean loss (lse - z_label) / B, dlogits = (p - [j == label]) / B.  The label is only compared with the column
+// index, never used as an address: a label outside [0, cols) reads nothing out of bounds (its row then has no target).
+int sf_sparse_softmax_xent(const float* logits, int ld_logits, const float* labels, int ld_labels,
+                           float* loss, __nv_bfloat16* dz, int ld_dz, __nv_bfloat16* dzT, int ld_t,
+                           float* dbias, int rows, int cols, cudaStream_t st);
 // mean squared error over all elements of out (after activation `act`, out is post-activation; act_alpha: the slope of a
 // leaky ReLU): loss += mean((out-target)^2); dz = 2*(out-target)/(rows*cols) * act'(out)
 int sf_mse_loss(const float* out, int ld_out, const float* target, int ld_target, int act, float act_alpha,

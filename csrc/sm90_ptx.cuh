@@ -46,7 +46,7 @@ __device__ unsigned int g_trace_n = 0;
 
 enum KernelId { KID_GEMM = 1, KID_CAST = 2, KID_SOFTMAX = 3, KID_MSE = 4, KID_ARGMAX = 5, KID_PUSH = 6, KID_PULL = 7,
                 KID_IM2COL = 8, KID_COL2IM = 9, KID_POOL_FWD = 10, KID_POOL_BWD = 11, KID_POOL_GEN_FWD = 12, KID_POOL_GEN_BWD = 13,
-                KID_ACT_BWD = 14, KID_SIGMOID_XENT = 15,
+                KID_ACT_BWD = 14, KID_SIGMOID_XENT = 15, KID_SPARSE_SOFTMAX = 16,
                 // phase stamps (ids 100 and up): one extra record of three stamps in t0 / t1 / t2
                 KID_PUSH_LEAD = 106,      // push, block 0: grant seen, gradient loads returned, optimizer math done
                 KID_PUSH_TAIL = 107 };    // push, last CTA: stores issued, done-counter arrival returned, tail done

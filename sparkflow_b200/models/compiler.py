@@ -3,7 +3,7 @@
 The reference runs whatever graph the user serialised through a TF session.  The H100 engine
 instead executes a *compiled* plan: the forward chain between ``tfInput`` and the loss is pattern-
 matched into dense / conv / pool / reshape layers with fused bias+activation, the loss into
-softmax-cross-entropy, sigmoid-cross-entropy or mean-squared-error, ``tf.nn.dropout`` / ``tf.layers.dropout`` after a dense layer into a
+softmax-cross-entropy (one-hot labels or class indices), sigmoid-cross-entropy or mean-squared-error, ``tf.nn.dropout`` / ``tf.layers.dropout`` after a dense layer into a
 fused Philox mask in that layer's epilogue, and ``tfOutput`` into "activation of layer k" (+ optional ArgMax /
 Softmax).  Graphs outside this family (custom losses, exotic ops) are reported as unsupported so the caller can use the
 generic interpreter engine instead (loudly: a RuntimeWarning names the reason).
@@ -75,12 +75,12 @@ class OutputSpec:
 @dataclass
 class LayerPlan:
     layers: List[Layer]
-    loss: Optional[str]                         # softmax_xent | sigmoid_xent | mse | None (inference only)
+    loss: Optional[str]                         # softmax_xent | sparse_softmax_xent | sigmoid_xent | mse | None (inference only)
     input_name: str
     label_name: Optional[str]                   # placeholder fed with labels; None if target is the input
     target_is_input: bool
     input_dim: int
-    label_dim: int
+    label_dim: int                              # label columns fed per row (1 for sparse_softmax_xent: the class index)
     output: Optional[OutputSpec]
     var_order: List[str]
 
@@ -238,6 +238,78 @@ def _float_cast(node: Node) -> bool:
     return node.attrs.get("SrcT", "DT_FLOAT") in _FLOAT_TYPES and node.attrs.get("DstT", "DT_FLOAT") in _FLOAT_TYPES
 
 
+# casts a class index may pass through: each of these types holds every index below MAX_SPARSE_CLASSES exactly, so the
+# kernels, which read the placeholder's float32, see the index TF computes.  A narrower type (half, bfloat16, 8 / 16-bit
+# ints) or an unsigned one can round or wrap an index.
+_INDEX_CAST_TYPES = ("DT_FLOAT", "DT_DOUBLE", "DT_INT32", "DT_INT64")
+# The stand-alone sparse softmax kernel (N > 32) accumulates the bias gradient of every class in shared memory, 4 bytes per
+# class within the 48 KB a launch gets without opting in to more.
+MAX_SPARSE_CLASSES = 12288
+
+
+def _attr_ints(v) -> List[int]:
+    return [int(a) for a in (v if isinstance(v, (list, tuple)) else [v])]
+
+
+def _one_hot_of(ir: GraphIR, ref: Tuple[str, int]) -> Optional[Node]:
+    """the OneHot node behind ``ref`` (through Identity / StopGradient / PlaceholderWithDefault), or None"""
+    node = ir.nodes[ref[0]]
+    while node.op in _PASS and node.inputs:
+        node = ir.nodes[node.inputs[0][0]]
+    return node if node.op == "OneHot" else None
+
+
+def _check_one_hot(ir: GraphIR, node: Node, n_classes: int) -> None:
+    """``tf.one_hot(idx, N)`` with the defaults the sparse head computes: depth N, on 1, off 0, the class axis last"""
+    depth = _const_scalar(ir, node.inputs[1]) if len(node.inputs) == 4 else None
+    on = _const_scalar(ir, node.inputs[2]) if len(node.inputs) == 4 else None
+    off = _const_scalar(ir, node.inputs[3]) if len(node.inputs) == 4 else None
+    if depth is None or int(depth) != n_classes:
+        raise UnsupportedGraph(f"one_hot '{node.name}' with depth {depth} for {n_classes} logits is not covered by the compiled plan")
+    if on is None or off is None:
+        raise UnsupportedGraph(f"one_hot '{node.name}' with an on_value or off_value that is not a constant is not covered by the "
+                               "compiled plan")
+    if on != 1.0 or off != 0.0:
+        raise UnsupportedGraph(f"one_hot '{node.name}' with on_value {on} / off_value {off} (label smoothing) is not covered by the "
+                               "compiled plan")
+    if int(node.attrs.get("axis", -1)) != -1:
+        raise UnsupportedGraph(f"one_hot '{node.name}' along axis {node.attrs.get('axis')} is not covered by the compiled plan")
+
+
+def _class_index_placeholder(ir: GraphIR, ref: Tuple[str, int]) -> Node:
+    """Walk the class indices of a sparse softmax cross-entropy (or of its ``tf.one_hot``) back to their placeholder: through
+    Identity / StopGradient / PlaceholderWithDefault, Cast between float32, float64, int32 and int64, and exactly one Reshape to [-1] or
+    Squeeze of axis 1, which flattens the [None, 1] column ``ml_util`` feeds a scalar label with."""
+    node = ir.nodes[ref[0]]
+    flattened = False
+    for _ in range(32):
+        if node.op in _PASS and node.inputs:
+            node = ir.nodes[node.inputs[0][0]]
+        elif node.op == "Cast" and node.inputs:
+            src, dst = node.attrs.get("SrcT", "DT_FLOAT"), node.attrs.get("DstT", "DT_FLOAT")
+            if src not in _INDEX_CAST_TYPES or dst not in _INDEX_CAST_TYPES:
+                raise UnsupportedGraph(f"Cast '{node.name}' from {src} to {dst} on the class-index path can round or wrap a class "
+                                       "index; the compiled plan takes casts between float32, float64, int32 and int64")
+            node = ir.nodes[node.inputs[0][0]]
+        elif node.op == "Reshape" and not flattened and len(node.inputs) == 2 and ir.nodes[node.inputs[1][0]].op == "Const" \
+                and [int(v) for v in ir.nodes[node.inputs[1][0]].attrs["value"].reshape(-1)] == [-1]:
+            flattened = True
+            node = ir.nodes[node.inputs[0][0]]
+        elif node.op == "Squeeze" and not flattened and node.inputs and _attr_ints(node.attrs.get("squeeze_dims", [])) in ([1], [-1]):
+            flattened = True
+            node = ir.nodes[node.inputs[0][0]]
+        else:
+            break
+    if node.op not in ("Placeholder", "PlaceholderV2"):
+        raise UnsupportedGraph(f"class labels reach the loss through '{node.op}' ({node.name}): the compiled plan covers Identity, "
+                               "Cast and one Reshape to [-1] or Squeeze of axis 1 of a [None, 1] label placeholder")
+    shape = node.attrs.get("shape")
+    if not flattened or not shape or len(shape) != 2:
+        raise UnsupportedGraph(f"class labels need a rank-2 [None, 1] label placeholder flattened by a Reshape to [-1] or a Squeeze "
+                               f"of axis 1; '{node.name}' has shape {shape}")
+    return node
+
+
 def _preact_reason(what: str) -> str:
     return (f"{what} is not covered by the compiled plan: its derivative is not a function of its output, and the step "
             "keeps only activation outputs")
@@ -298,7 +370,10 @@ def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
         seen.add(name)
         node = ir.nodes[name]
         if node.op == "SoftmaxCrossEntropyWithLogits":
-            return "softmax_xent", node
+            # tf.one_hot of class indices as the labels: the sparse head
+            return ("sparse_softmax_xent" if _one_hot_of(ir, node.inputs[1]) is not None else "softmax_xent"), node
+        if node.op == "SparseSoftmaxCrossEntropyWithLogits":
+            return "sparse_softmax_xent", node
         if node.op == "SquaredDifference":
             return "mse", node
         if node.op == "Square" and node.inputs and ir.nodes[node.inputs[0][0]].op == "Sub":
@@ -324,8 +399,9 @@ def _check_mean_reduction(ir: GraphIR, loss_ref: str, kind: str, core: Node) -> 
     hops = 0
     while node.name != core.name and hops < 16:
         ops_on_path.append(node.op)
-        if kind == "sigmoid_xent" and node.op == "Mul" and not any(_const_ones(ir, i) for i in node.inputs):
-            raise UnsupportedGraph("weighted sigmoid cross-entropy is not covered by the compiled plan")
+        if kind in ("sigmoid_xent", "sparse_softmax_xent") and node.op == "Mul" and not any(_const_ones(ir, i) for i in node.inputs):
+            raise UnsupportedGraph(f"weighted {'sigmoid' if kind == 'sigmoid_xent' else 'sparse softmax'} cross-entropy is not "
+                                   "covered by the compiled plan")
         nxt = None
         for src, _ in node.inputs:
             if ir.nodes[src].op not in ("Const", "Size", "Shape", "Cast") or src == core.name:
@@ -341,6 +417,9 @@ def _check_mean_reduction(ir: GraphIR, loss_ref: str, kind: str, core: Node) -> 
         if kind == "sigmoid_xent" and "Sum" in ops_on_path:
             # e.g. reduce_mean(reduce_sum(per_element, axis=1)): a sum over the labels, N times the element mean
             raise UnsupportedGraph("a sum under a mean of sigmoid cross-entropy is not covered by the compiled plan")
+        if kind == "sparse_softmax_xent" and "Sum" in ops_on_path:
+            # reduce_mean(reduce_sum(per_row)): the batch total, B times the mean
+            raise UnsupportedGraph("a sum under a mean of sparse softmax cross-entropy is not covered by the compiled plan")
         return
     if "Sum" in ops_on_path and any(o in ops_on_path for o in ("RealDiv", "Div", "DivNoNan")):
         return
@@ -366,8 +445,8 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
         loss_kind, core = _find_loss_core(ir, ir.losses[0])
         _check_mean_reduction(ir, ir.losses[0], loss_kind, core)
         a, b = core.inputs[0], core.inputs[1]
-        if loss_kind == "softmax_xent":
-            pred_ref, target_ref = a, b               # (features=logits, labels)
+        if loss_kind in ("softmax_xent", "sparse_softmax_xent"):
+            pred_ref, target_ref = a, b               # (features=logits, labels / class indices / their one_hot)
         elif loss_kind == "sigmoid_xent":
             pred_ref, target_ref = _match_sigmoid_xent(ir, core)
         else:
@@ -554,7 +633,28 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
     label_name = None
     target_is_input = False
     label_dim = 0
-    if need_loss:
+    n_out = layers[-1].out_features
+    if need_loss and loss_kind == "sparse_softmax_xent":
+        # one class index per row: SparseSoftmaxCrossEntropyWithLogits(logits, idx) or the one-hot spelling
+        # SoftmaxCrossEntropyWithLogits(logits, OneHot(idx, N, 1, 0))
+        one_hot = _one_hot_of(ir, target_ref)
+        if one_hot is not None:
+            _check_one_hot(ir, one_hot, n_out)
+            target_ref = one_hot.inputs[0]
+        tnode = _class_index_placeholder(ir, target_ref)
+        label_name = f"{tnode.name}:0"
+        if tf_label is not None and split_ref(tf_label)[0] != tnode.name:
+            raise UnsupportedGraph(f"the loss target is placeholder '{tnode.name}' but tfLabel is '{tf_label}'")
+        tshape = tnode.attrs.get("shape")
+        label_dim = int(tshape[1]) if tshape[1] is not None else -1
+        if label_dim != 1:
+            raise UnsupportedGraph(f"label width does not match: class labels take a [None, 1] placeholder, '{tnode.name}' is {tshape}")
+        if n_out < 2:
+            raise UnsupportedGraph("sparse softmax cross-entropy needs at least 2 classes")
+        if n_out > MAX_SPARSE_CLASSES:
+            raise UnsupportedGraph(f"sparse softmax cross-entropy over {n_out} classes is not covered by the compiled plan (at most "
+                                   f"{MAX_SPARSE_CLASSES}: the loss kernel keeps one bias-gradient word per class in shared memory)")
+    elif need_loss:
         tnode = ir.nodes[target_ref[0]]
         # tf.losses.sigmoid_cross_entropy casts the labels to the logits' dtype
         passes = _PASS + ("Cast",) if loss_kind == "sigmoid_xent" else _PASS
@@ -571,10 +671,11 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
                 raise UnsupportedGraph(f"the loss target is placeholder '{tnode.name}' but tfLabel is '{tf_label}'")
         else:
             raise UnsupportedGraph("loss target must be a placeholder or the input itself")
-        if label_dim != layers[-1].out_features:
+        if label_dim != n_out:
             raise UnsupportedGraph("label width does not match the network output width")
-        if loss_kind in ("softmax_xent", "sigmoid_xent") and layers[-1].act is not None:
-            raise UnsupportedGraph(f"{loss_kind.split('_')[0]} cross-entropy expects raw logits")
+    if need_loss:
+        if loss_kind in ("softmax_xent", "sigmoid_xent", "sparse_softmax_xent") and layers[-1].act is not None:
+            raise UnsupportedGraph(f"{'sigmoid' if loss_kind == 'sigmoid_xent' else 'softmax'} cross-entropy expects raw logits")
         if layers[-1].dropout_keep:
             raise UnsupportedGraph("dropout on the network output is not covered by the compiled plan")
 

@@ -13,6 +13,8 @@ Each function mirrors a model definition of the reference:
     the flatten
   * :func:`binary_dnn` / :func:`multilabel_dnn` – binary and multi-label classifiers trained with sigmoid cross-entropy
   * :func:`selu_dnn` / :func:`leaky_cnn` / :func:`softplus_autoencoder` – SELU, leaky ReLU + ELU and softplus networks
+  * :func:`sparse_dnn` / :func:`onehot_cnn` / :func:`sparse_dnn100` – classifiers trained on a numeric class column
+    ([None, 1] labels) with sparse softmax cross-entropy or a ``tf.one_hot`` in the graph
 """
 from __future__ import annotations
 
@@ -55,6 +57,32 @@ def multilabel_dnn(tags: int = 40):
     return loss
 
 
+def sparse_dnn():
+    """simple_dnn trained on a numeric class column (e.g. StringIndexer output): a [None, 1] label placeholder and
+    ``tf.losses.sparse_softmax_cross_entropy``"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 1], name="y")
+    h1 = tf.layers.dense(x, 256, activation=tf.nn.relu, kernel_initializer=tf.glorot_uniform_initializer())
+    h2 = tf.layers.dense(h1, 256, activation=tf.nn.relu, kernel_initializer=tf.glorot_uniform_initializer())
+    logits = tf.layers.dense(h2, 10, kernel_initializer=tf.glorot_uniform_initializer())
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.sparse_softmax_cross_entropy(tf.cast(tf.reshape(y, [-1]), tf.int32), logits)
+
+
+def sparse_dnn100():
+    """784-256-100 classifier on class indices, spelled ``reduce_mean(sparse_softmax_cross_entropy_with_logits)`` +
+    ``add_loss`` (100 classes: wider than the fused softmax head)"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 1], name="y")
+    h = tf.layers.dense(x, 256, activation=tf.nn.relu)
+    logits = tf.layers.dense(h, 100)
+    tf.argmax(logits, 1, name="out")
+    loss = tf.reduce_mean(tf.nn.sparse_softmax_cross_entropy_with_logits(labels=tf.cast(tf.squeeze(y, axis=1), tf.int64),
+                                                                         logits=logits))
+    tf.losses.add_loss(loss)
+    return loss
+
+
 def cnn():
     x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
     y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
@@ -64,6 +92,18 @@ def cnn():
     logits = tf.layers.dense(tf.layers.flatten(c2), 10)
     tf.argmax(logits, 1, name="out")
     return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def onehot_cnn():
+    """cnn on a numeric class column, one-hot encoded in the graph: ``tf.one_hot`` of the [None, 1] label column"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 1], name="y")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    c1 = tf.layers.max_pooling2d(tf.layers.conv2d(img, 32, 5, activation=tf.nn.relu), 2, 2)
+    c2 = tf.layers.max_pooling2d(tf.layers.conv2d(c1, 64, 3, activation=tf.nn.relu), 2, 2)
+    logits = tf.layers.dense(tf.layers.flatten(c2), 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(tf.one_hot(tf.cast(tf.reshape(y, [-1]), tf.int32), 10), logits)
 
 
 def cnn_same():
@@ -200,6 +240,9 @@ MODELS: Dict[str, Callable] = {
     "selu_dnn": selu_dnn,
     "leaky_cnn": leaky_cnn,
     "softplus_autoencoder": softplus_autoencoder,
+    "sparse_dnn": sparse_dnn,
+    "onehot_cnn": onehot_cnn,
+    "sparse_dnn100": sparse_dnn100,
 }
 
 

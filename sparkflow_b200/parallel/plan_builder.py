@@ -129,7 +129,7 @@ def act_arg(l: Layer) -> int:
     return ACT_IDS[l.act] | (struct.unpack("<I", struct.pack("<f", l.act_alpha))[0] << 32)
 
 
-_LOSS_MODES = {"softmax_xent": 1, "mse": 2, "sigmoid_xent": 3}     # SfLossMode (csrc/sf_api.h)
+_LOSS_MODES = {"softmax_xent": 1, "mse": 2, "sigmoid_xent": 3, "sparse_softmax_xent": 4}     # SfLossMode (csrc/sf_api.h)
 
 
 def loss_mode(kind: Optional[str]) -> int:
@@ -381,8 +381,9 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             drop = dict(keep=float(l.dropout_keep), seed=seed, stream=i, ctr=done_dev)
         rec[i] = dict(a_in=cur["buf"], a_in_ld=cur["ld"], a_inT=cur.get("bufT"), drop=drop)
         if last:
-            # the element-wise heads take any width; the softmax row must fit one 32-column epilogue chunk
-            fuse_loss = train and worker.fuse_loss and (lp.loss != "softmax_xent" or ks.cols <= 32)
+            # the element-wise heads take any width; a softmax row (dense or sparse labels) must fit one 32-column
+            # epilogue chunk
+            fuse_loss = train and worker.fuse_loss and (lp.loss not in ("softmax_xent", "sparse_softmax_xent") or ks.cols <= 32)
             if fuse_loss:
                 dz_last, dzT_last = zeros(B, round_up(ks.cols, 8)), (None if use_mn else zeros(ks.cols, ldB))
                 db = P(worker.grads) + bs.offset * 4 if bs else 0
@@ -413,6 +414,9 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
         args = (P(out_f32), n_out, P(target), target.shape[1])
         if lp.loss == "softmax_xent":
             plan.add_softmax_xent(*args, loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
+        elif lp.loss == "sparse_softmax_xent":
+            # a label row of width 1 < n_out: the binding reads it as one class index per row
+            plan.add_softmax_xent(P(out_f32), n_out, P(target), 1, loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
         elif lp.loss == "sigmoid_xent":
             plan.add_sigmoid_xent(*args, loss, dz, ld_dz, dzT, ld_t, db, B, n_out)
         elif lp.loss == "mse":

@@ -32,6 +32,20 @@ from ..graph.ir import GraphIR
 Rows = Union[slice, np.ndarray]
 
 
+def check_class_labels(labels: np.ndarray, n_classes: int) -> None:
+    """Class-index labels of a sparse softmax cross-entropy plan: each must be finite and truncate (toward zero, as TF's
+    Cast does) into [0, n_classes).  TF rejects any other label too; the step kernels would silently give its row no
+    target.  Raises ValueError naming the first bad row."""
+    v = np.asarray(labels, dtype=np.float32)
+    v = v[:, 0] if v.ndim == 2 else v.reshape(-1)
+    with np.errstate(invalid="ignore"):
+        bad = ~np.isfinite(v) | (np.trunc(v) < 0) | (np.trunc(v) >= n_classes)
+    if bad.any():
+        r = int(np.argmax(bad))
+        raise ValueError(f"label {v[r]} of row {r} is not a class index in [0, {n_classes}) (the graph takes class labels "
+                         f"through a sparse softmax cross-entropy over {n_classes} classes)")
+
+
 def clamp_batch(n: int, mini_batch_size: int) -> int:
     """``mini_batch_size > n  ->  n - 1`` (reference quirk, ml_util.py:105-106)."""
     return n - 1 if mini_batch_size > n else mini_batch_size
@@ -200,6 +214,9 @@ class B200Engine(Engine):
         minibatch host->device.  ``resident``: the partition is uploaded to HBM once (80 GB per H100 hold any Spark
         partition the reference could train on); shuffles are a device index permutation and every step gathers its rows
         on the device - no PCIe traffic in the training loop.  ``auto``: resident when it fits in a quarter of free HBM."""
+        lp = self.w.plan
+        if labels is not None and lp.loss == "sparse_softmax_xent":
+            check_class_labels(labels, lp.layers[-1].out_features)        # before any device work
         self.X = torch.as_tensor(np.ascontiguousarray(features, dtype=np.float32)).pin_memory()
         self.Y = None
         if labels is not None and not self.w.plan.target_is_input:

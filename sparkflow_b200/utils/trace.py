@@ -16,7 +16,7 @@ from ..ops import native
 
 KERNEL_NAMES = {1: "gemm", 2: "cast_transpose", 3: "softmax_xent", 4: "mse", 5: "argmax", 6: "push", 7: "pull", 8: "im2col",
                 9: "col2im", 10: "maxpool_fwd", 11: "maxpool_bwd", 12: "maxpool_gen_fwd", 13: "maxpool_gen_bwd", 14: "act_bwd_bias",
-                15: "sigmoid_xent"}
+                15: "sigmoid_xent", 16: "sparse_softmax_xent"}
 
 
 class DeviceTrace:

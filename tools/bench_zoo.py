@@ -43,6 +43,7 @@ def _partition(model: str, rows: int):
 
     from sparkflow_b200.graph.ir import GraphIR
     from sparkflow_b200.models import zoo
+    from sparkflow_b200.models.compiler import compile_graph
 
     graph = zoo.build(model)
     ir = GraphIR.from_metagraph(graph)
@@ -52,6 +53,10 @@ def _partition(model: str, rows: int):
     rng = np.random.default_rng(100)
     x = rng.random((rows, in_dim), dtype=np.float32)
     y = np.eye(n_classes, dtype=np.float32)[rng.integers(0, n_classes, rows)] if n_classes else None
+    lp = compile_graph(ir, "x:0", "y:0") if n_classes else None
+    if lp is not None and lp.loss == "sparse_softmax_xent":
+        # a [None, 1] column of class indices (a StringIndexer output)
+        y = rng.integers(0, lp.layers[-1].out_features, (rows, 1)).astype(np.float32)
     return graph, x, y
 
 

@@ -37,7 +37,12 @@ if resident:
     rows = 20 * BATCH
     D = w.plan.input_dim
     x = rng.random((rows, D), dtype=np.float32)
-    y = None if w.plan.target_is_input else np.eye(w.plan.label_dim, dtype=np.float32)[rng.integers(0, w.plan.label_dim, rows)]
+    if w.plan.target_is_input:
+        y = None
+    elif w.plan.loss == "sparse_softmax_xent":                    # one class index per row
+        y = rng.integers(0, w.plan.layers[-1].out_features, (rows, 1)).astype(np.float32)
+    else:
+        y = np.eye(w.plan.label_dim, dtype=np.float32)[rng.integers(0, w.plan.label_dim, rows)]
     eng_r = B200Engine(w)
     eng_r.partition_mode = "resident"
     eng_r.load_partition(x, y)
@@ -89,7 +94,7 @@ for kid, rs in by_kid.items():
         cur["end"] = max(cur["end"], r["t2"])
 summ.sort(key=lambda c: c["ready"])
 names = {1: "gemm", 2: "cast", 3: "softmax", 4: "mse", 5: "argmax", 6: "push", 7: "pull", 8: "im2col", 9: "col2im", 10: "pool_fwd", 11: "pool_bwd", 12: "pool_gen_fwd", 13: "pool_gen_bwd",
-         14: "act_bwd", 15: "sigmoid_xent"}
+         14: "act_bwd", 15: "sigmoid_xent", 16: "sparse_softmax_xent"}
 print("card:", torch.cuda.get_device_name(0), "| plan:", plan.names())
 print("%-8s %5s %9s %9s %9s %8s" % ("kernel", "ctas", "start_us", "ready_us", "end_us", "dur_us"))
 for s in summ:
