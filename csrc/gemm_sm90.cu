@@ -811,6 +811,11 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->ep.loss_mode < SF_LOSS_NONE || g->ep.loss_mode > SF_LOSS_SPARSE_SOFTMAX_XENT) return -5;
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->bn > 64) g->bn = 64;    // the widest tile of its variant
+  if (g->ep.loss_mode == SF_LOSS_SOFTMAX_XENT || g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT) {
+    // the row must fit one epilogue chunk; settled before the B tensor map, whose box height is the tile width
+    if (g->N > 32) return -5;
+    g->bn = 32;
+  }
   if (g->split_k <= 0) g->split_k = 1;
   // large, un-split problems go to the persistent cluster-pair kernel (gemm_pair_sm90.cu): 256 x 128 tiles per CTA pair.
   // A GEMM that carries the fused read-your-writes wait stays on the one-CTA kernel, the only one that implements it.
@@ -846,10 +851,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   g->kblocks_per_split = (total_kb + g->split_k - 1) / g->split_k;
   g->split_k = (total_kb + g->kblocks_per_split - 1) / g->kblocks_per_split;
   if (g->split_k > 1) g->ep.accumulate = 1;
-  if (g->ep.loss_mode == SF_LOSS_SOFTMAX_XENT || g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT) {
-    if (g->N > 32 || g->split_k > 1) return -5;     // the row must fit one epilogue chunk
-    g->bn = 32;
-  }
+  // a loss head needs the finished logits: no K split
   if (g->ep.loss_mode != SF_LOSS_NONE && (g->split_k > 1 || !g->ep.target || !g->ep.loss)) return -5;
   // largest column any output can hold
   int lim = g->N;

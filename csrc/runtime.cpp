@@ -135,6 +135,7 @@ struct Gemm {
   void launch(uintptr_t stream) const { ck_rc(sf_gemm_launch(&g, S(stream)), "sf_gemm_launch"); }
   int bn() const { return g.bn; }
   int split_k() const { return g.split_k; }
+  int kblocks_per_split() const { return g.kblocks_per_split; }
   int pair() const { return g.pair; }
   int epi() const { return g.epi; }
   py::tuple grid() const {
@@ -1055,6 +1056,7 @@ PYBIND11_MODULE(_C, m) {
       .def("launch", &Gemm::launch)
       .def_property_readonly("bn", &Gemm::bn)
       .def_property_readonly("split_k", &Gemm::split_k)
+      .def_property_readonly("kblocks_per_split", &Gemm::kblocks_per_split)
       .def_property_readonly("pair", &Gemm::pair)
       .def_property_readonly("epi", &Gemm::epi)
       .def("mn_major", &Gemm::mn_major)

@@ -17,146 +17,9 @@ def _act(x, a):
     return {None: lambda v: v, "relu": torch.relu, "sigmoid": torch.sigmoid, "tanh": torch.tanh}[a](x)
 
 
-def _dact(a_out, a):
-    if a == "relu":
-        return (a_out > 0).float()
-    if a == "sigmoid":
-        return a_out * (1 - a_out)
-    if a == "tanh":
-        return 1 - a_out * a_out
-    return torch.ones_like(a_out)
-
-
 @pytest.fixture(scope="module")
 def C():
     return native.cuda_ext()
-
-
-def _bf16_pad(x, ld):
-    out = torch.zeros(x.shape[0], ld, dtype=torch.bfloat16, device="cuda")
-    out[:, : x.shape[1]] = x.to(torch.bfloat16)
-    return out
-
-
-def _run_gemm(C, M, N, K, bn=0, split_k=1, bias=False, act=None, aux_act=None, colsum=False, want_bf16=True,
-              want_t=True, accumulate=False, seed=0, pair=-1, pair_ctas=0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    a = torch.randn(M, K, device="cuda", generator=g) * 0.5
-    b = torch.randn(N, K, device="cuda", generator=g) * 0.5
-    lda, ldb = round_up(K, 8), round_up(K, 8)
-    a16, b16 = _bf16_pad(a, lda), _bf16_pad(b, ldb)
-    ref = a16[:, :K].float() @ b16[:, :K].float().t()
-    ldn = round_up(N, 8)
-    ldt = round_up(M, 8)
-    out_f32 = torch.full((M, N), 7.0 if accumulate else float("nan"), device="cuda")
-    out_bf16 = torch.zeros(M, ldn, dtype=torch.bfloat16, device="cuda") if want_bf16 else None
-    outT = torch.zeros(N, ldt, dtype=torch.bfloat16, device="cuda") if want_t else None
-    bias_t = torch.randn(N, device="cuda", generator=g) if bias else None
-    aux = None
-    if aux_act is not None:
-        aux = _bf16_pad(_act(torch.randn(M, N, device="cuda", generator=g), aux_act), ldn)
-    cs = torch.zeros(N, device="cuda") if colsum else None
-    d = dict(a=native.ptr(a16), b=native.ptr(b16), M=M, N=N, K=K, lda=lda, ldb=ldb, bn=bn, split_k=split_k,
-             out_f32=native.ptr(out_f32), ld_f32=N, out_bf16=native.ptr(out_bf16), ld_bf16=ldn,
-             outT_bf16=native.ptr(outT), ld_t=ldt, bias=native.ptr(bias_t), act=ACT[act], aux=native.ptr(aux),
-             ld_aux=ldn, aux_act=ACT[aux_act], colsum=native.ptr(cs), alpha=1.0, accumulate=int(accumulate), pair=pair,
-             pair_ctas=pair_ctas)
-    gm = C.Gemm(d)
-    gm.launch(native.current_stream())
-    torch.cuda.synchronize()
-    assert C.read_error_code() == 0
-    exp = ref
-    if bias:
-        exp = exp + bias_t
-    exp = _act(exp, act)
-    if aux is not None:
-        exp = exp * _dact(aux[:, :N].float(), aux_act)
-    tol = dict(rtol=2e-2, atol=2e-2 * max(1.0, K ** 0.5 * 0.25))
-    got = out_f32 - 7.0 if accumulate else out_f32
-    torch.testing.assert_close(got, exp, **tol)
-    if want_bf16:
-        torch.testing.assert_close(out_bf16[:, :N].float(), exp, rtol=3e-2, atol=tol["atol"] + 0.05)
-        assert torch.all(out_bf16[:, N:] == 0)
-    if want_t:
-        torch.testing.assert_close(outT[:, :M].float().t(), exp, rtol=3e-2, atol=tol["atol"] + 0.05)
-    if colsum:
-        torch.testing.assert_close(cs, exp.sum(0), rtol=2e-2, atol=tol["atol"] * 4)
-    return gm
-
-
-@pytest.mark.parametrize("M,N,K", [(128, 32, 64), (128, 64, 128), (300, 256, 784), (300, 10, 256),
-                                     (784, 256, 300), (256, 10, 300), (1000, 520, 1000)])
-def test_gemm_plain(C, M, N, K):
-    _run_gemm(C, M, N, K)
-
-
-@pytest.mark.parametrize("bn", [32, 64, 128, 256])
-def test_gemm_tile_widths(C, bn):
-    _run_gemm(C, 384, 512, 320, bn=bn)
-
-
-def test_gemm_bias_relu(C):
-    _run_gemm(C, 300, 256, 784, bias=True, act="relu")
-
-
-def test_gemm_bias_sigmoid_tanh(C):
-    _run_gemm(C, 257, 130, 200, bias=True, act="sigmoid")
-    _run_gemm(C, 257, 130, 200, bias=True, act="tanh")
-
-
-def test_gemm_dgrad_epilogue(C):
-    _run_gemm(C, 300, 256, 10, aux_act="relu", colsum=True)
-    _run_gemm(C, 300, 256, 256, aux_act="sigmoid", colsum=True)
-
-
-def test_gemm_split_k_accumulate(C):
-    gm = _run_gemm(C, 32, 64, 4096, split_k=8, want_bf16=False, want_t=False, accumulate=True)
-    assert gm.split_k == 8
-
-
-def test_gemm_large(C):
-    _run_gemm(C, 2048, 2048, 2048, want_t=False)
-
-
-@pytest.mark.parametrize("M,N,K,bn,split_k", [(784, 256, 300, 0, 1), (256, 256, 300, 64, 1), (256, 10, 300, 0, 1), (1600, 10, 300, 0, 1),
-                                              (288, 64, 30000, 0, 8), (25, 32, 4000, 64, 1), (4096, 4096, 300, 128, 1), (130, 70, 17, 0, 1)])
-def test_gemm_mn_major_operands(C, M, N, K, bn, split_k):
-    """D = a^T . b with a [K, M] and b [K, N] row-major (both operands MN-major for the tensor core): the weight-gradient
-    form dW = activations^T . dz consumed straight from the row-major activation / dz buffers, no transposed copies."""
-    g = torch.Generator(device="cuda").manual_seed(7)
-    lda, ldb = round_up(M, 8), round_up(N, 8)
-    a = torch.zeros(K, lda, dtype=torch.bfloat16, device="cuda")
-    b = torch.zeros(K, ldb, dtype=torch.bfloat16, device="cuda")
-    a[:, :M] = (torch.randn(K, M, device="cuda", generator=g) * 0.5).to(torch.bfloat16)
-    b[:, :N] = (torch.randn(K, N, device="cuda", generator=g) * 0.5).to(torch.bfloat16)
-    ref = a[:, :M].float().t() @ b[:, :N].float()
-    out = torch.zeros(M, N, device="cuda") if split_k > 1 else torch.full((M, N), float("nan"), device="cuda")
-    cs = torch.zeros(N, device="cuda")
-    gm = C.Gemm(dict(a=native.ptr(a), lda=lda, b=native.ptr(b), ldb=ldb, M=M, N=N, K=K, mn_major=1, bn=bn, split_k=split_k,
-                     out_f32=native.ptr(out), ld_f32=N, colsum=native.ptr(cs) if split_k == 1 else 0, accumulate=1 if split_k > 1 else 0))
-    assert gm.mn_major() == 1 and gm.bn in (64, 128)
-    gm.launch(torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    scale = max(1.0, ref.abs().max().item())
-    assert torch.isfinite(out).all()
-    assert (out - ref).abs().max().item() < 2e-2 * scale * (K / 300) ** 0.5 + 1e-3
-    if split_k == 1:
-        assert torch.allclose(cs, ref.sum(0), rtol=2e-2, atol=2e-2 * scale)
-
-
-@pytest.mark.parametrize("M,N,K,ctas", [(512, 512, 256, 0), (1000, 520, 1000, 0), (256, 256, 64, 0), (2048, 2048, 512, 8),
-                                          (1536, 1280, 320, 6), (4096, 4096, 1024, 0)])
-def test_gemm_pair_kernel(C, M, N, K, ctas):
-    """persistent 2-CTA (cta_group::2) kernel: tails, more tiles than CTA pairs (double-buffered TMEM phases)"""
-    gm = _run_gemm(C, M, N, K, pair=1, pair_ctas=ctas, want_t=(M * N <= 1 << 22))
-    assert gm.pair == 1
-
-
-def test_gemm_pair_kernel_epilogues(C):
-    gm = _run_gemm(C, 768, 512, 512, pair=1, bias=True, act="relu")
-    assert gm.pair == 1
-    _run_gemm(C, 768, 512, 512, pair=1, aux_act="sigmoid", colsum=True)
-    _run_gemm(C, 512, 768, 256, pair=1, want_bf16=False, want_t=False, accumulate=True)
 
 
 def test_cast_transpose(C):
@@ -350,61 +213,6 @@ def test_plan_capture_replay(C):
         plan.replay(st.cuda_stream)
     st.synchronize()
     assert torch.equal(out, x.to(torch.bfloat16))
-
-
-def test_gemm_fused_softmax_xent_epilogue(C):
-    """Last dense layer + softmax-CE + gradient in one kernel (dz, dz^T, dbias, loss)."""
-    M, N, K = 300, 10, 256
-    g = torch.Generator(device="cuda").manual_seed(0)
-    a = (torch.randn(M, K, device="cuda", generator=g) * 0.3).to(torch.bfloat16)
-    w = (torch.randn(N, K, device="cuda", generator=g) * 0.3).to(torch.bfloat16)
-    bias = torch.randn(N, device="cuda", generator=g)
-    y = torch.nn.functional.one_hot(torch.randint(0, N, (M,), device="cuda"), N).float()
-    ldn, ldt = round_up(N, 8), round_up(M, 8)
-    dz = torch.full((M, ldn), 3.0, dtype=torch.bfloat16, device="cuda")
-    dzT = torch.zeros(N, ldt, dtype=torch.bfloat16, device="cuda")
-    db = torch.zeros(N, device="cuda")
-    loss = torch.zeros(1, device="cuda")
-    gm = C.Gemm(dict(a=native.ptr(a), b=native.ptr(w), M=M, N=N, K=K, lda=K, ldb=K, bias=native.ptr(bias), loss_mode=1,
-                     target=native.ptr(y), ld_target=N, loss=native.ptr(loss), out_bf16=native.ptr(dz), ld_bf16=ldn,
-                     outT_bf16=native.ptr(dzT), ld_t=ldt, colsum=native.ptr(db)))
-    gm.launch(native.current_stream())
-    torch.cuda.synchronize()
-    z = (a.float() @ w.float().t() + bias).requires_grad_(True)
-    ref = -(y * torch.log_softmax(z, 1)).sum(1).mean()
-    ref.backward()
-    torch.testing.assert_close(loss[0], ref.detach(), rtol=1e-3, atol=1e-4)
-    torch.testing.assert_close(dz[:, :N].float(), z.grad, rtol=2e-2, atol=2e-5)
-    torch.testing.assert_close(dzT[:, :M].float().t(), z.grad, rtol=2e-2, atol=2e-5)
-    assert torch.all(dz[:, N:] == 0)
-    torch.testing.assert_close(db, z.grad.sum(0), rtol=1e-2, atol=1e-5)
-
-
-@pytest.mark.parametrize("act", [None, "sigmoid"])
-def test_gemm_fused_mse_epilogue(C, act):
-    M, N, K = 256, 784, 256
-    g = torch.Generator(device="cuda").manual_seed(1)
-    a = (torch.randn(M, K, device="cuda", generator=g) * 0.2).to(torch.bfloat16)
-    w = (torch.randn(N, K, device="cuda", generator=g) * 0.2).to(torch.bfloat16)
-    bias = torch.randn(N, device="cuda", generator=g) * 0.1
-    tgt = torch.rand(M, N, device="cuda", generator=g)
-    ldn, ldt = round_up(N, 8), round_up(M, 8)
-    dz = torch.zeros(M, ldn, dtype=torch.bfloat16, device="cuda")
-    dzT = torch.zeros(N, ldt, dtype=torch.bfloat16, device="cuda")
-    db = torch.zeros(N, device="cuda")
-    loss = torch.zeros(1, device="cuda")
-    gm = C.Gemm(dict(a=native.ptr(a), b=native.ptr(w), M=M, N=N, K=K, lda=K, ldb=K, bias=native.ptr(bias), act=ACT[act],
-                     loss_mode=2, target=native.ptr(tgt), ld_target=N, loss=native.ptr(loss), out_bf16=native.ptr(dz),
-                     ld_bf16=ldn, outT_bf16=native.ptr(dzT), ld_t=ldt, colsum=native.ptr(db)))
-    gm.launch(native.current_stream())
-    torch.cuda.synchronize()
-    z = (a.float() @ w.float().t() + bias).requires_grad_(True)
-    ref = ((_act(z, act) - tgt) ** 2).mean()
-    ref.backward()
-    torch.testing.assert_close(loss[0], ref.detach(), rtol=1e-3, atol=1e-6)
-    torch.testing.assert_close(dz[:, :N].float(), z.grad, rtol=2e-2, atol=1e-7)
-    torch.testing.assert_close(dzT[:, :M].float().t(), z.grad, rtol=2e-2, atol=1e-7)
-    torch.testing.assert_close(db, z.grad.sum(0), rtol=1e-2, atol=1e-6)
 
 
 def test_plan_branches_fork_join(C):
