@@ -192,11 +192,12 @@ struct EpiFeatures {
 
 // One 32-column chunk of a thread's output row: everything between the accumulator (v, already in registers) and
 // global memory.  `aux_pref` / `tgt_pref` are the act'(a) operand / label row of this chunk when the caller fetched
-// them before the accumulator wait (nullptr: read here).  EXT: the extended activations (twin kernels only).
-template <int EPI, bool EXT>
+// them before the accumulator wait (nullptr: read here).  EXT: the extended activations (twin kernels only).  PEN: the L2
+// weight penalty (penalty kernels only); the chunk's sum of W^2 is added to *pen_sq.
+template <int EPI, bool EXT, bool PEN = false>
 __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32_t (&v)[32], const float* s_bias32, int row, bool row_ok,
                                           int col0, int M, int N, int lane, const uint4* aux_pref, const float* tgt_pref,
-                                          unsigned long long* tq = nullptr) {
+                                          unsigned long long* tq = nullptr, float* pen_sq = nullptr) {
     using F = EpiFeatures<EPI>;
     float f[32];
 #pragma unroll
@@ -328,6 +329,27 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
 #pragma unroll
     for (int j = 0; j < 32; ++j)
       if (col0 + j >= N || !row_ok) f[j] = 0.f;
+    if constexpr (PEN) {
+      // the penalty gradient 2c * W, added once: by K split 0 only (the other splits accumulate into the same element)
+      if (ep.pen_w != nullptr && blockIdx.z == 0 && row_ok) {
+        float sq = 0.f;
+        // eight weights in flight at a time: all 32 at once would spill the WGRAD variant's registers
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+#pragma unroll
+          for (int j = 8 * g; j < 8 * g + 8; ++j) {
+            if (col0 + j < N) {
+              const size_t at = ep.pen_wt ? static_cast<size_t>(col0 + j) * ep.pen_ld + row : static_cast<size_t>(row) * ep.pen_ld + col0 + j;
+              const float w = __bfloat162float(ep.pen_w[at]);
+              f[j] += ep.pen_w2c * w;
+              sq += w * w;
+            }
+          }
+          asm volatile("" ::: "memory");
+        }
+        *pen_sq += sq;
+      }
+    }
 
     if (F::kColsum && ep.colsum != nullptr) {
       // transpose-reduce over the 32 rows held by this warp: 31 shuffles, lane j ends up with
@@ -495,8 +517,9 @@ __device__ __forceinline__ void epi_prefetch(const SfGemmEpilogue& ep, uint4 (&a
 
 // Epilogue of one 128 x BN tile from the staged accumulator, by the 256 consumer threads: warp q owns rows
 // 32 * (q % 4) .. + 32 (one row per lane) and every other 32-column chunk starting at chunk q / 4.  aux_pref / tgt_pref:
-// the thread's chunk fetched by epi_prefetch (variants with EpiFeatures::kPrefetch only).
-template <int BN, int EPI, bool EXT>
+// the thread's chunk fetched by epi_prefetch (variants with EpiFeatures::kPrefetch only).  PEN: the L2 weight penalty, whose
+// loss term each warp adds with one atomic.
+template <int BN, int EPI, bool EXT, bool PEN = false>
 __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const float* stg, const float* s_bias, int m0, int n0, int M,
                                               int N, int ct, const uint4* aux_pref = nullptr, const float* tgt_pref = nullptr) {
   using F = EpiFeatures<EPI>;
@@ -505,6 +528,7 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
   const int row = m0 + r;
   const bool row_ok = row < M;
   const float* srow = stg + r * (BN + 1);
+  float pen_sq = 0.f;
 #pragma unroll 1
   for (int c = q >> 2; c < BN / 32; c += 2) {
     const int col0 = n0 + c * 32;
@@ -512,7 +536,10 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
     uint32_t v[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(srow[c * 32 + j]);
-    if constexpr (F::kPrefetch) {
+    if constexpr (PEN) {
+      static_assert(!F::kPrefetch, "the penalty rides on weight-gradient epilogues (sf_gemm_prepare refuses a loss head)");
+      epi_chunk<EPI, EXT, true>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, nullptr, nullptr, nullptr, &pen_sq);
+    } else if constexpr (F::kPrefetch) {
       epi_chunk<EPI, EXT>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, aux_pref, tgt_pref);
     } else {
       float tgt[32];
@@ -524,6 +551,11 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
       epi_chunk<EPI, EXT>(ep, v, s_bias + c * 32, row, row_ok, col0, M, N, lane, nullptr, F::kLoss ? tgt : nullptr);
     }
   }
+  if constexpr (PEN) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) pen_sq += __shfl_xor_sync(0xffffffffu, pen_sq, o);
+    if (lane == 0 && pen_sq != 0.f) atomicAdd(ep.pen_loss, 0.5f * ep.pen_w2c * pen_sq);
+  }
 }
 
 // Thread roles (384 threads): warp 0 lane 0 is the TMA producer, warps 1-3 load the bias tile, warpgroups 1 and 2 each
@@ -531,8 +563,8 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 // MN: both operands MN-major (D = a^T . b with a [K, M], b [K, N] row-major): the stage buffers have the same size, but a
 // stage is filled with {64 MN elements, 64 K rows} boxes and described to the tensor core as MN-major.
 // EPI: epilogue feature set (SfEpi); only the generic kernel handles the fused read-your-writes wait.  EXT: the extended
-// activations are compiled in (the twin kernels below).
-template <int BN, bool MN, int EPI, bool EXT = false>
+// activations are compiled in (the twin kernels below).  PEN: the L2 weight penalty (the penalty kernels below).
+template <int BN, bool MN, int EPI, bool EXT = false, bool PEN = false>
 __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorMap& tmB, const SfGemmEpilogue& ep, int M, int N,
                                          int K, int kblocks_per_split) {
   static_assert(!MN || BN % 64 == 0, "MN-major B needs whole 64-element swizzle atoms");
@@ -626,6 +658,22 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
     for (int j = threadIdx.x - 32; j < BN; j += 96)
       s_bias[j] = (ep.bias != nullptr && is_split0 && n0 + j < N) ? ep.bias[n0 + j] : 0.f;
     asm volatile("bar.arrive 2, 352;" ::: "memory");
+    if constexpr (PEN) {
+      // the bias term of the penalty, once per column: by the CTAs of row tile 0, split 0
+      if (ep.pen_b != nullptr && is_split0 && blockIdx.y == 0) {
+        float sq = 0.f;
+        for (int j = threadIdx.x - 32; j < BN; j += 96) {
+          if (n0 + j < N) {
+            const float b = ep.pen_b[n0 + j];
+            atomicAdd(ep.pen_db + n0 + j, ep.pen_b2c * b);
+            sq += b * b;
+          }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+        if (lane == 0 && sq != 0.f) atomicAdd(ep.pen_loss, 0.5f * ep.pen_b2c * sq);
+      }
+    }
   } else {
     // ===================== wgmma main loop + epilogue =====================
     const int ct = threadIdx.x - 128;
@@ -648,7 +696,7 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
     if constexpr (F::kPrefetch) {
       epilogue_tile<BN, EPI, EXT>(ep, stg, s_bias, m0, n0, M, N, ct, aux_pref, tgt_pref);
     } else {
-      epilogue_tile<BN, EPI, EXT>(ep, stg, s_bias, m0, n0, M, N, ct);
+      epilogue_tile<BN, EPI, EXT, PEN>(ep, stg, s_bias, m0, n0, M, N, ct);
     }
   }
   trace.end(KID_GEMM);
@@ -706,6 +754,22 @@ sf_gemm_epi_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                        const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
   static_assert(EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD, "only these variants apply an activation");
   gemm_cta<BN, false, EPI, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+
+// Penalty kernels: the weight-gradient GEMMs of a layer with an L2 weight penalty (SfGemmEpilogue.pen_*).  The generic
+// one-CTA kernel (K-major wgrads, split-K conv wgrads, route mode, accumulate) and the MN-major WGRAD variant, each with the
+// penalty compiled in, so that no other GEMM carries its code.
+template <int BN, bool MN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_pen_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  gemm_cta<BN, MN, SF_EPI_GENERIC, false, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+}
+template <int BN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+sf_gemm_wgrad_pen_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                         const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
+  gemm_cta<BN, true, SF_EPI_WGRAD, false, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
 }
 
 // ---------------------------------------------------------------------------
@@ -803,12 +867,21 @@ static int pick_epi(const SfGemm* g) {
 
 // the epilogue applies (or differentiates) one of the extended activations: the GEMM runs on a twin kernel
 static bool uses_ext_act(const SfGemmEpilogue& e) { return e.act >= SF_ACT_ELU || e.aux_act >= SF_ACT_ELU; }
+// the GEMM carries an L2 weight penalty: it runs on a penalty kernel
+static bool has_penalty(const SfGemmEpilogue& e) { return e.pen_w != nullptr || e.pen_b != nullptr; }
 
 extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return -2;
   if (g->ep.act < SF_ACT_NONE || g->ep.act > SF_ACT_RELU6 || g->ep.aux_act < SF_ACT_NONE || g->ep.aux_act > SF_ACT_RELU6) return -5;
   if (g->mn_major && uses_ext_act(g->ep)) return -7;     // no MN-major twin: the weight-gradient GEMMs apply no activation
   if (g->ep.loss_mode < SF_LOSS_NONE || g->ep.loss_mode > SF_LOSS_SPARSE_SOFTMAX_XENT) return -5;
+  if (has_penalty(g->ep)) {
+    // a weight gradient: fp32 output (or routed), no activation, loss head or bf16 output; the loss term needs its target
+    if (g->ep.pen_loss == nullptr || (g->ep.pen_w != nullptr && g->ep.pen_ld <= 0) || (g->ep.pen_b != nullptr && g->ep.pen_db == nullptr) ||
+        uses_ext_act(g->ep) || g->ep.loss_mode != SF_LOSS_NONE || g->ep.act != SF_ACT_NONE || g->ep.aux != nullptr ||
+        g->ep.out_bf16 != nullptr || g->ep.outT_bf16 != nullptr || g->ep.drop_keep != 0.f || (g->ep.out_f32 == nullptr && g->ep.route == nullptr))
+      return -5;
+  }
   if (g->bn == 0) g->bn = sf_gemm_pick_bn(g->M, g->N);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->bn > 64) g->bn = 64;    // the widest tile of its variant
   if (g->ep.loss_mode == SF_LOSS_SOFTMAX_XENT || g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT) {
@@ -821,10 +894,13 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   // A GEMM that carries the fused read-your-writes wait stays on the one-CTA kernel, the only one that implements it.
   {
     const long long pair_tiles = static_cast<long long>((g->M + 255) / 256) * ((g->N + sf::kPairBN - 1) / sf::kPairBN);
-    const bool eligible = g->split_k == 1 && g->ep.loss_mode == SF_LOSS_NONE && g->ep.ryw == nullptr && g->M >= 256 && g->N >= 256;
+    // a penalised weight gradient stays on the one-CTA kernel too: the pair kernel has no penalty epilogue
+    const bool eligible = g->split_k == 1 && g->ep.loss_mode == SF_LOSS_NONE && g->ep.ryw == nullptr && !has_penalty(g->ep) &&
+                          g->M >= 256 && g->N >= 256;
     const char* env = getenv("SPARKFLOW_GEMM_PAIR");
     int want = g->pair;
     if (env != nullptr && want < 0) want = atoi(env);
+    if (want > 0 && has_penalty(g->ep)) return -7;
     if (want < 0) want = (g->bn == 256 && pair_tiles >= sf_num_sms() / 2 && g->K >= 512) ? 1 : 0;
     g->pair = (want > 0 && eligible && !g->mn_major) ? 1 : 0;
     if (g->pair) g->bn = sf::kPairBN;
@@ -864,11 +940,13 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   return 0;
 }
 
-template <int BN, bool MN = false, int EPI = SF_EPI_GENERIC, bool EXT = false>
+template <int BN, bool MN = false, int EPI = SF_EPI_GENERIC, bool EXT = false, bool PEN = false>
 static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
   using S = sf::GemmSmem<BN>;
   auto kernel = [] {
-    if constexpr (EXT && EPI == SF_EPI_GENERIC) return sf::sf_gemm_ext_kernel<BN>;
+    if constexpr (PEN && EPI == SF_EPI_WGRAD) return sf::sf_gemm_wgrad_pen_kernel<BN>;
+    else if constexpr (PEN) return sf::sf_gemm_pen_kernel<BN, MN>;
+    else if constexpr (EXT && EPI == SF_EPI_GENERIC) return sf::sf_gemm_ext_kernel<BN>;
     else if constexpr (EXT) return sf::sf_gemm_epi_ext_kernel<BN, EPI>;
     else if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
     else if constexpr (EPI == SF_EPI_SIGMOID_LOSS) return sf::sf_gemm_sigmoid_loss_kernel<BN>;
@@ -913,8 +991,35 @@ static int launch_ext(const SfGemm* g, cudaStream_t st) {
   return static_cast<int>(e);
 }
 
+// the penalty kernels: the MN-major WGRAD variant at BN 64 / 128, the generic kernel at every tile width
+static int launch_pen(const SfGemm* g, cudaStream_t st) {
+  cudaError_t e;
+  if (g->epi == SF_EPI_WGRAD) {
+    e = g->bn == 64 ? launch_bn<64, true, SF_EPI_WGRAD, false, true>(g, st) : launch_bn<128, true, SF_EPI_WGRAD, false, true>(g, st);
+    return static_cast<int>(e);
+  }
+  if (g->epi != SF_EPI_GENERIC) return -3;
+  if (g->mn_major) {
+    switch (g->bn) {
+      case 64: e = launch_bn<64, true, SF_EPI_GENERIC, false, true>(g, st); break;
+      case 128: e = launch_bn<128, true, SF_EPI_GENERIC, false, true>(g, st); break;
+      default: return -3;
+    }
+    return static_cast<int>(e);
+  }
+  switch (g->bn) {
+    case 32: e = launch_bn<32, false, SF_EPI_GENERIC, false, true>(g, st); break;
+    case 64: e = launch_bn<64, false, SF_EPI_GENERIC, false, true>(g, st); break;
+    case 128: e = launch_bn<128, false, SF_EPI_GENERIC, false, true>(g, st); break;
+    case 256: e = launch_bn<256, false, SF_EPI_GENERIC, false, true>(g, st); break;
+    default: return -3;
+  }
+  return static_cast<int>(e);
+}
+
 extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
   if (g->pair) return sf_gemm_pair_launch(g, st);
+  if (has_penalty(g->ep)) return launch_pen(g, st);
   if (uses_ext_act(g->ep)) return launch_ext(g, st);
   cudaError_t e;
   switch (g->epi) {

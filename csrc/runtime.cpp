@@ -127,6 +127,14 @@ struct Gemm {
     g.ep.route_tile0 = getd<int>(d, "route_tile0", 0);
     g.ep.route_tiles_c = getd<int>(d, "route_tiles_c", 1);
     g.ep.route_off = getd<long long>(d, "route_off", 0);
+    g.ep.pen_w2c = getd<float>(d, "pen_w2c", 0.0f);
+    g.ep.pen_w = P<const __nv_bfloat16>(getd<uintptr_t>(d, "pen_w", 0));
+    g.ep.pen_ld = getd<int>(d, "pen_ld", 0);
+    g.ep.pen_wt = getd<int>(d, "pen_wt", 0);
+    g.ep.pen_b = P<const float>(getd<uintptr_t>(d, "pen_b", 0));
+    g.ep.pen_b2c = getd<float>(d, "pen_b2c", 0.0f);
+    g.ep.pen_db = P<float>(getd<uintptr_t>(d, "pen_db", 0));
+    g.ep.pen_loss = P<float>(getd<uintptr_t>(d, "pen_loss", 0));
     if ((g.lda % 8) || (g.ldb % 8)) throw std::runtime_error("gemm: lda/ldb must be multiples of 8 (16-byte TMA strides)");
     if (g.ep.out_bf16 && (g.ep.ld_bf16 % 8)) throw std::runtime_error("gemm: ld_bf16 must be a multiple of 8");
     if (g.ep.aux && (g.ep.ld_aux % 8)) throw std::runtime_error("gemm: ld_aux must be a multiple of 8");

@@ -105,6 +105,19 @@ struct SfGemmEpilogue {
   const SfRyw* ryw;               // device memory; nullptr = no wait
   // slope of a leaky ReLU `act` / `aux_act` (SF_ACT_LEAKY_RELU); appended last so every field above keeps its offset
   float act_alpha, aux_act_alpha;
+  // L2 weight penalty c * sum(W^2) + c_b * sum(b^2) of the layer whose weight gradient this GEMM computes (appended last,
+  // like act_alpha).  Set only on weight-gradient GEMMs; they then run the penalty kernels (sf_gemm_prepare).
+  //   weight: K split 0 adds pen_w2c * W to every fp32 output element (before the store, atomic add or routed red), W
+  //           read from the bf16 replica the step computed with: W [M, pen_ld] or, pen_wt = 1, W^T [N, pen_ld]
+  //   bias:   the CTAs of row tile 0, split 0 atomically add pen_b2c * b[n] into pen_db[n]
+  //   loss:   pen_w2c / 2 * sum(W^2) + pen_b2c / 2 * sum(b^2) over the elements a CTA covers, atomically added to pen_loss
+  float pen_w2c;                  // 2c (0 with pen_w = nullptr: no weight term)
+  const __nv_bfloat16* pen_w;
+  int pen_ld, pen_wt;
+  const float* pen_b;             // fp32 bias [N] (nullptr: no bias term)
+  float pen_b2c;                  // 2c_b
+  float* pen_db;                  // bias gradient [N]
+  float* pen_loss;                // loss accumulator (required with a penalty)
 };
 
 enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, SF_LOSS_SIGMOID_XENT = 3, SF_LOSS_SPARSE_SOFTMAX_XENT = 4 };

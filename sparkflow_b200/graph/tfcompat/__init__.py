@@ -25,6 +25,7 @@ from .ops import (ceil, clip_by_value, equal, floor, greater, greater_equal, les
                   zeros_like)
 from .ops import (cond, cos, cumsum, erf, floormod, gather, logical_or, one_hot, pad, reduce_all, reduce_any, round, sin, split,  # noqa: A004,F401
                   unstack)
+from .ops import add_n  # noqa: F401
 from .session import InteractiveSession, Session, get_default_session  # noqa: F401
 
 __version__ = "1.10.0-sparkflow_b200"
@@ -91,6 +92,7 @@ losses = _types.SimpleNamespace(
     sigmoid_cross_entropy=_ops.sigmoid_cross_entropy, absolute_difference=_ops.absolute_difference,
     add_loss=_ops.add_loss, get_losses=_ops.get_losses, log_loss=_ops.log_loss, hinge_loss=_ops.hinge_loss,
     huber_loss=_ops.huber_loss, sparse_softmax_cross_entropy=_ops.sparse_softmax_cross_entropy,
+    get_regularization_loss=_ops.get_regularization_loss,
 )
 initializers = _types.SimpleNamespace(
     glorot_uniform=glorot_uniform_initializer, glorot_normal=glorot_normal_initializer, zeros=zeros_initializer,
@@ -100,7 +102,7 @@ initializers = _types.SimpleNamespace(
 contrib = _types.SimpleNamespace(layers=_types.SimpleNamespace(
     xavier_initializer=lambda uniform=True, seed=None, dtype=float32: (glorot_uniform_initializer(seed) if uniform else glorot_normal_initializer(seed)),
     fully_connected=lambda inputs, num_outputs, activation_fn=_ops.relu, **kw: _ops.dense(inputs, num_outputs, activation=activation_fn, **kw),
-    flatten=_ops.flatten,
+    flatten=_ops.flatten, l2_regularizer=_ops.l2_regularizer,
 ))
 train = _train_mod
 keras = _types.SimpleNamespace(initializers=initializers)

@@ -590,8 +590,19 @@ def _apply_activation(fn, x: Tensor) -> Tensor:
     return unary(an, x, name=an)
 
 
+def _regularize(var: Variable, regularizer) -> None:
+    """TF's layer regularizer: ``regularizer(var)`` under ``<var>/Regularizer``, added to REGULARIZATION_LOSSES"""
+    if regularizer is None or var is None:
+        return
+    g = _g()
+    with g.name_scope(f"{var.name.split(':')[0]}/Regularizer/"):
+        r = regularizer(var.value())
+    if r is not None:
+        g.add_to_collection(GraphKeys.REGULARIZATION_LOSSES, r)
+
+
 def dense(inputs, units, activation=None, use_bias=True, kernel_initializer=None, bias_initializer=None, trainable=True,
-          name=None, **_unused) -> Tensor:
+          name=None, kernel_regularizer=None, bias_regularizer=None, **_unused) -> Tensor:
     """``tf.layers.dense``: variables ``<scope>/kernel`` [in, units] and ``<scope>/bias`` [units]."""
     x = convert_to_tensor(inputs)
     g = _g()
@@ -602,6 +613,8 @@ def dense(inputs, units, activation=None, use_bias=True, kernel_initializer=None
         sc = scope[:-1]
         kernel = _make_variable(f"{sc}/kernel", (in_dim, units), x.dtype, kernel_initializer or _GlorotUniform(), trainable)
         bias = _make_variable(f"{sc}/bias", (units,), x.dtype, bias_initializer or _Zeros(), trainable) if use_bias else None
+        _regularize(kernel, kernel_regularizer)
+        _regularize(bias, bias_regularizer)
         if len(x._shape) > 2:
             raise NotImplementedError("dense on rank>2 inputs is not supported by the tfcompat builder")
         out = matmul(x, kernel.value(), name="MatMul")
@@ -615,7 +628,8 @@ def _pair(v) -> Tuple[int, int]:
 
 
 def conv2d_layer(inputs, filters, kernel_size, strides=(1, 1), padding="valid", activation=None, use_bias=True,
-                 kernel_initializer=None, bias_initializer=None, trainable=True, name=None, **_unused) -> Tensor:
+                 kernel_initializer=None, bias_initializer=None, trainable=True, name=None, kernel_regularizer=None,
+                 bias_regularizer=None, **_unused) -> Tensor:
     """``tf.layers.conv2d`` (NHWC): variables ``<scope>/kernel`` [kh, kw, cin, filters], ``<scope>/bias``."""
     x = convert_to_tensor(inputs)
     g = _g()
@@ -626,6 +640,8 @@ def conv2d_layer(inputs, filters, kernel_size, strides=(1, 1), padding="valid", 
         sc = scope[:-1]
         kernel = _make_variable(f"{sc}/kernel", (kh, kw, cin, filters), x.dtype, kernel_initializer or _GlorotUniform(), trainable)
         bias = _make_variable(f"{sc}/bias", (filters,), x.dtype, bias_initializer or _Zeros(), trainable) if use_bias else None
+        _regularize(kernel, kernel_regularizer)
+        _regularize(bias, bias_regularizer)
         out = conv2d(x, kernel.value(), (1, sh, sw, 1), padding, name="Conv2D")
         if bias is not None:
             out = bias_add(out, bias.value(), name="BiasAdd")
@@ -734,6 +750,44 @@ def add_loss(loss, loss_collection=GraphKeys.LOSSES):
 
 def get_losses(scope=None, loss_collection=GraphKeys.LOSSES):
     return _g().get_collection(loss_collection, scope)
+
+
+def add_n(inputs, name=None) -> Tensor:
+    """``tf.add_n``: one AddN node over every input; as in TF, a single input is returned as it is (through an Identity
+    when a name is given)"""
+    xs = [convert_to_tensor(x) for x in inputs]
+    if not xs:
+        raise ValueError("add_n needs at least one input")
+    if len(xs) == 1:
+        return identity(xs[0], name=name) if name else xs[0]
+    return _g().add_node("AddN", name or "AddN", xs, {"T": attr_type(xs[0].dtype), "N": attr_i(len(xs))}, [xs[0].dtype],
+                         [xs[0]._shape]).outputs[0]
+
+
+def l2_regularizer(scale, scope=None):
+    """``tf.contrib.layers.l2_regularizer``: w -> Mul(scale, L2Loss(w)) under ``l2_regularizer``; scale 0 regularizes nothing"""
+    scale = float(scale)
+    if scale < 0.0 or not math.isfinite(scale):
+        raise ValueError(f"l2_regularizer: scale must be a finite value >= 0, got {scale}")
+    if scale == 0.0:
+        return lambda weights: None
+
+    def l2(weights):
+        w = convert_to_tensor(weights)
+        g = _g()
+        with g.name_scope(scope or "l2_regularizer"):
+            k = constant(np.float32(scale), dtype=w.dtype, name="scale")
+            sq = g.add_node("L2Loss", "L2Loss", [w], {"T": attr_type(w.dtype)}, [w.dtype], [()]).outputs[0]
+            return binary("Mul", k, sq, name="value")
+    return l2
+
+
+def get_regularization_loss(scope=None, name="total_regularization_loss") -> Tensor:
+    """``tf.losses.get_regularization_loss``: AddN of the REGULARIZATION_LOSSES collection, or the constant 0"""
+    losses = _g().get_collection(GraphKeys.REGULARIZATION_LOSSES, scope)
+    if losses:
+        return add_n(losses, name=name)
+    return constant(np.float32(0.0), name="zero_regularization_loss")
 
 
 # -------------------------------------------------------------------------------------------------

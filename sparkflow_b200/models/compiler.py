@@ -17,6 +17,7 @@ VALID or SAME padding (e.g. the "Deep MNIST" network).  Output sizes and pads fo
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
@@ -83,6 +84,8 @@ class LayerPlan:
     label_dim: int                              # label columns fed per row (1 for sparse_softmax_xent: the class index)
     output: Optional[OutputSpec]
     var_order: List[str]
+    # L2 weight penalties of the loss: variable -> c of the term c * sum(v ** 2) (kernels and biases of the layers only)
+    penalty: Dict[str, float] = field(default_factory=dict)
 
     def trainable_layers(self) -> List[Layer]:
         return [l for l in self.layers if l.kind in ("dense", "conv")]
@@ -359,6 +362,167 @@ def _match_activation(ir: GraphIR, node: Node) -> Optional[Tuple[str, float, Tup
     return node.op, 0.0, node.inputs[0]
 
 
+def _strip_pass(ir: GraphIR, ref: Tuple[str, int]) -> Node:
+    node = ir.nodes[ref[0]]
+    while node.op in _PASS and node.inputs:
+        node = ir.nodes[node.inputs[0][0]]
+    return node
+
+
+def _sums_all_axes(ir: GraphIR, node: Node, var: str) -> bool:
+    """Sum ``node`` reduces every axis of variable ``var``"""
+    if len(node.inputs) != 2 or ir.nodes[node.inputs[1][0]].op != "Const":
+        return False
+    rank = len(ir.nodes[var].attrs.get("shape", ()))
+    axes = sorted({int(a) % max(rank, 1) for a in ir.nodes[node.inputs[1][0]].attrs["value"].reshape(-1)})
+    return axes == list(range(rank))
+
+
+def _const_node(ir: GraphIR, ref: Tuple[str, int]) -> Node:
+    node = ir.nodes[ref[0]]
+    for _ in range(6):
+        if node.op not in ("Identity", "PlaceholderWithDefault", "Cast") or not node.inputs:
+            break
+        node = ir.nodes[node.inputs[0][0]]
+    return node
+
+
+def _scalar_factor(ir: GraphIR, ref: Tuple[str, int]) -> Optional[float]:
+    """The value of ``ref`` when it is a constant of exactly one element (a scalar, or [1], [1, 1], ...), possibly
+    behind Identity / PlaceholderWithDefault / Cast or `a - b` of such constants; None otherwise.  A penalty coefficient
+    must be one: a constant of several elements weighs the elements of the variable differently."""
+    node = _const_node(ir, ref)
+    if node.op == "Const":
+        try:
+            v = node.attrs["value"].reshape(-1)
+        except Exception:
+            return None
+        return float(v[0]) if v.size == 1 else None
+    if node.op == "Sub" and len(node.inputs) == 2:
+        a, b = _scalar_factor(ir, node.inputs[0]), _scalar_factor(ir, node.inputs[1])
+        return None if a is None or b is None else a - b
+    return None
+
+
+def _const_elements(ir: GraphIR, ref: Tuple[str, int]) -> int:
+    """element count of the constant behind ``ref`` (0: not a constant)"""
+    node = _const_node(ir, ref)
+    try:
+        return int(node.attrs["value"].size) if node.op == "Const" else 0
+    except Exception:
+        return 0
+
+
+def _per_element_reason(node: Node, n: int) -> str:
+    return (f"L2 penalty '{node.name}' with a coefficient that is a constant of {n} elements (per-element or masked decay) is "
+            "not covered by the compiled plan: it takes one coefficient per variable")
+
+
+def _l2_terms(ir: GraphIR, ref: Tuple[str, int]) -> Optional[List[Tuple[Tuple[str, int], float]]]:
+    """[(x, c)] when ``ref`` is a sum of L2 penalties c * sum(x ** 2) of the accepted forms - L2Loss(x), Sum(Square(x)),
+    Sum(Mul(k, Square(x))) (Keras's l2) - each, and the sum, times constant factors (the builder's l2_loss is
+    Mul(Sum(Square(x)), 0.5); ``5e-4 * add_n([...])`` scales a sum), or None.  Raises for an L1 term and for a penalty
+    whose coefficient is not a constant."""
+    node = _strip_pass(ir, ref)
+    c = 1.0
+    for _ in range(16):
+        if node.op != "Mul" or len(node.inputs) != 2:
+            break
+        a, b = node.inputs
+        ka, kb = _scalar_factor(ir, a), _scalar_factor(ir, b)
+        if kb is not None:
+            c, node = c * kb, _strip_pass(ir, a)
+        elif ka is not None:
+            c, node = c * ka, _strip_pass(ir, b)
+        else:
+            for k_ref, t_ref in ((a, b), (b, a)):
+                n = _const_elements(ir, k_ref)
+                if n > 1 and _is_penalty_shaped(ir, t_ref):
+                    raise UnsupportedGraph(_per_element_reason(node, n))
+            if _is_penalty_shaped(ir, a) or _is_penalty_shaped(ir, b):
+                raise UnsupportedGraph(f"L2 penalty '{node.name}' with a coefficient that is not a constant is not covered by the "
+                                       "compiled plan")
+            return None
+    if node.op in ("Add", "AddV2", "AddN") and node.inputs:
+        terms = []
+        for i in node.inputs:
+            t = _l2_terms(ir, i)
+            if t is None:
+                return None
+            terms += [(x, c * k) for x, k in t]
+        return terms
+    if node.op == "L2Loss" and len(node.inputs) == 1:
+        return [(node.inputs[0], 0.5 * c)]
+    if node.op != "Sum" or not node.inputs:
+        return None
+    inner = _strip_pass(ir, node.inputs[0])
+    if inner.op == "Mul" and len(inner.inputs) == 2:
+        for k_ref, s_ref in ((inner.inputs[0], inner.inputs[1]), (inner.inputs[1], inner.inputs[0])):
+            k, sq = _scalar_factor(ir, k_ref), _strip_pass(ir, s_ref)
+            if sq.op in ("Square", "Abs") and k is None and _const_elements(ir, k_ref) > 1:
+                raise UnsupportedGraph(_per_element_reason(inner, _const_elements(ir, k_ref)))
+            if k is not None and sq.op in ("Square", "Abs"):
+                c, inner = c * k, sq
+                break
+    if inner.op == "Abs":
+        raise UnsupportedGraph(f"L1 penalty '{node.name}' (Abs) is not covered by the compiled plan")
+    if inner.op != "Square" or len(inner.inputs) != 1:
+        return None
+    var = _var_of(ir, inner.inputs[0])
+    if var is not None and not _sums_all_axes(ir, node, var):
+        raise UnsupportedGraph(f"'{node.name}' sums the squares of a variable over some of its axes: only a penalty over the whole "
+                               "variable is covered by the compiled plan")
+    return [(inner.inputs[0], c)]
+
+
+def _is_penalty_shaped(ir: GraphIR, ref: Tuple[str, int]) -> bool:
+    try:
+        return _l2_terms(ir, ref) is not None
+    except UnsupportedGraph:
+        return True
+
+
+def _split_loss(ir: GraphIR, loss_ref: str) -> Tuple[str, Dict[str, float]]:
+    """Split the training loss into its data term and its L2 weight penalties: a top-level Add / AddV2 / AddN (through
+    Identity, nested in any order) of exactly one data loss and terms c * sum(v ** 2) of bare variables.  Returns the data
+    term and {variable: summed c}, without the variables whose coefficients add to 0."""
+    top = _strip_pass(ir, split_ref(loss_ref))
+    if top.op not in ("Add", "AddV2", "AddN") or _match_sigmoid_xent(ir, top) is not None:
+        return loss_ref, {}
+    terms: List[Tuple[str, int]] = []
+
+    def flatten(node: Node) -> None:
+        for ref in node.inputs:
+            n = _strip_pass(ir, ref)
+            if n.op in ("Add", "AddV2", "AddN") and _match_sigmoid_xent(ir, n) is None:
+                flatten(n)
+            else:
+                terms.append(ref)
+
+    flatten(top)
+    data: List[Tuple[str, int]] = []
+    penalty: Dict[str, float] = {}
+    for ref in terms:
+        l2 = _l2_terms(ir, ref)
+        if l2 is None:
+            if _scalar_factor(ir, ref) == 0.0:         # tf.losses.get_regularization_loss() of a graph without regularizers
+                continue
+            data.append(ref)
+            continue
+        for x, c in l2:
+            var = _var_of(ir, x)
+            if var is None:
+                raise UnsupportedGraph(f"L2 penalty on '{_strip_pass(ir, x).op}' ({x[0]}): the compiled plan covers penalties on bare "
+                                       "variables only (no activity regularizers or penalties of expressions)")
+            if not math.isfinite(c):
+                raise UnsupportedGraph(f"L2 penalty on '{var}' with the coefficient {c} is not covered by the compiled plan")
+            penalty[var] = penalty.get(var, 0.0) + c
+    if len(data) != 1:
+        raise UnsupportedGraph(f"loss '{loss_ref}' adds {len(data)} data losses: the compiled plan covers one data loss plus L2 "
+                               "weight penalties")
+    return f"{data[0][0]}:{data[0][1]}", {v: c for v, c in penalty.items() if c != 0.0}
+
+
 def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
     """Walk back from the scalar loss through reductions / scalings to the per-element loss node."""
     seen = set()
@@ -369,6 +533,9 @@ def _find_loss_core(ir: GraphIR, loss_ref: str) -> Tuple[str, Node]:
             continue
         seen.add(name)
         node = ir.nodes[name]
+        if node.op in ("Add", "AddV2", "AddN") and any(_is_penalty_shaped(ir, i) for i in node.inputs):
+            raise UnsupportedGraph(f"loss '{loss_ref}' adds an L2 penalty under a reduction or a scaling ('{node.name}'): the compiled "
+                                   "plan covers penalties added at the top of the loss")
         if node.op == "SoftmaxCrossEntropyWithLogits":
             # tf.one_hot of class indices as the labels: the sparse head
             return ("sparse_softmax_xent" if _one_hot_of(ir, node.inputs[1]) is not None else "softmax_xent"), node
@@ -437,13 +604,15 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
     input_dim = int(in_shape[1])
 
     loss_kind: Optional[str] = None
+    penalty: Dict[str, float] = {}
     pred_ref: Optional[Tuple[str, int]] = None
     target_ref: Optional[Tuple[str, int]] = None
     if need_loss:
         if not ir.losses:
             raise ValueError("the graph has no 'losses' collection entry; training needs tf.losses.* (or add_loss)")
-        loss_kind, core = _find_loss_core(ir, ir.losses[0])
-        _check_mean_reduction(ir, ir.losses[0], loss_kind, core)
+        data_ref, penalty = _split_loss(ir, ir.losses[0])
+        loss_kind, core = _find_loss_core(ir, data_ref)
+        _check_mean_reduction(ir, data_ref, loss_kind, core)
         a, b = core.inputs[0], core.inputs[1]
         if loss_kind in ("softmax_xent", "sparse_softmax_xent"):
             pred_ref, target_ref = a, b               # (features=logits, labels / class indices / their one_hot)
@@ -700,6 +869,10 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             elif out_spec is None:
                 raise UnsupportedGraph(f"tfOutput '{tf_output}' is not a tensor of the forward chain")
 
+    layer_vars = {v for l in layers for v in (l.kernel, l.bias) if v is not None}
+    for v in penalty:
+        if v not in layer_vars:
+            raise UnsupportedGraph(f"L2 penalty on '{v}', which is not a kernel or bias of a layer of the compiled plan")
     return LayerPlan(layers=layers, loss=loss_kind, input_name=f"{input_node}:0", label_name=label_name,
                      target_is_input=target_is_input, input_dim=input_dim, label_dim=label_dim, output=out_spec,
-                     var_order=[v.name for v in ir.trainable])
+                     var_order=[v.name for v in ir.trainable], penalty=penalty)

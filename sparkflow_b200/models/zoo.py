@@ -15,6 +15,8 @@ Each function mirrors a model definition of the reference:
   * :func:`selu_dnn` / :func:`leaky_cnn` / :func:`softplus_autoencoder` – SELU, leaky ReLU + ELU and softplus networks
   * :func:`sparse_dnn` / :func:`onehot_cnn` / :func:`sparse_dnn100` – classifiers trained on a numeric class column
     ([None, 1] labels) with sparse softmax cross-entropy or a ``tf.one_hot`` in the graph
+  * :func:`l2_dnn` / :func:`l2_cnn` / :func:`l2_autoencoder` – simple_dnn, cnn_same and autoencoder with an L2 weight
+    penalty in the loss, in three TF-1.x spellings
 """
 from __future__ import annotations
 
@@ -197,6 +199,53 @@ def wide_dnn(width: int = 4096, depth: int = 4, classes: int = 1000):
     return tf.losses.softmax_cross_entropy(y, logits)
 
 
+def l2_dnn():
+    """simple_dnn with ``5e-4 * add_n(l2_loss)`` of its three kernels added to the loss"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    h1 = tf.layers.dense(x, 256, activation=tf.nn.relu, kernel_initializer=tf.glorot_uniform_initializer())
+    h2 = tf.layers.dense(h1, 256, activation=tf.nn.relu, kernel_initializer=tf.glorot_uniform_initializer())
+    logits = tf.layers.dense(h2, 10, kernel_initializer=tf.glorot_uniform_initializer())
+    tf.argmax(logits, 1, name="out")
+    kernels = [v for v in tf.trainable_variables() if v.name.split(":")[0].endswith("/kernel")]
+    loss = (tf.reduce_mean(tf.nn.softmax_cross_entropy_with_logits(labels=y, logits=logits))
+            + 5e-4 * tf.add_n([tf.nn.l2_loss(w) for w in kernels]))
+    tf.losses.add_loss(loss)
+    return loss
+
+
+def l2_cnn():
+    """cnn_same with ``l2_regularizer(1e-4)`` kernel regularizers: ``softmax_cross_entropy`` outside the losses
+    collection plus ``get_regularization_loss()``, added with ``add_loss``"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    reg = tf.contrib.layers.l2_regularizer(1e-4)
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    c1 = tf.layers.max_pooling2d(tf.layers.conv2d(img, 32, 5, padding="same", activation=tf.nn.relu, kernel_regularizer=reg), 2, 2,
+                                 padding="same")
+    c2 = tf.layers.max_pooling2d(tf.layers.conv2d(c1, 64, 5, padding="same", activation=tf.nn.relu, kernel_regularizer=reg), 2, 2,
+                                 padding="same")
+    h = tf.layers.dense(tf.layers.flatten(c2), 1024, activation=tf.nn.relu, kernel_regularizer=reg)
+    logits = tf.layers.dense(h, 10, kernel_regularizer=reg)
+    tf.argmax(logits, 1, name="out")
+    loss = tf.losses.softmax_cross_entropy(y, logits, loss_collection=None) + tf.losses.get_regularization_loss()
+    tf.losses.add_loss(loss)
+    return loss
+
+
+def l2_autoencoder():
+    """autoencoder with ``1e-5 * add_n(l2_loss)`` of every trainable variable, biases included"""
+    x = tf.placeholder("float", shape=[None, 784], name="x")
+    e1 = tf.layers.dense(x, 256, activation=tf.nn.relu)
+    code = tf.layers.dense(e1, 128, activation=tf.nn.sigmoid, name="out")
+    d1 = tf.layers.dense(code, 256, activation=tf.nn.relu)
+    rec = tf.layers.dense(d1, 784, activation=tf.nn.sigmoid)
+    loss = (tf.losses.mean_squared_error(rec, x, loss_collection=None)
+            + 1e-5 * tf.add_n([tf.nn.l2_loss(v) for v in tf.trainable_variables()]))
+    tf.losses.add_loss(loss)
+    return loss
+
+
 def test_mlp(in_dim: int = 10):
     x = tf.placeholder(tf.float32, shape=[None, in_dim], name="x")
     h1 = tf.layers.dense(x, 12, activation=tf.nn.relu)
@@ -243,6 +292,9 @@ MODELS: Dict[str, Callable] = {
     "sparse_dnn": sparse_dnn,
     "onehot_cnn": onehot_cnn,
     "sparse_dnn100": sparse_dnn100,
+    "l2_dnn": l2_dnn,
+    "l2_cnn": l2_cnn,
+    "l2_autoencoder": l2_autoencoder,
 }
 
 

@@ -574,7 +574,22 @@ class DeviceWorker:
                 plan.run(self.stream.cuda_stream)
             self.stream.synchronize()
             total += float(bufs.loss_out[0]) * rows
-        return total / max(n, 1)
+        return total / max(n, 1) + self._penalty_value()
+
+    def _penalty_value(self) -> float:
+        """The loss's L2 weight penalties, sum of c * sum(v^2), over the bf16 kernel replica (its W^T copy, which is always
+        published) and the fp32 biases the forward plans read"""
+        lay, total = self.layout, 0.0
+        with torch.cuda.stream(self.stream):
+            wsrc = self._weight_src()
+            for name, c in self.plan.penalty.items():
+                seg = lay.by_name(name)
+                if seg.wt_off >= 0:
+                    v = wsrc[seg.wt_off:seg.wt_off + seg.cols * seg.wt_ld].view(seg.cols, seg.wt_ld)[:, :seg.rows]
+                else:
+                    v = self.vec_local[seg.offset - lay.vec_offset:seg.offset - lay.vec_offset + seg.rows * seg.cols]
+                total += c * float(v.double().square().sum())
+        return total
 
     def predict(self, X: np.ndarray, upto: int, post: Optional[str]) -> np.ndarray:
         n = X.shape[0]

@@ -115,6 +115,8 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
         return None
     if l.strides != (1, 1):
         return None
+    if lp.penalty.get(l.kernel) or (l.bias and lp.penalty.get(l.bias)):
+        return None                 # the direct kernels have no L2 penalty term: im2col + the penalised wgrad GEMM
     cin, cout = l.in_shape[2], l.out_shape[2]
     if l.ksize[0] * l.ksize[1] * cin > 64 or cout not in (8, 16, 32, 64) or l.act not in (None, "Relu", "Sigmoid", "Tanh"):
         return None
@@ -290,6 +292,23 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             side(lambda: plan.add_gemm(g, name))
         else:
             plan.add_gemm(g, name)
+
+    def penalty_args(l: Layer, ks) -> Dict[str, Any]:
+        """the L2 penalty terms of layer ``l``'s weight-gradient GEMM: 2c * W, 2c_b * b into the bias gradient, and the
+        loss term.  W is read from the replica's W^T copy, which every layer publishes (the forward GEMMs read it): there
+        the 32 rows a warp's lanes hold are contiguous, so each weight load is coalesced (the W copy would put them a row
+        pitch apart)."""
+        c = lp.penalty.get(l.kernel, 0.0)
+        cb = lp.penalty.get(l.bias, 0.0) if l.bias else 0.0
+        if not c and not cb:
+            return {}
+        d: Dict[str, Any] = dict(pen_loss=P(worker.loss_acc))
+        if c:
+            d.update(pen_w=P(wsrc) + ks.wt_off * 2, pen_ld=ks.wt_ld, pen_wt=1, pen_w2c=2.0 * c)
+        if cb:
+            bs = lay.by_name(l.bias)
+            d.update(pen_b=worker._bias_ptr(bs), pen_b2c=2.0 * cb, pen_db=P(worker.grads) + bs.offset * 4)
+        return d
 
     def wgrad_on_side(i: int) -> bool:
         """The first trainable layer's wgrad is the last GEMM of the step and the only one the push still waits for: it
@@ -475,6 +494,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 wd.update(worker.route_args(ks))          # push fused into the epilogue: tiles go to the owners' mailboxes
             else:
                 wd.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
+            wd.update(penalty_args(l, ks))
             wg = C.Gemm(wd)
             r["wgrad"] = wg
             emit(wg, f"wgrad{i}", on_side=wgrad_on_side(i))
@@ -554,6 +574,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 cw.update(worker.route_args(ks))          # red.add into the owners' mailboxes (appliers hand them back zeroed)
             else:
                 cw.update(out_f32=P(worker.grads) + ks.offset * 4, ld_f32=ks.cols)
+            cw.update(penalty_args(l, ks))
             wg = C.Gemm(cw)
             gemms.append(wg)
             r["wgrad"] = wg
@@ -573,7 +594,10 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             plan.add_col2im(P(dpatch), r["ldK"], B, h, w, cin, l.ksize[0], l.ksize[1], P(g_img), l.strides[0], l.strides[1], l.pads[0],
                             l.pads[2], l.out_shape[0], l.out_shape[1])
             continue
-    if sharded and with_push:
+    # a penalised wgrad adds to bias gradients (the 1-D tail), and any wgrad may be the first layer's, which runs beside
+    # the tail forwarding: a penalised sharded step forwards the tail after the join, in the post itself
+    tail_after_join = bool(lp.penalty)
+    if sharded and with_push and not tail_after_join:
         # forward the 1-D tail (bias gradients, all complete by now on the main branch) beside the last wgrad, so the post
         # after the join is a bare flag store: no store of its own to order, no system fence on the critical path
         plan.add_post_flags(worker._post_flags_args(loss_out, phase=1))
@@ -582,7 +606,7 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
     if with_push:
         extra = dict(done_dev=P(done_dev)) if done_dev is not None else {}
         if sharded:
-            plan.add_post_flags(dict(worker._post_flags_args(loss_out, phase=2), **extra))
+            plan.add_post_flags(dict(worker._post_flags_args(loss_out, phase=0 if tail_after_join else 2), **extra))
         elif worker.served:
             plan.add_post(dict(worker._post_args(loss_out), **extra), P(worker.sync_push), 0)
         else:
