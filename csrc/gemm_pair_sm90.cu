@@ -122,30 +122,17 @@ __device__ __forceinline__ void pair_cta(const CUtensorMap& tmA, const CUtensorM
   trace.end(KID_GEMM);
 }
 
+template <bool EXT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
 sf_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const SfGemmEpilogue ep,
                     int M, int N, int K, int tiles_m, int tiles_n, int group_m) {
-  pair_cta<false>(tmA, tmB, ep, M, N, K, tiles_m, tiles_n, group_m);
-}
-
-// the twin that carries the extended activations (a large layer with ELU, SELU, ...; see sf_gemm_ext_kernel)
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-sf_gemm_pair_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const SfGemmEpilogue ep,
-                        int M, int N, int K, int tiles_m, int tiles_n, int group_m) {
-  pair_cta<true>(tmA, tmB, ep, M, N, K, tiles_m, tiles_n, group_m);
+  pair_cta<EXT>(tmA, tmB, ep, M, N, K, tiles_m, tiles_n, group_m);
 }
 
 }  // namespace sf
 
-template <bool EXT>
-static int pair_launch(const SfGemm* g, cudaStream_t st) {
-  const auto kernel = EXT ? sf::sf_gemm_pair_ext_kernel : sf::sf_gemm_pair_kernel;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sf::kPairSmemBytes);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    attr_set = true;
-  }
+extern "C" int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st) {
+  const bool ext = g->ep.act >= SF_ACT_ELU || g->ep.aux_act >= SF_ACT_ELU;
   const int tiles_m = (g->M + 2 * sf::kBM - 1) / (2 * sf::kBM);
   const int tiles_n = (g->N + sf::kPairBN - 1) / sf::kPairBN;
   const int tiles = tiles_m * tiles_n;
@@ -156,20 +143,26 @@ static int pair_launch(const SfGemm* g, cudaStream_t st) {
   static const int env_group = [] { const char* v = getenv("SPARKFLOW_PAIR_GROUP_M"); return v ? atoi(v) : 0; }();
   int group_m = env_group > 0 ? env_group : 8;
   if (group_m > tiles_m) group_m = tiles_m;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(sf::kGemmThreads);
-  cfg.dynamicSmemBytes = sf::kPairSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = sf::pdl_enabled() ? 1 : 0;
-  return static_cast<int>(cudaLaunchKernelEx(&cfg, kernel, g->tmA, g->tmB, g->ep, g->M, g->N, g->K, tiles_m, tiles_n, group_m));
+  return static_cast<int>(sf::launch(ext ? sf::sf_gemm_pair_kernel<true> : sf::sf_gemm_pair_kernel<false>, dim3(2 * pairs),
+                                     dim3(sf::kGemmThreads), sf::kPairSmemBytes, st, g->tmA, g->tmB, g->ep, g->M, g->N, g->K, tiles_m,
+                                     tiles_n, group_m));
 }
 
-extern "C" int sf_gemm_pair_launch(const SfGemm* g, cudaStream_t st) {
-  const bool ext = g->ep.act >= SF_ACT_ELU || g->ep.aux_act >= SF_ACT_ELU;
-  return ext ? pair_launch<true>(g, st) : pair_launch<false>(g, st);
+// Sets a GEMM kernel's opt-in shared-memory size and forces its module load
+template <typename Fn>
+static int preload_gemm(Fn* fn, int smem) {
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, fn);
+  return static_cast<int>(e);
+}
+
+// Every GEMM kernel instance: the one-CTA kernels of kGemmKernels (gemm_sm90.cu) and both pair instances.  Nothing else
+// grants a GEMM its shared memory (every instance needs more than the default 48 KB), so an instance missing here fails
+// its first launch.  Called by sf_preload_kernels, once per device.
+static int sf_gemm_preload() {
+  for (const sf::GemmKernel& k : sf::kGemmKernels)
+    if (const int rc = preload_gemm(k.fn, k.smem)) return rc;
+  if (const int rc = preload_gemm(sf::sf_gemm_pair_kernel<false>, sf::kPairSmemBytes)) return rc;
+  return preload_gemm(sf::sf_gemm_pair_kernel<true>, sf::kPairSmemBytes);
 }

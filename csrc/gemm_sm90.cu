@@ -16,10 +16,11 @@
 //   * column sums (bias gradient) via an in-register transpose-reduce + one red per column,
 //   * fp32 store or atomic accumulate (split-K / straight into the flat gradient buffer that the
 //     push kernel consumes).
-// The generic kernel (sf_gemm_kernel) tests each of these at run time.  The training GEMMs run specialized variants
-// (sf_gemm_epi_kernel, one per SfEpi kind, sf_gemm_sigmoid_loss_kernel and sf_gemm_sparse_loss_kernel) that contain only their own epilogue code, a
-// fifth to a half of the generic kernel's; the DGRAD / loss variants also fetch their act'(aux) / label rows before the
-// main loop.
+// One kernel template, sf_gemm_kernel<BN, MN, EPI, EXT, PEN>, is instantiated once per feature set in kGemmKernels, the
+// table that sf_gemm_prepare resolves a GEMM to and that sf_gemm_preload (gemm_pair_sm90.cu) loads.  The generic epilogue
+// tests each of the features above at run time.  The training GEMMs run specialized variants (one per other SfEpi kind)
+// that contain only their own epilogue code, a fifth to a half of the generic kernel's; the DGRAD / loss variants also
+// fetch their act'(aux) / label rows before the main loop.
 //
 // The B operand may live in *peer* GPU memory: the tensor map simply carries the peer-mapped
 // address, and the TMA engine pulls weight tiles over NVLink while the MMA pipeline runs
@@ -108,8 +109,8 @@ __device__ __forceinline__ void act_ext_bwd32(float (&f)[32], const float (&a)[3
   }
 }
 
-// whole-chunk forms: ONE (uniform) branch on the activation kind instead of one per element.  EXT: the kernel is a twin
-// that also carries the extended set (act >= SF_ACT_ELU); without it these are the ReLU / sigmoid / tanh code alone.
+// whole-chunk forms: ONE (uniform) branch on the activation kind instead of one per element.  EXT: the kernel instance
+// also carries the extended set (act >= SF_ACT_ELU); without it these are the ReLU / sigmoid / tanh code alone.
 template <bool EXT>
 __device__ __forceinline__ void act_fwd32(float (&f)[32], int act, float alpha) {
   if (EXT && act >= SF_ACT_ELU) {
@@ -192,8 +193,8 @@ struct EpiFeatures {
 
 // One 32-column chunk of a thread's output row: everything between the accumulator (v, already in registers) and
 // global memory.  `aux_pref` / `tgt_pref` are the act'(a) operand / label row of this chunk when the caller fetched
-// them before the accumulator wait (nullptr: read here).  EXT: the extended activations (twin kernels only).  PEN: the L2
-// weight penalty (penalty kernels only); the chunk's sum of W^2 is added to *pen_sq.
+// them before the accumulator wait (nullptr: read here).  EXT: the extended activations (EXT instances only).  PEN: the L2
+// weight penalty (PEN instances only); the chunk's sum of W^2 is added to *pen_sq.
 template <int EPI, bool EXT, bool PEN = false>
 __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32_t (&v)[32], const float* s_bias32, int row, bool row_ok,
                                           int col0, int M, int N, int lane, const uint4* aux_pref, const float* tgt_pref,
@@ -563,8 +564,8 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 // MN: both operands MN-major (D = a^T . b with a [K, M], b [K, N] row-major): the stage buffers have the same size, but a
 // stage is filled with {64 MN elements, 64 K rows} boxes and described to the tensor core as MN-major.
 // EPI: epilogue feature set (SfEpi); only the generic kernel handles the fused read-your-writes wait.  EXT: the extended
-// activations are compiled in (the twin kernels below).  PEN: the L2 weight penalty (the penalty kernels below).
-template <int BN, bool MN, int EPI, bool EXT = false, bool PEN = false>
+// activations are compiled in.  PEN: the L2 weight penalty is compiled in.  See kGemmKernels for which sets exist.
+template <int BN, bool MN, int EPI, bool EXT, bool PEN>
 __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorMap& tmB, const SfGemmEpilogue& ep, int M, int N,
                                          int K, int kblocks_per_split) {
   static_assert(!MN || BN % 64 == 0, "MN-major B needs whole 64-element swizzle atoms");
@@ -702,75 +703,79 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
   trace.end(KID_GEMM);
 }
 
-// The generic kernel: every epilogue feature, each behind a runtime test.
-template <int BN, bool MN = false>
+// The one-CTA GEMM kernel, instantiated only through kGemmKernels.
+template <int BN, bool MN, int EPI, bool EXT, bool PEN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 sf_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  gemm_cta<BN, MN, SF_EPI_GENERIC>(tmA, tmB, ep, M, N, K, kblocks_per_split);
+  gemm_cta<BN, MN, EPI, EXT, PEN>(tmA, tmB, ep, M, N, K, kblocks_per_split);
 }
 
-// A specialized epilogue variant (EPI != SF_EPI_GENERIC): a fraction of the generic kernel's code, which matters because
-// the epilogue runs once per launch on a cold instruction cache.
-template <int BN, bool MN, int EPI>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  static_assert(EPI != SF_EPI_GENERIC, "the generic epilogue is sf_gemm_kernel");
-  gemm_cta<BN, MN, EPI>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
+using GemmKernelFn = void (*)(CUtensorMap, CUtensorMap, SfGemmEpilogue, int, int, int, int);
+struct GemmKernel {
+  int bn;
+  bool mn;
+  int epi;
+  bool ext, pen;
+  GemmKernelFn fn;
+  int smem;                      // dynamic shared memory bytes (opt-in: more than 48 KB for every instance)
+};
+#define SF_GEMM(BN, MN, EPI, EXT, PEN) {BN, MN, EPI, EXT, PEN, sf_gemm_kernel<BN, MN, EPI, EXT, PEN>, GemmSmem<BN>::kBytes}
 
-// The sigmoid cross-entropy head (SF_EPI_SIGMOID_LOSS, K-major) runs only here: as a runtime branch of the LOSS variant
-// it raised that variant's register count, and in the generic kernel it added a quarter to the code every generic GEMM
-// of the training step fetches.  It carries what a loss GEMM may need beyond the LOSS variant: the transposed dz of the
-// K-major weight-gradient path and the read-your-writes wait of a network whose only dense layer is the loss layer.
-template <int BN>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_sigmoid_loss_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                            const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  gemm_cta<BN, false, SF_EPI_SIGMOID_LOSS>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
-
-// The sparse softmax cross-entropy head (SF_EPI_SPARSE_LOSS, K-major, BN 32: the row fits one chunk) runs only here, so
-// that the LOSS variant and the generic kernel keep their code; it carries the same extras as the sigmoid kernel.
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_sparse_loss_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                           const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  gemm_cta<32, false, SF_EPI_SPARSE_LOSS>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
-
-// Twins of the generic kernel (K-major) and of the FWD / LOSS / DGRAD variants that also carry the extended activations
-// (SfAct 4-9): their code would otherwise sit in every ReLU / sigmoid / tanh GEMM's epilogue, which is instruction-fetch
-// bound.  sf_gemm_launch picks a twin exactly when ep.act or ep.aux_act is one of them.
-template <int BN>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  gemm_cta<BN, false, SF_EPI_GENERIC, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
-template <int BN, int EPI>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_epi_ext_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  static_assert(EPI == SF_EPI_FWD || EPI == SF_EPI_LOSS || EPI == SF_EPI_DGRAD, "only these variants apply an activation");
-  gemm_cta<BN, false, EPI, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
-
-// Penalty kernels: the weight-gradient GEMMs of a layer with an L2 weight penalty (SfGemmEpilogue.pen_*).  The generic
-// one-CTA kernel (K-major wgrads, split-K conv wgrads, route mode, accumulate) and the MN-major WGRAD variant, each with the
-// penalty compiled in, so that no other GEMM carries its code.
-template <int BN, bool MN>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_pen_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  gemm_cta<BN, MN, SF_EPI_GENERIC, false, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
-template <int BN>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-sf_gemm_wgrad_pen_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                         const SfGemmEpilogue ep, int M, int N, int K, int kblocks_per_split) {
-  gemm_cta<BN, true, SF_EPI_WGRAD, false, true>(tmA, tmB, ep, M, N, K, kblocks_per_split);
-}
+// Every instance of sf_gemm_kernel: (BN, MN, EPI, EXT, PEN).  A feature set gets an instance of its own rather than a
+// runtime branch in another one because the epilogue is instruction-fetch bound (it runs once per launch on a cold
+// instruction cache): code a GEMM does not need still costs it fetches, and a branch can raise the register count of
+// every GEMM that carries it.
+//   * the generic epilogue: every feature behind a runtime test;
+//   * the specialized variants (FWD, LOSS, DGRAD, WGRAD): a fraction of the generic kernel's code, at the tile shapes the
+//     dense training plans use (pick_epi);
+//   * the loss heads SIGMOID_LOSS and SPARSE_LOSS (K-major; SPARSE_LOSS at BN 32, where its row fits one chunk) exist
+//     only in their own variants: as a runtime branch of the LOSS variant the sigmoid head raised its register count, and
+//     in the generic kernel it added a quarter to the code every generic GEMM of the training step fetches.  They carry
+//     what a loss GEMM may need beyond the LOSS variant: the transposed dz of the K-major weight-gradient path and the
+//     read-your-writes wait of a network whose only dense layer is the loss layer;
+//   * EXT: the extended activations (SfAct 4-9) on the K-major generic kernel and the FWD / LOSS / DGRAD variants, chosen
+//     exactly when ep.act or ep.aux_act is one of them, so that the ReLU / sigmoid / tanh GEMMs keep their code;
+//   * PEN: the L2 weight penalty (SfGemmEpilogue.pen_*) on the weight-gradient GEMMs of a penalised layer: the generic
+//     kernel (K-major wgrads, split-K conv wgrads, route mode, accumulate) and the MN-major WGRAD variant.
+static const GemmKernel kGemmKernels[] = {
+    SF_GEMM(32, false, SF_EPI_GENERIC, false, false),
+    SF_GEMM(64, false, SF_EPI_GENERIC, false, false),
+    SF_GEMM(128, false, SF_EPI_GENERIC, false, false),
+    SF_GEMM(256, false, SF_EPI_GENERIC, false, false),
+    SF_GEMM(64, true, SF_EPI_GENERIC, false, false),
+    SF_GEMM(128, true, SF_EPI_GENERIC, false, false),
+    SF_GEMM(32, false, SF_EPI_FWD, false, false),
+    SF_GEMM(64, false, SF_EPI_FWD, false, false),
+    SF_GEMM(32, false, SF_EPI_LOSS, false, false),
+    SF_GEMM(64, false, SF_EPI_LOSS, false, false),
+    SF_GEMM(32, false, SF_EPI_DGRAD, false, false),
+    SF_GEMM(64, false, SF_EPI_DGRAD, false, false),
+    SF_GEMM(64, true, SF_EPI_WGRAD, false, false),
+    SF_GEMM(128, true, SF_EPI_WGRAD, false, false),
+    SF_GEMM(32, false, SF_EPI_SIGMOID_LOSS, false, false),
+    SF_GEMM(64, false, SF_EPI_SIGMOID_LOSS, false, false),
+    SF_GEMM(32, false, SF_EPI_SPARSE_LOSS, false, false),
+    SF_GEMM(32, false, SF_EPI_GENERIC, true, false),
+    SF_GEMM(64, false, SF_EPI_GENERIC, true, false),
+    SF_GEMM(128, false, SF_EPI_GENERIC, true, false),
+    SF_GEMM(256, false, SF_EPI_GENERIC, true, false),
+    SF_GEMM(32, false, SF_EPI_FWD, true, false),
+    SF_GEMM(64, false, SF_EPI_FWD, true, false),
+    SF_GEMM(32, false, SF_EPI_LOSS, true, false),
+    SF_GEMM(64, false, SF_EPI_LOSS, true, false),
+    SF_GEMM(32, false, SF_EPI_DGRAD, true, false),
+    SF_GEMM(64, false, SF_EPI_DGRAD, true, false),
+    SF_GEMM(32, false, SF_EPI_GENERIC, false, true),
+    SF_GEMM(64, false, SF_EPI_GENERIC, false, true),
+    SF_GEMM(128, false, SF_EPI_GENERIC, false, true),
+    SF_GEMM(256, false, SF_EPI_GENERIC, false, true),
+    SF_GEMM(64, true, SF_EPI_GENERIC, false, true),
+    SF_GEMM(128, true, SF_EPI_GENERIC, false, true),
+    SF_GEMM(64, true, SF_EPI_WGRAD, false, true),
+    SF_GEMM(128, true, SF_EPI_WGRAD, false, true),
+};
+#undef SF_GEMM
 
 // ---------------------------------------------------------------------------
 // Host side
@@ -865,10 +870,19 @@ static int pick_epi(const SfGemm* g) {
   return e.colsum == nullptr ? SF_EPI_FWD : SF_EPI_GENERIC;
 }
 
-// the epilogue applies (or differentiates) one of the extended activations: the GEMM runs on a twin kernel
+// the epilogue applies (or differentiates) one of the extended activations: the GEMM runs on an EXT instance
 static bool uses_ext_act(const SfGemmEpilogue& e) { return e.act >= SF_ACT_ELU || e.aux_act >= SF_ACT_ELU; }
-// the GEMM carries an L2 weight penalty: it runs on a penalty kernel
+// the GEMM carries an L2 weight penalty: it runs on a PEN instance
 static bool has_penalty(const SfGemmEpilogue& e) { return e.pen_w != nullptr || e.pen_b != nullptr; }
+
+// index of the kGemmKernels entry compiled for this feature set, or -1: there is no such instance
+static int find_gemm_kernel(int bn, bool mn, int epi, bool ext, bool pen) {
+  for (int i = 0; i < static_cast<int>(sizeof(sf::kGemmKernels) / sizeof(sf::kGemmKernels[0])); ++i) {
+    const sf::GemmKernel& k = sf::kGemmKernels[i];
+    if (k.bn == bn && k.mn == mn && k.epi == epi && k.ext == ext && k.pen == pen) return i;
+  }
+  return -1;
+}
 
 extern "C" int sf_gemm_prepare(SfGemm* g) {
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return -2;
@@ -937,119 +951,19 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   g->epi = g->epi == SF_EPI_GENERIC ? SF_EPI_GENERIC : pick_epi(g);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->epi != SF_EPI_SIGMOID_LOSS) return -5;
   if (g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT && g->epi != SF_EPI_SPARSE_LOSS) return -5;
+  if (!g->pair) {
+    g->kernel = find_gemm_kernel(g->bn, g->mn_major != 0, g->epi, uses_ext_act(g->ep), has_penalty(g->ep));
+    if (g->kernel < 0) return -3;
+  }
   return 0;
-}
-
-template <int BN, bool MN = false, int EPI = SF_EPI_GENERIC, bool EXT = false, bool PEN = false>
-static cudaError_t launch_bn(const SfGemm* g, cudaStream_t st) {
-  using S = sf::GemmSmem<BN>;
-  auto kernel = [] {
-    if constexpr (PEN && EPI == SF_EPI_WGRAD) return sf::sf_gemm_wgrad_pen_kernel<BN>;
-    else if constexpr (PEN) return sf::sf_gemm_pen_kernel<BN, MN>;
-    else if constexpr (EXT && EPI == SF_EPI_GENERIC) return sf::sf_gemm_ext_kernel<BN>;
-    else if constexpr (EXT) return sf::sf_gemm_epi_ext_kernel<BN, EPI>;
-    else if constexpr (EPI == SF_EPI_GENERIC) return sf::sf_gemm_kernel<BN, MN>;
-    else if constexpr (EPI == SF_EPI_SIGMOID_LOSS) return sf::sf_gemm_sigmoid_loss_kernel<BN>;
-    else if constexpr (EPI == SF_EPI_SPARSE_LOSS) return sf::sf_gemm_sparse_loss_kernel;
-    else return sf::sf_gemm_epi_kernel<BN, MN, EPI>;
-  }();
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kBytes);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  dim3 grid((g->N + BN - 1) / BN, (g->M + sf::kBM - 1) / sf::kBM, g->split_k);
-  return sf::launch(kernel, grid, dim3(sf::kGemmThreads), S::kBytes, st, g->tmA, g->tmB, g->ep,
-                    g->M, g->N, g->K, g->kblocks_per_split);
-}
-
-// K-major epilogue variants exist at BN 32 and 64 (pick_epi)
-template <int EPI, bool EXT = false>
-static cudaError_t launch_kmajor_variant(const SfGemm* g, cudaStream_t st) {
-  return g->bn == 32 ? launch_bn<32, false, EPI, EXT>(g, st) : launch_bn<64, false, EPI, EXT>(g, st);
-}
-
-// the twins of the extended activations (K-major only, see sf_gemm_prepare)
-static int launch_ext(const SfGemm* g, cudaStream_t st) {
-  cudaError_t e;
-  switch (g->epi) {
-    case SF_EPI_GENERIC: break;
-    case SF_EPI_FWD: return static_cast<int>(launch_kmajor_variant<SF_EPI_FWD, true>(g, st));
-    case SF_EPI_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_LOSS, true>(g, st));
-    case SF_EPI_DGRAD: return static_cast<int>(launch_kmajor_variant<SF_EPI_DGRAD, true>(g, st));
-    default: return -3;
-  }
-  if (g->mn_major) return -3;
-  switch (g->bn) {
-    case 32: e = launch_bn<32, false, SF_EPI_GENERIC, true>(g, st); break;
-    case 64: e = launch_bn<64, false, SF_EPI_GENERIC, true>(g, st); break;
-    case 128: e = launch_bn<128, false, SF_EPI_GENERIC, true>(g, st); break;
-    case 256: e = launch_bn<256, false, SF_EPI_GENERIC, true>(g, st); break;
-    default: return -3;
-  }
-  return static_cast<int>(e);
-}
-
-// the penalty kernels: the MN-major WGRAD variant at BN 64 / 128, the generic kernel at every tile width
-static int launch_pen(const SfGemm* g, cudaStream_t st) {
-  cudaError_t e;
-  if (g->epi == SF_EPI_WGRAD) {
-    e = g->bn == 64 ? launch_bn<64, true, SF_EPI_WGRAD, false, true>(g, st) : launch_bn<128, true, SF_EPI_WGRAD, false, true>(g, st);
-    return static_cast<int>(e);
-  }
-  if (g->epi != SF_EPI_GENERIC) return -3;
-  if (g->mn_major) {
-    switch (g->bn) {
-      case 64: e = launch_bn<64, true, SF_EPI_GENERIC, false, true>(g, st); break;
-      case 128: e = launch_bn<128, true, SF_EPI_GENERIC, false, true>(g, st); break;
-      default: return -3;
-    }
-    return static_cast<int>(e);
-  }
-  switch (g->bn) {
-    case 32: e = launch_bn<32, false, SF_EPI_GENERIC, false, true>(g, st); break;
-    case 64: e = launch_bn<64, false, SF_EPI_GENERIC, false, true>(g, st); break;
-    case 128: e = launch_bn<128, false, SF_EPI_GENERIC, false, true>(g, st); break;
-    case 256: e = launch_bn<256, false, SF_EPI_GENERIC, false, true>(g, st); break;
-    default: return -3;
-  }
-  return static_cast<int>(e);
 }
 
 extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
   if (g->pair) return sf_gemm_pair_launch(g, st);
-  if (has_penalty(g->ep)) return launch_pen(g, st);
-  if (uses_ext_act(g->ep)) return launch_ext(g, st);
-  cudaError_t e;
-  switch (g->epi) {
-    case SF_EPI_GENERIC: break;
-    case SF_EPI_FWD: return static_cast<int>(launch_kmajor_variant<SF_EPI_FWD>(g, st));
-    case SF_EPI_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_LOSS>(g, st));
-    case SF_EPI_DGRAD: return static_cast<int>(launch_kmajor_variant<SF_EPI_DGRAD>(g, st));
-    case SF_EPI_SIGMOID_LOSS: return static_cast<int>(launch_kmajor_variant<SF_EPI_SIGMOID_LOSS>(g, st));
-    case SF_EPI_SPARSE_LOSS: return static_cast<int>(launch_bn<32, false, SF_EPI_SPARSE_LOSS>(g, st));
-    case SF_EPI_WGRAD:
-      e = g->bn == 64 ? launch_bn<64, true, SF_EPI_WGRAD>(g, st) : launch_bn<128, true, SF_EPI_WGRAD>(g, st);
-      return static_cast<int>(e);
-    default: return -3;
-  }
-  if (g->mn_major) {
-    switch (g->bn) {
-      case 64: e = launch_bn<64, true>(g, st); break;
-      case 128: e = launch_bn<128, true>(g, st); break;
-      default: return -3;
-    }
-    return static_cast<int>(e);
-  }
-  switch (g->bn) {
-    case 32: e = launch_bn<32>(g, st); break;
-    case 64: e = launch_bn<64>(g, st); break;
-    case 128: e = launch_bn<128>(g, st); break;
-    case 256: e = launch_bn<256>(g, st); break;
-    default: return -3;
-  }
-  return static_cast<int>(e);
+  const sf::GemmKernel& k = sf::kGemmKernels[g->kernel];
+  const dim3 grid((g->N + k.bn - 1) / k.bn, (g->M + sf::kBM - 1) / sf::kBM, g->split_k);
+  return static_cast<int>(sf::launch(k.fn, grid, dim3(sf::kGemmThreads), k.smem, st, g->tmA, g->tmB, g->ep, g->M, g->N, g->K,
+                                     g->kblocks_per_split));
 }
 
 extern "C" void sf_set_pdl(int enabled) { sf::pdl_enabled() = enabled ? 1 : 0; }

@@ -7,7 +7,8 @@
 
 // 4-9: the extended set.  Each derivative is a function of the activation's output a = act(z), which is all the backward
 // pass stores; LeakyRelu takes its slope from the epilogue's act_alpha / aux_act_alpha (the kernels' alpha argument).  The
-// GEMMs run them on twins of their kernels (gemm_sm90.cu), so the kernels of ReLU / sigmoid / tanh models are unchanged.
+// GEMMs run them on kernel instances of their own (EXT, gemm_sm90.cu), so the kernels of ReLU / sigmoid / tanh models are
+// unchanged.
 enum SfAct {
   SF_ACT_NONE = 0,
   SF_ACT_RELU = 1,
@@ -106,7 +107,7 @@ struct SfGemmEpilogue {
   // slope of a leaky ReLU `act` / `aux_act` (SF_ACT_LEAKY_RELU); appended last so every field above keeps its offset
   float act_alpha, aux_act_alpha;
   // L2 weight penalty c * sum(W^2) + c_b * sum(b^2) of the layer whose weight gradient this GEMM computes (appended last,
-  // like act_alpha).  Set only on weight-gradient GEMMs; they then run the penalty kernels (sf_gemm_prepare).
+  // like act_alpha).  Set only on weight-gradient GEMMs; they then run the PEN kernel instances (sf_gemm_prepare).
   //   weight: K split 0 adds pen_w2c * W to every fp32 output element (before the store, atomic add or routed red), W
   //           read from the bf16 replica the step computed with: W [M, pen_ld] or, pen_wt = 1, W^T [N, pen_ld]
   //   bias:   the CTAs of row tile 0, split 0 atomically add pen_b2c * b[n] into pen_db[n]
@@ -152,6 +153,7 @@ struct SfGemm {
   int pair_ctas;                  // CTAs of the persistent cluster-pair kernel (0 = one per SM)
   int epi;                        // in: -1 = auto, SF_EPI_GENERIC = force the generic kernel; out: the SfEpi variant launched
   SfGemmEpilogue ep;
+  int kernel;                     // filled by sf_gemm_prepare: the one-CTA kernel instance launched (kGemmKernels, gemm_sm90.cu)
 };
 
 #ifdef __cplusplus

@@ -8,11 +8,7 @@ test_step_gradients._forward (whose helpers it reuses); it differs in taking act
 (SELU and leaky ReLU at 0, ReLU6 at 0 and 6) on the branch the step took, and in carrying the step's stored
 activations forward where they are a rounding of its own, both read from the step's stored output.
 """
-import os
-import re
-import shutil
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -26,10 +22,8 @@ from sparkflow_b200.graph_utils import build_graph
 from sparkflow_b200.models import zoo
 from sparkflow_b200.models.compiler import ACT_IDS, UnsupportedGraph, compile_graph
 from sparkflow_b200.parallel.plan_builder import act_arg, check_grammar, fused_first_conv
+from kernel_usage import gemm_instances, needs_binary_utils, res_usage
 from test_step_gradients import _assert_grads, _bf16, _conv, _grads, _pool_argmax, _pool_gather, _rejects
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "sparkflow_b200", "_C.so")
 
 SELU = (1.0507009873554805, 1.6732632423543772)       # (lambda, alpha)
 NEW_ACTS = ("Elu", "Selu", "Softplus", "Softsign", "LeakyRelu", "Relu6")
@@ -570,20 +564,19 @@ def test_mlp_scale_exercises_relu6_saturation():
 # ------------------------------------------------------------------------------------------------------------------
 # build artifacts
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not os.path.exists(SO) or shutil.which("cuobjdump") is None or shutil.which("c++filt") is None,
-                    reason="needs the built extension and the CUDA binary utilities")
-def test_new_kernels_have_no_stack_frame():
-    txt = subprocess.run(["cuobjdump", "-res-usage", SO], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, check=True).stdout
-    names = re.findall(r"Function (\S+):\n\s+REG:(\d+) STACK:(\d+)", txt)
-    dem = subprocess.run(["c++filt"], input="\n".join(n for n, _, _ in names), stdout=subprocess.PIPE, text=True, check=True).stdout.splitlines()
-    use = {re.sub(r"\(.*", "", d).replace("void ", ""): (int(r), int(s)) for d, (_, r, s) in zip(dem, names)}
-    gemms = [f"sf::sf_gemm_ext_kernel<{bn}>" for bn in (32, 64, 128, 256)] + ["sf::sf_gemm_pair_ext_kernel"]
-    gemms += [f"sf::sf_gemm_epi_ext_kernel<{bn}, {epi}>" for bn in (32, 64) for epi in (1, 2, 3)]
+@needs_binary_utils
+def test_ext_kernel_instances_have_no_stack_frame():
+    use = res_usage()
+    # the EXT instances of the GEMM kernels: the K-major generic kernel, the FWD / LOSS / DGRAD variants, the pair kernel
+    gemms = [f"sf::sf_gemm_kernel<{bn}, false, 0, true, false>" for bn in (32, 64, 128, 256)] + ["sf::sf_gemm_pair_kernel<true>"]
+    gemms += [f"sf::sf_gemm_kernel<{bn}, false, {epi}, true, false>" for bn in (32, 64) for epi in (1, 2, 3)]
     others = ["sf::maxpool_bwd_ext_kernel", "sf::maxpool_gen_bwd_ext_kernel", "sf::act_bwd_bias_ext_kernel", "sf::mse_ext_loss_kernel"]
     missing = [k for k in gemms + others if k not in use]
     assert not missing, (missing, sorted(use))
     spilled = {k: use[k] for k in gemms + others if use[k][1] != 0}
     assert not spilled, f"kernels with a local-memory stack frame (REG, STACK): {spilled}"
-    # the twins run under the GEMMs' launch bounds (384 threads, one CTA per SM): no more registers than the kernels they twin
-    bound = max(r for k, (r, _) in use.items() if k.startswith(("sf::sf_gemm_kernel<", "sf::sf_gemm_pair_kernel", "sf::sf_gemm_epi_kernel<")))
+    # the EXT instances run under the GEMMs' launch bounds (384 threads, one CTA per SM): no more registers than the
+    # instances without the extended activations (EXT = false, PEN = false)
+    bound = max([r for (_, _, _, ext, pen), (r, _) in gemm_instances(use).items() if not ext and not pen] +
+                [use["sf::sf_gemm_pair_kernel<false>"][0]])
     assert all(use[k][0] <= bound for k in gemms), {k: use[k] for k in gemms}

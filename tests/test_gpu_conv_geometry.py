@@ -1,10 +1,7 @@
 """SAME-padded / strided convolutions and general max-pools on the native path: every new or generalized kernel against
 PyTorch fp32, the compiled training step of the new zoo CNNs against the interpreter oracle, sessions and inference on
 them, and the unchanged kernel sequence of the VALID stride-1 ``cnn`` model."""
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,6 +10,7 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
+from kernel_usage import needs_binary_utils, res_usage
 from sparkflow_b200.graph.executor import GraphProgram
 from sparkflow_b200.graph.ir import GraphIR
 from sparkflow_b200.models import zoo
@@ -200,16 +198,9 @@ def test_conv_first_fused_same_padding(C, n, h, w, cin, kh, kw, cout, act):
     assert torch.allclose(db, bt.grad, rtol=3e-2, atol=3e-2 * max(1.0, bt.grad.abs().max().item()))
 
 
-SO = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "sparkflow_b200", "_C.so")
-
-
-@pytest.mark.skipif(not os.path.exists(SO) or shutil.which("cuobjdump") is None or shutil.which("c++filt") is None,
-                    reason="needs the built extension and the CUDA binary utilities")
+@needs_binary_utils
 def test_new_and_generalized_kernels_have_no_stack_frame():
-    txt = subprocess.run(["cuobjdump", "-res-usage", SO], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, check=True).stdout
-    names = re.findall(r"Function (\S+):\n\s+REG:(\d+) STACK:(\d+)", txt)
-    dem = subprocess.run(["c++filt"], input="\n".join(n for n, _, _ in names), stdout=subprocess.PIPE, text=True, check=True).stdout.splitlines()
-    use = {re.sub(r"\(.*", "", d).replace("void ", ""): int(s) for d, (_, _, s) in zip(dem, names)}
+    use = {k: s for k, (_, s) in res_usage().items()}
     want = [k for k in use if re.match(r"sf::(maxpool_gen_fwd_kernel|maxpool_gen_bwd_kernel|act_bwd_bias_kernel|im2col_kernel|im2col_vec8_kernel|"
                                         r"col2im_kernel|col2im_vec8_kernel|conv_first_fwd_kernel|conv_first_wgrad_kernel)", k)]
     assert len(want) >= 15, sorted(use)[:10]

@@ -1,21 +1,17 @@
 """Specialized GEMM epilogue variants: each computes exactly what the generic kernel computes for the same GEMM, the
 dense training plans select them, and none of them keeps a stack frame."""
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
 from sparkflow_b200.ops import native
+from kernel_usage import gemm_instances, needs_binary_utils, res_usage
 from sparkflow_b200.ops.layout import round_up
 
 # SfEpi (csrc/sf_api.h)
 GENERIC, FWD, LOSS, DGRAD, WGRAD = 0, 1, 2, 3, 4
 RELU, SIGMOID = 1, 2
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "sparkflow_b200", "_C.so")
 
 
 def _bf16(rows, cols, ld, g, scale=0.5, fn=None):
@@ -176,13 +172,9 @@ def test_dense_training_plan_selects_a_variant_for_every_gemm(model):
     master.close()
 
 
-@pytest.mark.skipif(not os.path.exists(SO) or shutil.which("cuobjdump") is None or shutil.which("c++filt") is None,
-                    reason="needs the built extension and the CUDA binary utilities")
-def test_epilogue_variants_have_no_stack_frame():
-    txt = subprocess.run(["cuobjdump", "-res-usage", SO], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, check=True).stdout
-    names = re.findall(r"Function (\S+):\n\s+REG:(\d+) STACK:(\d+)", txt)
-    dem = subprocess.run(["c++filt"], input="\n".join(n for n, _, _ in names), stdout=subprocess.PIPE, text=True, check=True).stdout.splitlines()
-    use = {re.sub(r"\(.*", "", k).replace("void ", ""): (int(r), int(s)) for k, (_, r, s) in zip(dem, names)}
-    variants = {k: v for k, v in use.items() if k.startswith("sf::sf_gemm_epi_kernel<")}
+@needs_binary_utils
+def test_epilogue_variant_instances_have_no_stack_frame():
+    # the FWD / LOSS / DGRAD / WGRAD instances without the extended activations or the penalty
+    variants = {k: v for k, v in gemm_instances(res_usage()).items() if FWD <= k[2] <= WGRAD and not k[3] and not k[4]}
     assert len(variants) == 8, sorted(variants)
     assert all(s == 0 for _, s in variants.values()), variants

@@ -6,10 +6,6 @@ tolerances of the GPU test reject plausible gradient bugs; and the new kernels k
 The oracle and graph helpers here are shared with tests/test_gpu_sigmoid_xent.py.
 """
 import dataclasses
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -24,10 +20,8 @@ from sparkflow_b200.graph_utils import build_graph
 from sparkflow_b200.models import zoo
 from sparkflow_b200.models.compiler import UnsupportedGraph, compile_graph
 from sparkflow_b200.parallel.plan_builder import loss_mode
+from kernel_usage import needs_binary_utils, res_usage
 from test_step_gradients import _assert_grads, _forward, _grads, _rejects
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "sparkflow_b200", "_C.so")
 
 
 def _tf1_sigmoid_xent(labels, logits):
@@ -282,17 +276,12 @@ def test_tolerances_reject_plausible_loss_bugs(name, B):
 # ------------------------------------------------------------------------------------------------------------------
 # build artifacts
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not os.path.exists(SO) or shutil.which("cuobjdump") is None or shutil.which("c++filt") is None,
-                    reason="needs the built extension and the CUDA binary utilities")
-def test_sigmoid_xent_kernels_have_no_stack_frame():
-    """the stand-alone kernel and the SIGMOID_LOSS GEMM variant (SfEpi 5, sf_gemm_sigmoid_loss_kernel), and the LOSS
-    variants beside them"""
-    txt = subprocess.run(["cuobjdump", "-res-usage", SO], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, check=True).stdout
-    names = re.findall(r"Function (\S+):\n\s+REG:(\d+) STACK:(\d+)", txt)
-    dem = subprocess.run(["c++filt"], input="\n".join(n for n, _, _ in names), stdout=subprocess.PIPE, text=True, check=True).stdout.splitlines()
-    use = {re.sub(r"\(.*", "", d).replace("void ", ""): (int(r), int(s)) for d, (_, r, s) in zip(dem, names)}
+@needs_binary_utils
+def test_sigmoid_xent_kernel_instances_have_no_stack_frame():
+    """the stand-alone kernel and the SIGMOID_LOSS GEMM variant (SfEpi 5), and the LOSS variants beside them"""
+    use = res_usage()
     want = ["sf::elementwise_loss_kernel<sf::SigmoidXentHead>", "sf::elementwise_loss_kernel<sf::MseHead>"]
-    want += [k for bn in (32, 64) for k in (f"sf::sf_gemm_epi_kernel<{bn}, false, 2>", f"sf::sf_gemm_sigmoid_loss_kernel<{bn}>")]
+    want += [f"sf::sf_gemm_kernel<{bn}, false, {epi}, false, false>" for bn in (32, 64) for epi in (2, 5)]
     missing = [k for k in want if k not in use]
     assert not missing, (missing, sorted(use))
     spilled = {k: use[k] for k in want if use[k][1] != 0}

@@ -8,10 +8,6 @@ that are not class indices; and the new kernels keep no stack frame.
 The oracle and graph helpers here are shared with tests/test_gpu_sparse_xent.py.
 """
 import dataclasses
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -27,10 +23,8 @@ from sparkflow_b200.models import zoo
 from sparkflow_b200.models.compiler import MAX_SPARSE_CLASSES, UnsupportedGraph, compile_graph
 from sparkflow_b200.parallel.plan_builder import check_grammar, loss_mode
 from sparkflow_b200.parallel.worker import check_class_labels
+from kernel_usage import needs_binary_utils, res_usage
 from test_step_gradients import _assert_grads, _forward, _grads, _rejects
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "sparkflow_b200", "_C.so")
 
 GRAPHS = {"sparse_dnn": zoo.sparse_dnn, "onehot_cnn": zoo.onehot_cnn, "sparse_dnn100": zoo.sparse_dnn100}
 CNN_GRAPHS = ("onehot_cnn",)
@@ -338,18 +332,15 @@ def test_label_check_accepts_class_indices():
 # ------------------------------------------------------------------------------------------------------------------
 # build artifacts
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not os.path.exists(SO) or shutil.which("cuobjdump") is None or shutil.which("c++filt") is None,
-                    reason="needs the built extension and the CUDA binary utilities")
-def test_sparse_xent_kernels_have_no_stack_frame():
+@needs_binary_utils
+def test_sparse_xent_kernel_instances_have_no_stack_frame():
     """the stand-alone kernel and the SPARSE_LOSS GEMM variant (SfEpi 6), which stays within the register count of the
     sigmoid loss variant it mirrors"""
-    txt = subprocess.run(["cuobjdump", "-res-usage", SO], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, check=True).stdout
-    names = re.findall(r"Function (\S+):\n\s+REG:(\d+) STACK:(\d+)", txt)
-    dem = subprocess.run(["c++filt"], input="\n".join(n for n, _, _ in names), stdout=subprocess.PIPE, text=True, check=True).stdout.splitlines()
-    use = {re.sub(r"\(.*", "", d).replace("void ", ""): (int(r), int(s)) for d, (_, r, s) in zip(dem, names)}
-    want = ["sf::sparse_softmax_xent_kernel", "sf::sf_gemm_sparse_loss_kernel"]
+    use = res_usage()
+    sparse, sigmoid = "sf::sf_gemm_kernel<32, false, 6, false, false>", "sf::sf_gemm_kernel<32, false, 5, false, false>"
+    want = ["sf::sparse_softmax_xent_kernel", sparse]
     missing = [k for k in want if k not in use]
     assert not missing, (missing, sorted(use))
     spilled = {k: use[k] for k in want if use[k][1] != 0}
     assert not spilled, f"kernels with a local-memory stack frame (REG, STACK): {spilled}"
-    assert use["sf::sf_gemm_sparse_loss_kernel"][0] <= use["sf::sf_gemm_sigmoid_loss_kernel<32>"][0]
+    assert use[sparse][0] <= use[sigmoid][0]
