@@ -2,11 +2,13 @@
 //
 //   D[M,N] = alpha * A[M,K] . B[N,K]^T          (both operands K-major, bf16, fp32 accumulate)
 //
-// One CTA computes one 128 x BN output tile (optionally one K-split of it):
+// One CTA computes one BM x BN output tile (optionally one K-split of it), BM = 128, or 64 for the specialized epilogue
+// variants when that keeps the grid one wave (sf_gemm_prepare):
 //   warp 0       : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx-count)
 //   warps 1-3    : bias tile loader
-//   warpgroups 1-2: wgmma main loop, 64 rows each, accumulator in registers; then both stage the fp32 tile in the
-//                  drained operand ring and run the epilogue (one row per thread, 32-column chunks -> fused math -> global)
+//   warpgroups 1-2: wgmma main loop, 64 rows each (64-row tile: warpgroup 1 alone), accumulator in registers; then both
+//                  stage the fp32 tile in the drained operand ring and run the epilogue (one row per thread, 32-column
+//                  chunks -> fused math -> global)
 //
 // Fused epilogues cover everything a dense layer needs in training (reference ops K1/K2 of
 // SURVEY.md section 2.4: MatMul+BiasAdd+{Relu,Sigmoid,Tanh}, their gradients and BiasAddGrad):
@@ -493,15 +495,16 @@ __device__ __forceinline__ void stage_acc(float* stg, const float (&acc)[BN / 2]
 // The act'(aux) chunk (DGRAD), label row (LOSS) or class index (SPARSE_LOSS, into tgt[0]) that consumer thread ct's
 // epilogue reads, fetched before the main loop
 // so that the load's latency hides under it.  Earlier launches wrote both, and everything upstream of this grid is
-// complete once pdl_wait has returned.  BN <= 64: a thread owns at most one chunk (c = q / 4, see epilogue_tile).
+// complete once pdl_wait has returned.  BN <= 64: a thread owns at most one chunk (its first, see epilogue_tile).
 template <int BN, int EPI>
 __device__ __forceinline__ void epi_prefetch(const SfGemmEpilogue& ep, uint4 (&aux)[4], float (&tgt)[32], int m0, int n0, int M, int N,
-                                             int ct) {
+                                             int ct, bool rows64) {
   static_assert(BN <= 64, "one 32-column chunk per consumer thread");
   const int q = ct >> 5, lane = ct & 31;
-  const int row = m0 + (q & 3) * 32 + lane;
-  const int col0 = n0 + (q >> 2) * 32;
-  const bool live = row < M && (q >> 2) < BN / 32 && col0 < ep.n_store_limit;
+  const int row = m0 + (q & (rows64 ? 1 : 3)) * 32 + lane;
+  const int c = q >> (rows64 ? 1 : 2);
+  const int col0 = n0 + c * 32;
+  const bool live = row < M && c < BN / 32 && col0 < ep.n_store_limit;
   if constexpr (EPI == SF_EPI_DGRAD) {
     const __nv_bfloat16* ap = ep.aux + static_cast<size_t>(live ? row : 0) * ep.ld_aux + col0;
 #pragma unroll
@@ -517,21 +520,23 @@ __device__ __forceinline__ void epi_prefetch(const SfGemmEpilogue& ep, uint4 (&a
 }
 
 // Epilogue of one 128 x BN tile from the staged accumulator, by the 256 consumer threads: warp q owns rows
-// 32 * (q % 4) .. + 32 (one row per lane) and every other 32-column chunk starting at chunk q / 4.  aux_pref / tgt_pref:
+// 32 * (q % 4) .. + 32 (one row per lane) and every other 32-column chunk starting at chunk q / 4.  A 64 x BN tile
+// (rows64): warp q owns rows 32 * (q % 2) .. + 32 and every fourth chunk starting at chunk q / 2.  aux_pref / tgt_pref:
 // the thread's chunk fetched by epi_prefetch (variants with EpiFeatures::kPrefetch only).  PEN: the L2 weight penalty, whose
 // loss term each warp adds with one atomic.
 template <int BN, int EPI, bool EXT, bool PEN = false>
 __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const float* stg, const float* s_bias, int m0, int n0, int M,
-                                              int N, int ct, const uint4* aux_pref = nullptr, const float* tgt_pref = nullptr) {
+                                              int N, int ct, bool rows64 = false, const uint4* aux_pref = nullptr,
+                                              const float* tgt_pref = nullptr) {
   using F = EpiFeatures<EPI>;
   const int q = ct >> 5, lane = ct & 31;
-  const int r = (q & 3) * 32 + lane;
+  const int r = (q & (rows64 ? 1 : 3)) * 32 + lane;
   const int row = m0 + r;
   const bool row_ok = row < M;
   const float* srow = stg + r * (BN + 1);
   float pen_sq = 0.f;
 #pragma unroll 1
-  for (int c = q >> 2; c < BN / 32; c += 2) {
+  for (int c = q >> (rows64 ? 1 : 2); c < BN / 32; c += (rows64 ? 4 : 2)) {
     const int col0 = n0 + c * 32;
     if (col0 >= ep.n_store_limit) break;   // whole chunk outside every output pitch
     uint32_t v[32];
@@ -560,7 +565,8 @@ __device__ __forceinline__ void epilogue_tile(const SfGemmEpilogue& ep, const fl
 }
 
 // Thread roles (384 threads): warp 0 lane 0 is the TMA producer, warps 1-3 load the bias tile, warpgroups 1 and 2 each
-// run the wgmma main loop for 64 rows of the tile and then, together, the epilogue.
+// run the wgmma main loop for 64 rows of the tile and then, together, the epilogue (a 64-row tile, ep.bm = 64: warpgroup 1
+// alone runs the main loop).
 // MN: both operands MN-major (D = a^T . b with a [K, M], b [K, N] row-major): the stage buffers have the same size, but a
 // stage is filled with {64 MN elements, 64 K rows} boxes and described to the tensor core as MN-major.
 // EPI: epilogue feature set (SfEpi); only the generic kernel handles the fused read-your-writes wait.  EXT: the extended
@@ -585,10 +591,15 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
   // waits for needs for its own CTAs.  A grid of several waves triggers at entry: its successor's CTAs only get SMs as
   // this grid drains.  A one-wave grid triggers after its main loop, see there.
   if ((!F::kRyw || ep.ryw == nullptr) && !ep.one_wave) pdl_launch_dependents();
+  // 64-row tile (specialized variants only): the A box, and with it the operand bytes this CTA streams through its SM,
+  // is half as tall, and the first consumer warpgroup alone runs the main loop - each output element still comes from the
+  // same m64 x BN x k16 wgmma sequence as in a 128-row tile
+  bool rows64 = false;
+  if constexpr (EPI != SF_EPI_GENERIC) rows64 = ep.bm == 64;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * BN;
-  const int m0 = blockIdx.y * kBM;
+  const int m0 = blockIdx.y * (rows64 ? 64 : kBM);
   const int total_kb = (K + kBK - 1) / kBK;
   const int kb_begin = blockIdx.z * kblocks_per_split;
   int kb_end = kb_begin + kblocks_per_split;
@@ -600,7 +611,7 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < S::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);        // one arrive per consumer warpgroup
+      mbar_init(&empty_bar[s], rows64 ? 1 : 2);        // one arrive per consumer warpgroup that runs the main loop
     }
     mbar_fence_init();
   }
@@ -640,15 +651,16 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
         mbar_wait(&empty_bar[s], ph ^ 1, 0x100 + s);
         uint8_t* a_dst = stage_base + s * S::kStageBytes;
         uint8_t* b_dst = a_dst + S::kABytes;
-        mbar_expect_tx(&full_bar[s], S::kStageBytes);
+        mbar_expect_tx(&full_bar[s], rows64 ? S::kABytes / 2 + S::kBBytes : S::kStageBytes);
         const int kc = (kb_begin + i) * kBK;
         if constexpr (MN) {
-#pragma unroll
-          for (int h = 0; h < kBM / 64; ++h) tma_load_2d(a_dst + h * 8192, &tmA, &full_bar[s], m0 + h * 64, kc, hintA);
+          static_assert(kBM == 128, "two 64-row A boxes per 128-row tile");
+          tma_load_2d(a_dst, &tmA, &full_bar[s], m0, kc, hintA);
+          if (!rows64) tma_load_2d(a_dst + 8192, &tmA, &full_bar[s], m0 + 64, kc, hintA);
 #pragma unroll
           for (int h = 0; h < BN / 64; ++h) tma_load_2d(b_dst + h * 8192, &tmB, &full_bar[s], n0 + h * 64, kc, hintB);
         } else {
-          tma_load_2d(a_dst, &tmA, &full_bar[s], kc, m0, hintA);
+          tma_load_2d(a_dst, &tmA, &full_bar[s], kc, m0, hintA);       // a box of BM rows: tmA is encoded at the tile height
           tma_load_2d(b_dst, &tmB, &full_bar[s], kc, n0, hintB);
         }
       }
@@ -680,24 +692,29 @@ __device__ __forceinline__ void gemm_cta(const CUtensorMap& tmA, const CUtensorM
     const int ct = threadIdx.x - 128;
     uint4 aux_pref[4];
     float tgt_pref[32];
-    if constexpr (F::kPrefetch) epi_prefetch<BN, EPI>(ep, aux_pref, tgt_pref, m0, n0, M, N, ct);
+    if constexpr (F::kPrefetch) epi_prefetch<BN, EPI>(ep, aux_pref, tgt_pref, m0, n0, M, N, ct, rows64);
     float acc[BN / 2];
-    mma_mainloop<BN, MN, S::kStages, S::kStageBytes, S::kABytes>(acc, stage_base, full_bar, empty_bar, 0, num_kb, ct >> 7,
-                                                                 (ct & 127) == 0, 0x200);
+    const bool mma = !rows64 || ct < 128;      // 64-row tile: the second warpgroup only joins the epilogue
+    if (mma)
+      mma_mainloop<BN, MN, S::kStages, S::kStageBytes, S::kABytes>(acc, stage_base, full_bar, empty_bar, 0, num_kb, ct >> 7,
+                                                                   (ct & 127) == 0, 0x200);
     // One-wave grid: the successor launches once every CTA is past its main loop, so its launch and prologue overlap
     // this epilogue.  A trigger at entry would let a chain of small GEMMs pre-launch in a cascade, and those waiting
     // CTAs (one per SM at this register / shared-memory size, 149 for the push) hold SMs the GEMMs ahead of them need.
-    if ((!F::kRyw || ep.ryw == nullptr) && ep.one_wave) pdl_launch_dependents();
-    // every stage has been consumed by both warpgroups: the ring holds the staged accumulator tile from here on
+    // The idle warpgroup of a 64-row tile triggers only past the barrier below, once the main loop is done.
+    const bool trigger = (!F::kRyw || ep.ryw == nullptr) && ep.one_wave;
+    if (trigger && mma) pdl_launch_dependents();
+    // every stage has been consumed by the main loop: the ring holds the staged accumulator tile from here on
     float* stg = reinterpret_cast<float*>(stage_base);
     asm volatile("bar.sync 1, 256;" ::: "memory");
-    stage_acc<BN>(stg, acc, ct);
+    if (trigger && !mma) pdl_launch_dependents();
+    if (mma) stage_acc<BN>(stg, acc, ct);
     asm volatile("bar.sync 1, 256;" ::: "memory");
     asm volatile("bar.sync 2, 352;" ::: "memory");      // bias tile in shared memory
     if constexpr (F::kPrefetch) {
-      epilogue_tile<BN, EPI, EXT>(ep, stg, s_bias, m0, n0, M, N, ct, aux_pref, tgt_pref);
+      epilogue_tile<BN, EPI, EXT>(ep, stg, s_bias, m0, n0, M, N, ct, rows64, aux_pref, tgt_pref);
     } else {
-      epilogue_tile<BN, EPI, EXT, PEN>(ep, stg, s_bias, m0, n0, M, N, ct);
+      epilogue_tile<BN, EPI, EXT, PEN>(ep, stg, s_bias, m0, n0, M, N, ct, rows64);
     }
   }
   trace.end(KID_GEMM);
@@ -919,22 +936,10 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
     g->pair = (want > 0 && eligible && !g->mn_major) ? 1 : 0;
     if (g->pair) g->bn = sf::kPairBN;
   }
-  if (!g->pair && (g->M + sf::kBM - 1) / sf::kBM > 65535) return -2;     // the one-CTA grid puts M tiles on grid.y
-  int rc;
   if (g->mn_major) {
-    // a is [K, lda] (M contiguous), b is [K, ldb] (N contiguous): boxes of {64 MN elements, 64 K rows}
     if (g->pair || g->ep.loss_mode != SF_LOSS_NONE) return -7;
     if (g->bn < 64) g->bn = 64;
     if (g->bn > 128) g->bn = 128;
-    rc = sf_make_tmap_bf16_kmajor(&g->tmA, g->a, g->K, g->M, g->lda, 64);
-    if (rc) return rc;
-    rc = sf_make_tmap_bf16_kmajor(&g->tmB, g->b, g->K, g->N, g->ldb, 64);
-    if (rc) return rc;
-  } else {
-    rc = sf_make_tmap_bf16_kmajor(&g->tmA, g->a, g->M, g->K, g->lda, sf::kBM);
-    if (rc) return rc;
-    rc = sf_make_tmap_bf16_kmajor(&g->tmB, g->b, g->N, g->K, g->ldb, g->pair ? sf::kPairBN / 2 : g->bn);
-    if (rc) return rc;
   }
   const int total_kb = (g->K + sf::kBK - 1) / sf::kBK;
   if (g->split_k > total_kb) g->split_k = total_kb;
@@ -947,10 +952,35 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
   int lim = g->N;
   if (g->ep.out_bf16 && g->ep.ld_bf16 > lim) lim = g->ep.ld_bf16;
   g->ep.n_store_limit = lim;
-  g->ep.one_wave = static_cast<long long>((g->N + g->bn - 1) / g->bn) * ((g->M + sf::kBM - 1) / sf::kBM) * g->split_k <= sf_num_sms();
   g->epi = g->epi == SF_EPI_GENERIC ? SF_EPI_GENERIC : pick_epi(g);
   if (g->ep.loss_mode == SF_LOSS_SIGMOID_XENT && g->epi != SF_EPI_SIGMOID_LOSS) return -5;
   if (g->ep.loss_mode == SF_LOSS_SPARSE_SOFTMAX_XENT && g->epi != SF_EPI_SPARSE_LOSS) return -5;
+  // Tile rows, settled before the A tensor map, whose box height they are.  A small grid's main loop is bound by the
+  // operand bytes one SM can take in, so a 64-row tile (half the A bytes per CTA, twice the CTAs) finishes sooner as
+  // long as the grid stays one wave.  Only the specialized variants implement it; a generic, split or pair GEMM, and one
+  // that carries the read-your-writes wait, keeps 128 rows.
+  const long long n_tiles = (g->N + g->bn - 1) / g->bn;
+  const bool can64 = !g->pair && g->epi != SF_EPI_GENERIC && g->split_k == 1;
+  if (g->bm == 0)
+    g->bm = (can64 && g->ep.ryw == nullptr && n_tiles * ((g->M + 63) / 64) <= sf_num_sms()) ? 64 : sf::kBM;
+  else if (g->bm != sf::kBM && (g->bm != 64 || !can64))
+    return -7;
+  g->ep.bm = g->bm;
+  if (!g->pair && (g->M + g->bm - 1) / g->bm > 65535) return -2;     // the one-CTA grid puts M tiles on grid.y
+  g->ep.one_wave = n_tiles * ((g->M + g->bm - 1) / g->bm) * g->split_k <= sf_num_sms();
+  int rc;
+  if (g->mn_major) {
+    // a is [K, lda] (M contiguous), b is [K, ldb] (N contiguous): boxes of {64 MN elements, 64 K rows}
+    rc = sf_make_tmap_bf16_kmajor(&g->tmA, g->a, g->K, g->M, g->lda, 64);
+    if (rc) return rc;
+    rc = sf_make_tmap_bf16_kmajor(&g->tmB, g->b, g->K, g->N, g->ldb, 64);
+    if (rc) return rc;
+  } else {
+    rc = sf_make_tmap_bf16_kmajor(&g->tmA, g->a, g->M, g->K, g->lda, g->bm);
+    if (rc) return rc;
+    rc = sf_make_tmap_bf16_kmajor(&g->tmB, g->b, g->N, g->K, g->ldb, g->pair ? sf::kPairBN / 2 : g->bn);
+    if (rc) return rc;
+  }
   if (!g->pair) {
     g->kernel = find_gemm_kernel(g->bn, g->mn_major != 0, g->epi, uses_ext_act(g->ep), has_penalty(g->ep));
     if (g->kernel < 0) return -3;
@@ -961,7 +991,7 @@ extern "C" int sf_gemm_prepare(SfGemm* g) {
 extern "C" int sf_gemm_launch(const SfGemm* g, cudaStream_t st) {
   if (g->pair) return sf_gemm_pair_launch(g, st);
   const sf::GemmKernel& k = sf::kGemmKernels[g->kernel];
-  const dim3 grid((g->N + k.bn - 1) / k.bn, (g->M + sf::kBM - 1) / sf::kBM, g->split_k);
+  const dim3 grid((g->N + k.bn - 1) / k.bn, (g->M + g->bm - 1) / g->bm, g->split_k);
   return static_cast<int>(sf::launch(k.fn, grid, dim3(sf::kGemmThreads), k.smem, st, g->tmA, g->tmB, g->ep, g->M, g->N, g->K,
                                      g->kblocks_per_split));
 }

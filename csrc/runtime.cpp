@@ -91,6 +91,7 @@ struct Gemm {
     g.lda = getd<int>(d, "lda", g.K);
     g.ldb = getd<int>(d, "ldb", g.K);
     g.bn = getd<int>(d, "bn", 0);
+    g.bm = getd<int>(d, "bm", 0);
     g.split_k = getd<int>(d, "split_k", 1);
     g.pair = getd<int>(d, "pair", -1);
     g.mn_major = getd<int>(d, "mn_major", 0);
@@ -142,12 +143,13 @@ struct Gemm {
   }
   void launch(uintptr_t stream) const { ck_rc(sf_gemm_launch(&g, S(stream)), "sf_gemm_launch"); }
   int bn() const { return g.bn; }
+  int bm() const { return g.bm; }
   int split_k() const { return g.split_k; }
   int kblocks_per_split() const { return g.kblocks_per_split; }
   int pair() const { return g.pair; }
   int epi() const { return g.epi; }
   py::tuple grid() const {
-    return py::make_tuple((g.N + g.bn - 1) / g.bn, (g.M + 127) / 128, g.split_k);
+    return py::make_tuple((g.N + g.bn - 1) / g.bn, (g.M + g.bm - 1) / g.bm, g.split_k);
   }
   int mn_major() const { return g.mn_major; }
 };
@@ -1063,6 +1065,7 @@ PYBIND11_MODULE(_C, m) {
       .def(py::init<const py::dict&>())
       .def("launch", &Gemm::launch)
       .def_property_readonly("bn", &Gemm::bn)
+      .def_property_readonly("bm", &Gemm::bm)
       .def_property_readonly("split_k", &Gemm::split_k)
       .def_property_readonly("kblocks_per_split", &Gemm::kblocks_per_split)
       .def_property_readonly("pair", &Gemm::pair)

@@ -119,6 +119,7 @@ struct SfGemmEpilogue {
   float pen_b2c;                  // 2c_b
   float* pen_db;                  // bias gradient [N]
   float* pen_loss;                // loss accumulator (required with a penalty)
+  int bm;                         // filled by sf_gemm_prepare: rows of the one-CTA kernel's output tile (SfGemm.bm)
 };
 
 enum SfLossMode { SF_LOSS_NONE = 0, SF_LOSS_SOFTMAX_XENT = 1, SF_LOSS_MSE = 2, SF_LOSS_SIGMOID_XENT = 3, SF_LOSS_SPARSE_SOFTMAX_XENT = 4 };
@@ -144,6 +145,9 @@ struct SfGemm {
   int M, N, K;
   int lda, ldb;
   int bn;                         // 0 = auto
+  int bm;                         // in: 0 = auto, 64 or 128 = forced; out: rows of the one-CTA kernel's output tile.  64
+                                  // only on a specialized epilogue variant without a K split (auto: when the grid of
+                                  // 64-row tiles is still one wave); the pair kernel's value is 128
   int split_k;                    // 0/1 = none
   int kblocks_per_split;          // filled
   int mn_major;                   // 1: BOTH operands are MN-major: a is [K, lda] with M contiguous, b is [K, ldb] with N contiguous
