@@ -180,37 +180,95 @@ col2im_kernel(const __nv_bfloat16* __restrict__ dcols, int ld_cols, int n, int h
 // Optional outT[(y*ow + x)*C + c][b] is the transposed flattened activation (K-major operand of the
 // following dense layer's wgrad).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, __nv_bfloat16* __restrict__ out,
-                   uint8_t* __restrict__ argmax, __nv_bfloat16* __restrict__ outT, int ld_t) {
+// Dropout of a pool output (the *_drop_* kernels): each pooled element is kept with probability keep and scaled by 1 / keep,
+// under the key of the GEMM epilogue's dropout (dropout_keep4) with the pooled tensor as the matrix [n * oh * ow, c];
+// the kept bit goes into bit 7 of its argmax byte (a window has at most 16 cells: bits 4-7 are free), where the backward
+// kernels read it.  ctr: the device word that changes every step (nullptr: 0).  A thread of the 2x2 twin pools the 4
+// channels of one Philox group (c % 4 == 0), so each draw is computed once.
+struct PoolDropout {
+  float keep;
+  uint32_t seed, stream;
+  const uint32_t* ctr;
+};
+constexpr uint8_t kKeptBit = 0x80;
+
+// elements per thread: one, or a twin's Philox group of 4 channels
+template <bool DROP>
+constexpr int kPoolGroup = DROP ? 4 : 1;
+
+// the keep bits of the Philox group at pixel row `row`, channels cc0 .. cc0 + 3 (cc0 % 4 == 0): bit j = channel cc0 + j
+// kept (a bit mask, not an array: the general kernel's group loop stays rolled, and an indexed array would be local memory)
+__device__ __forceinline__ uint32_t pool_keep_bits(size_t row, int cc0, uint32_t step, const PoolDropout& d, uint32_t thr) {
+  const DropKeep4 k = dropout_keep4(static_cast<uint32_t>(row), static_cast<uint32_t>(cc0 >> 2), step, d.stream, d.seed, thr);
+  return (k.k0 ? 1u : 0u) | (k.k1 ? 2u : 0u) | (k.k2 ? 4u : 0u) | (k.k3 ? 8u : 0u);
+}
+
+// pooled element j (0..3) of a thread's group: value `best` (winner `bi`), after the dropout when DROP
+template <bool DROP>
+__device__ __forceinline__ void pool_store(__nv_bfloat16* __restrict__ out, uint8_t* __restrict__ argmax, size_t i, float best, int bi,
+                                           uint32_t keep_bits, int j, float inv_keep) {
+  bool kept = false;
+  if constexpr (DROP) {
+    kept = (keep_bits >> j) & 1u;
+    best = kept ? best * inv_keep : 0.f;
+  }
+  out[i] = __float2bfloat16(best);
+  argmax[i] = static_cast<uint8_t>(DROP && kept ? bi | kKeptBit : bi);
+}
+
+template <bool DROP>
+__device__ __forceinline__ void maxpool_fwd_body(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, __nv_bfloat16* __restrict__ out,
+                                                 uint8_t* __restrict__ argmax, __nv_bfloat16* __restrict__ outT, int ld_t, const PoolDropout& d) {
   TraceScope trace;
   pdl_launch_dependents();
   pdl_wait();
   trace.mark();
+  const uint32_t step = DROP && d.ctr != nullptr ? *d.ctr : 0u;
+  const uint32_t thr = DROP ? dropout_threshold(d.keep) : 0u;
+  const float inv_keep = DROP ? __fdividef(1.f, d.keep) : 1.f;
   const int oh = h / 2, ow = w / 2;
-  const size_t total = static_cast<size_t>(n) * oh * ow * c;
-  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int cc = static_cast<int>(i % c);
-    size_t t = i / c;
+  constexpr int G = kPoolGroup<DROP>;
+  const size_t total = static_cast<size_t>(n) * oh * ow * c / G;
+  for (size_t u = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; u < total;
+       u += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t i0 = u * G;
+    const int cc0 = static_cast<int>(i0 % c);
+    size_t t = i0 / c;
+    const uint32_t keep_bits = DROP ? pool_keep_bits(t, cc0, step, d, thr) : 0u;
     const int x = static_cast<int>(t % ow);
     t /= ow;
     const int y = static_cast<int>(t % oh);
     const int b = static_cast<int>(t / oh);
-    const __nv_bfloat16* p = in + ((static_cast<size_t>(b) * h + 2 * y) * w + 2 * x) * c + cc;
-    float best = __bfloat162float(p[0]);
-    int bi = 0;
-    const float v1 = __bfloat162float(p[c]);
-    const float v2 = __bfloat162float(p[static_cast<size_t>(w) * c]);
-    const float v3 = __bfloat162float(p[static_cast<size_t>(w) * c + c]);
-    if (v1 > best) { best = v1; bi = 1; }
-    if (v2 > best) { best = v2; bi = 2; }
-    if (v3 > best) { best = v3; bi = 3; }
-    out[i] = __float2bfloat16(best);
-    argmax[i] = static_cast<uint8_t>(bi);
-    if (outT != nullptr) outT[static_cast<size_t>((y * ow + x) * c + cc) * ld_t + b] = __float2bfloat16(best);
+#pragma unroll
+    for (int j = 0; j < G; ++j) {
+      const size_t i = i0 + j;
+      const int cc = cc0 + j;
+      const __nv_bfloat16* p = in + ((static_cast<size_t>(b) * h + 2 * y) * w + 2 * x) * c + cc;
+      float best = __bfloat162float(p[0]);
+      int bi = 0;
+      const float v1 = __bfloat162float(p[c]);
+      const float v2 = __bfloat162float(p[static_cast<size_t>(w) * c]);
+      const float v3 = __bfloat162float(p[static_cast<size_t>(w) * c + c]);
+      if (v1 > best) { best = v1; bi = 1; }
+      if (v2 > best) { best = v2; bi = 2; }
+      if (v3 > best) { best = v3; bi = 3; }
+      pool_store<DROP>(out, argmax, i, best, bi, keep_bits, j, inv_keep);
+      if (!DROP && outT != nullptr) outT[static_cast<size_t>((y * ow + x) * c + cc) * ld_t + b] = __float2bfloat16(best);
+    }
   }
   trace.end(KID_POOL_FWD);
+}
+
+__global__ void __launch_bounds__(256)
+maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, __nv_bfloat16* __restrict__ out,
+                   uint8_t* __restrict__ argmax, __nv_bfloat16* __restrict__ outT, int ld_t) {
+  maxpool_fwd_body<false>(in, n, h, w, c, out, argmax, outT, ld_t, PoolDropout{});
+}
+// the dropout twin writes no transposed copy: only the K-major weight gradient reads one, and it takes no image dropout
+__global__ void __launch_bounds__(256)
+maxpool_drop_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, __nv_bfloat16* __restrict__ out,
+                        uint8_t* __restrict__ argmax, PoolDropout d) {
+  maxpool_fwd_body<true>(in, n, h, w, c, out, argmax, nullptr, 0, d);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -233,12 +291,31 @@ template <bool EXT>
 __device__ __forceinline__ float pool_dact(float a, int act, float alpha) {
   return EXT ? act_ext_dact(a, act, alpha) : pool_dact(a, act);
 }
-
+// act'(z) / keep of a unit whose stored output a = act(z) * mask / keep carries a dropout (keep in (0, 1); otherwise plain
+// act'(a)): the dense dgrad's aux_keep rule - mask = a != 0, act' taken at a * keep; a ReLU6 saturates in stored units,
+// bf16(6 / keep), as the forward epilogue rounded it
 template <bool EXT>
+__device__ __forceinline__ float drop_dact(float a, int act, float alpha, float keep) {
+  if (!(keep > 0.f && keep < 1.f)) return pool_dact<EXT>(a, act, alpha);
+  const float ik = __fdividef(1.f, keep);
+  if (EXT && act == SF_ACT_RELU6) return (a > 0.f && a < __bfloat162float(__float2bfloat16(6.f * ik))) ? ik : 0.f;
+  return a != 0.f ? pool_dact<EXT>(a * keep, act, alpha) * ik : 0.f;
+}
+// the gradient `g` of a pooled element with argmax byte `am` that passes to its winner: times kept / keep under a dropout
+// of the pool output (DROP and pool_keep in (0, 1))
+template <bool DROP>
+__device__ __forceinline__ float pool_drop_grad(float g, uint8_t am, float pool_keep) {
+  if (DROP && pool_keep > 0.f && pool_keep < 1.f) return (am & kKeptBit) ? g * __fdividef(1.f, pool_keep) : 0.f;
+  return g;
+}
+
+// DROP: the dropout twins - pool_keep: a dropout on the pooled output (its kept bit in argmax bit 7), act_keep: one on the
+// conv output (in act_out); at most one of them in (0, 1).  They write no dz^T (no K-major weight gradient with dropout).
+template <bool EXT, bool DROP = false>
 __device__ __forceinline__ void maxpool_bwd_tile(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h,
                                                  int w, int c, const __nv_bfloat16* __restrict__ act_out, int act, float alpha,
                                                  __nv_bfloat16* __restrict__ dz, int ld_dz, __nv_bfloat16* __restrict__ dzT, int ld_t,
-                                                 float* __restrict__ dbias) {
+                                                 float* __restrict__ dbias, float pool_keep = 0.f, float act_keep = 0.f) {
   __shared__ __nv_bfloat16 tile[32][34];
   __shared__ float s_col[32];
   TraceScope trace;
@@ -262,12 +339,18 @@ __device__ __forceinline__ void maxpool_bwd_tile(const __nv_bfloat16* __restrict
       const int py = y >> 1, px = x >> 1;
       if (py < oh && px < ow) {
         const size_t o = ((static_cast<size_t>(b) * oh + py) * ow + px) * c + cc;
-        if (argmax[o] == ((y & 1) * 2 + (x & 1)))
+        if (DROP) {
+          const uint8_t am = argmax[o];
+          if ((am & ~kKeptBit) == ((y & 1) * 2 + (x & 1)))
+            g = pool_drop_grad<DROP>(__bfloat162float(dout[o]), am, pool_keep) *
+                drop_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha, act_keep);
+        } else if (argmax[o] == ((y & 1) * 2 + (x & 1))) {
           g = __bfloat162float(dout[o]) * pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha);
+        }
       }
     }
     const __nv_bfloat16 gb = __float2bfloat16(g);
-    tile[ty + 8 * i][tx] = gb;
+    if (!DROP) tile[ty + 8 * i][tx] = gb;
     cacc += g;
     if (dz != nullptr && m < M && cc < ld_dz) dz[static_cast<size_t>(m) * ld_dz + cc] = gb;
   }
@@ -275,7 +358,7 @@ __device__ __forceinline__ void maxpool_bwd_tile(const __nv_bfloat16* __restrict
   __syncthreads();
   if (dbias != nullptr && threadIdx.x < 32 && c0 + threadIdx.x < c && s_col[threadIdx.x] != 0.f)
     atomicAdd(dbias + c0 + threadIdx.x, s_col[threadIdx.x]);
-  if (dzT != nullptr) {
+  if (!DROP && dzT != nullptr) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int cc = c0 + ty + 8 * i, m = m0 + tx;
@@ -297,24 +380,38 @@ maxpool_bwd_ext_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __
                        __nv_bfloat16* __restrict__ dzT, int ld_t, float* __restrict__ dbias) {
   maxpool_bwd_tile<true>(dout, argmax, n, h, w, c, act_out, act, alpha, dz, ld_dz, dzT, ld_t, dbias);
 }
+template <bool EXT>
+__global__ void __launch_bounds__(256)
+maxpool_drop_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c,
+                        const __nv_bfloat16* __restrict__ act_out, int act, float alpha, float pool_keep, float act_keep,
+                        __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+  maxpool_bwd_tile<EXT, true>(dout, argmax, n, h, w, c, act_out, act, alpha, dz, ld_dz, nullptr, 0, dbias, pool_keep, act_keep);
+}
 
 // ------------------------------------------------------------------------------------------------
 // General max pool: kh x kw window (<= 4x4), stride (sh, sw), pad_top / pad_left cells in front (SAME or VALID).  argmax
 // stores the winner's in-window index dy * kw + dx; padded cells never win; ties go to the first cell in row-major order,
 // as in maxpool_fwd_kernel.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-maxpool_gen_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pt, int pl,
-                       int oh, int ow, __nv_bfloat16* __restrict__ out, uint8_t* __restrict__ argmax) {
+template <bool DROP>
+__device__ __forceinline__ void maxpool_gen_fwd_body(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, int kh, int kw, int sh,
+                                                     int sw, int pt, int pl, int oh, int ow, __nv_bfloat16* __restrict__ out,
+                                                     uint8_t* __restrict__ argmax, const PoolDropout& d) {
   TraceScope trace;
   pdl_launch_dependents();
   pdl_wait();
   trace.mark();
+  const uint32_t step = DROP && d.ctr != nullptr ? *d.ctr : 0u;
+  const uint32_t thr = DROP ? dropout_threshold(d.keep) : 0u;
+  const float inv_keep = DROP ? __fdividef(1.f, d.keep) : 1.f;
+  // one element per thread: grouping the 4 channels of a Philox draw, as the 2x2 twin does, puts this kernel's loop state in
+  // local memory; the draw of the group is recomputed per element and its lane taken
   const size_t total = static_cast<size_t>(n) * oh * ow * c;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int cc = static_cast<int>(i % c);
     size_t t = i / c;
+    const uint32_t keep_bits = DROP ? pool_keep_bits(t, cc & ~3, step, d, thr) >> (cc & 3) : 0u;
     const int x = static_cast<int>(t % ow);
     t /= ow;
     const int y = static_cast<int>(t % oh);
@@ -333,10 +430,20 @@ maxpool_gen_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w
         if (v > best) { best = v; bi = dy * kw + dx; }
       }
     }
-    out[i] = __float2bfloat16(best);
-    argmax[i] = static_cast<uint8_t>(bi);
+    pool_store<DROP>(out, argmax, i, best, bi, keep_bits, 0, inv_keep);
   }
   trace.end(KID_POOL_GEN_FWD);
+}
+
+__global__ void __launch_bounds__(256)
+maxpool_gen_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pt, int pl,
+                       int oh, int ow, __nv_bfloat16* __restrict__ out, uint8_t* __restrict__ argmax) {
+  maxpool_gen_fwd_body<false>(in, n, h, w, c, kh, kw, sh, sw, pt, pl, oh, ow, out, argmax, PoolDropout{});
+}
+__global__ void __launch_bounds__(256)
+maxpool_gen_drop_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pt, int pl,
+                            int oh, int ow, __nv_bfloat16* __restrict__ out, uint8_t* __restrict__ argmax, PoolDropout d) {
+  maxpool_gen_fwd_body<true>(in, n, h, w, c, kh, kw, sh, sw, pt, pl, oh, ow, out, argmax, d);
 }
 
 // General max-pool backward, a gather over the conv-output positions fused with act'(a) and the bias gradient:
@@ -344,11 +451,12 @@ maxpool_gen_fwd_kernel(const __nv_bfloat16* __restrict__ in, int n, int h, int w
 //                    of dout[b, py, px, c]
 // (overlapping windows: a position collects the gradient of every window it won).  Row-major dz [M, ld_dz] and the
 // column sums over M into dbias[C]; one 32(m) x 32(c) tile per CTA, M tiles on x.
-template <bool EXT>
+template <bool EXT, bool DROP = false>
 __device__ __forceinline__ void maxpool_gen_bwd_tile(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n,
                                                      int h, int w, int c, int kh, int kw, int sh, int sw, int pt, int pl, int oh, int ow,
                                                      const __nv_bfloat16* __restrict__ act_out, int act, float alpha,
-                                                     __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+                                                     __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias,
+                                                     float pool_keep = 0.f, float act_keep = 0.f) {
   __shared__ float s_col[32];
   TraceScope trace;
   pdl_launch_dependents();
@@ -375,10 +483,18 @@ __device__ __forceinline__ void maxpool_gen_bwd_tile(const __nv_bfloat16* __rest
         const int dy = yp - py * sh;
         for (int px = px_lo; px <= px_hi; ++px) {
           const size_t o = static_cast<size_t>((b * oh + py) * ow + px) * c + cc;
-          if (argmax[o] == dy * kw + (xp - px * sw)) g += __bfloat162float(dout[o]);
+          if (DROP) {
+            const uint8_t am = argmax[o];
+            if ((am & ~kKeptBit) == dy * kw + (xp - px * sw)) g += pool_drop_grad<DROP>(__bfloat162float(dout[o]), am, pool_keep);
+          } else if (argmax[o] == dy * kw + (xp - px * sw)) {
+            g += __bfloat162float(dout[o]);
+          }
         }
       }
-      if (g != 0.f) g *= pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha);
+      if (g != 0.f) {
+        const float a = __bfloat162float(act_out[static_cast<size_t>(m) * c + cc]);
+        g *= DROP ? drop_dact<EXT>(a, act, alpha, act_keep) : pool_dact<EXT>(a, act, alpha);
+      }
     }
     cacc += g;
     if (dz != nullptr && m < M && cc < ld_dz) dz[static_cast<size_t>(m) * ld_dz + cc] = __float2bfloat16(g);
@@ -403,16 +519,26 @@ maxpool_gen_bwd_ext_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t
                            float alpha, __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
   maxpool_gen_bwd_tile<true>(dout, argmax, n, h, w, c, kh, kw, sh, sw, pt, pl, oh, ow, act_out, act, alpha, dz, ld_dz, dbias);
 }
+template <bool EXT>
+__global__ void __launch_bounds__(256, 4)
+maxpool_gen_drop_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const uint8_t* __restrict__ argmax, int n, int h, int w, int c, int kh,
+                            int kw, int sh, int sw, int pt, int pl, int oh, int ow, const __nv_bfloat16* __restrict__ act_out, int act,
+                            float alpha, float pool_keep, float act_keep, __nv_bfloat16* __restrict__ dz, int ld_dz,
+                            float* __restrict__ dbias) {
+  maxpool_gen_bwd_tile<EXT, true>(dout, argmax, n, h, w, c, kh, kw, sh, sw, pt, pl, oh, ow, act_out, act, alpha, dz, ld_dz, dbias, pool_keep,
+                                  act_keep);
+}
 
 // ------------------------------------------------------------------------------------------------
 // Activation gradient of a conv with no pool after it: dz[m, c] = g[m, c] * act'(a[m, c]) written row-major [M, ld_dz], and
 // the column sums over M added into dbias[C].  g is the gradient wrt the conv's activation output: col2im of the next conv
 // or the flatten dgrad of the dense layer above.  Same 32(m) x 32(c) tile and s_col reduction as maxpool_bwd_kernel.
 // ------------------------------------------------------------------------------------------------
-template <bool EXT>
+// DROP: the dropout twins, keep = that of the conv output's dropout (drop_dact)
+template <bool EXT, bool DROP = false>
 __device__ __forceinline__ void act_bwd_bias_tile(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c,
                                                   const __nv_bfloat16* __restrict__ act_out, int act, float alpha,
-                                                  __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+                                                  __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias, float keep = 0.f) {
   __shared__ float s_col[32];
   TraceScope trace;
   pdl_launch_dependents();
@@ -429,7 +555,8 @@ __device__ __forceinline__ void act_bwd_bias_tile(const __nv_bfloat16* __restric
     float v = 0.f;
     if (m < M && cc < c)
       v = __bfloat162float(g[static_cast<size_t>(m) * ld_g + cc]) *
-          pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha);
+          (DROP ? drop_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha, keep)
+                : pool_dact<EXT>(__bfloat162float(act_out[static_cast<size_t>(m) * c + cc]), act, alpha));
     cacc += v;
     if (dz != nullptr && m < M && cc < ld_dz) dz[static_cast<size_t>(m) * ld_dz + cc] = __float2bfloat16(v);
   }
@@ -449,6 +576,12 @@ __global__ void __launch_bounds__(256)
 act_bwd_bias_ext_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c, const __nv_bfloat16* __restrict__ act_out, int act,
                         float alpha, __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
   act_bwd_bias_tile<true>(g, ld_g, M, c, act_out, act, alpha, dz, ld_dz, dbias);
+}
+template <bool EXT>
+__global__ void __launch_bounds__(256)
+act_drop_bwd_bias_kernel(const __nv_bfloat16* __restrict__ g, int ld_g, int M, int c, const __nv_bfloat16* __restrict__ act_out, int act,
+                         float alpha, float keep, __nv_bfloat16* __restrict__ dz, int ld_dz, float* __restrict__ dbias) {
+  act_bwd_bias_tile<EXT, true>(g, ld_g, M, c, act_out, act, alpha, dz, ld_dz, dbias, keep);
 }
 
 }  // namespace sf
@@ -514,6 +647,27 @@ extern "C" int sf_maxpool2_bwd(const __nv_bfloat16* dout, const uint8_t* argmax,
                                      ld_dz, dzT, ld_t, dbias));
 }
 
+extern "C" int sf_maxpool2_drop_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, __nv_bfloat16* out, uint8_t* argmax, float keep,
+                                    unsigned int seed, unsigned int stream, const unsigned int* ctr, cudaStream_t st) {
+  if (!(keep > 0.f && keep < 1.f) || (c & 3)) return -8;
+  const size_t total = static_cast<size_t>(n) * (h / 2) * (w / 2) * c;
+  return static_cast<int>(sf::launch(sf::maxpool_drop_fwd_kernel, dim3(grid_1d(total / 4)), dim3(256), 0, st, in, n, h, w, c, out, argmax,
+                                     sf::PoolDropout{keep, seed, stream, ctr}));
+}
+
+extern "C" int sf_maxpool2_drop_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, const __nv_bfloat16* act_out,
+                                    int act, float act_alpha, float pool_keep, float act_keep, __nv_bfloat16* dz, int ld_dz, float* dbias,
+                                    cudaStream_t st) {
+  const int M = n * h * w;
+  const int span_c = (dz && ld_dz > c) ? ld_dz : c;
+  dim3 grid((M + 31) / 32, (span_c + 31) / 32);
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::maxpool_drop_bwd_kernel<true>, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, act_out, act,
+                                       act_alpha, pool_keep, act_keep, dz, ld_dz, dbias));
+  return static_cast<int>(sf::launch(sf::maxpool_drop_bwd_kernel<false>, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, act_out, act,
+                                     act_alpha, pool_keep, act_keep, dz, ld_dz, dbias));
+}
+
 extern "C" int sf_maxpool_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left,
                               int out_h, int out_w, __nv_bfloat16* out, uint8_t* argmax, cudaStream_t st) {
   if (kh < 1 || kw < 1 || kh > 4 || kw > 4 || sh < 1 || sw < 1) return -8;
@@ -536,6 +690,42 @@ extern "C" int sf_maxpool_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, 
                                        pad_top, pad_left, out_h, out_w, act_out, act, act_alpha, dz, ld_dz, dbias));
   return static_cast<int>(sf::launch(sf::maxpool_gen_bwd_kernel, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, kh, kw, sh, sw, pad_top,
                                      pad_left, out_h, out_w, act_out, act, dz, ld_dz, dbias));
+}
+
+extern "C" int sf_maxpool_drop_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
+                                   int pad_left, int out_h, int out_w, __nv_bfloat16* out, uint8_t* argmax, float keep, unsigned int seed,
+                                   unsigned int stream, const unsigned int* ctr, cudaStream_t st) {
+  if (kh < 1 || kw < 1 || kh > 4 || kw > 4 || sh < 1 || sw < 1 || !(keep > 0.f && keep < 1.f)) return -8;
+  conv_out_size(h, w, kh, kw, sh, sw, out_h, out_w);
+  const size_t total = static_cast<size_t>(n) * out_h * out_w * c;
+  return static_cast<int>(sf::launch(sf::maxpool_gen_drop_fwd_kernel, dim3(grid_1d(total)), dim3(256), 0, st, in, n, h, w, c, kh, kw, sh, sw,
+                                     pad_top, pad_left, out_h, out_w, out, argmax, sf::PoolDropout{keep, seed, stream, ctr}));
+}
+
+extern "C" int sf_maxpool_drop_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw,
+                                   int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, float act_alpha,
+                                   float pool_keep, float act_keep, __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st) {
+  if (kh < 1 || kw < 1 || kh > 4 || kw > 4 || sh < 1 || sw < 1) return -8;
+  conv_out_size(h, w, kh, kw, sh, sw, out_h, out_w);
+  const int M = n * h * w;
+  const int span_c = (dz && ld_dz > c) ? ld_dz : c;
+  dim3 grid((M + 31) / 32, (span_c + 31) / 32);
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::maxpool_gen_drop_bwd_kernel<true>, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, kh, kw, sh, sw,
+                                       pad_top, pad_left, out_h, out_w, act_out, act, act_alpha, pool_keep, act_keep, dz, ld_dz, dbias));
+  return static_cast<int>(sf::launch(sf::maxpool_gen_drop_bwd_kernel<false>, grid, dim3(256), 0, st, dout, argmax, n, h, w, c, kh, kw, sh, sw,
+                                     pad_top, pad_left, out_h, out_w, act_out, act, act_alpha, pool_keep, act_keep, dz, ld_dz, dbias));
+}
+
+extern "C" int sf_act_drop_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, float act_alpha,
+                                    float keep, __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st) {
+  const int span_c = (dz && ld_dz > c) ? ld_dz : c;
+  dim3 grid((rows + 31) / 32, (span_c + 31) / 32);
+  if (act >= SF_ACT_ELU)
+    return static_cast<int>(sf::launch(sf::act_drop_bwd_bias_kernel<true>, grid, dim3(256), 0, st, g, ld_g, rows, c, act_out, act, act_alpha,
+                                       keep, dz, ld_dz, dbias));
+  return static_cast<int>(sf::launch(sf::act_drop_bwd_bias_kernel<false>, grid, dim3(256), 0, st, g, ld_g, rows, c, act_out, act, act_alpha,
+                                     keep, dz, ld_dz, dbias));
 }
 
 extern "C" int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, float act_alpha,

@@ -211,16 +211,16 @@ __device__ __forceinline__ void epi_chunk(const SfGemmEpilogue& ep, const uint32
     if (F::kGeneric && ep.drop_keep > 0.f && ep.drop_keep < 1.f) {
       // fused dropout: keep with probability drop_keep, scale the survivors by 1 / drop_keep
       const float inv_keep = __fdividef(1.f, ep.drop_keep);
-      const uint32_t thr = static_cast<uint32_t>(fminf(ep.drop_keep * 4294967296.f, 4294967040.f));
+      const uint32_t thr = dropout_threshold(ep.drop_keep);
       const uint32_t stepc = ep.drop_ctr != nullptr ? *ep.drop_ctr : 0u;
 #pragma unroll
       for (int g = 0; g < 8; ++g) {
-        const uint4 rnd = philox4x32_10(make_uint4(static_cast<uint32_t>(row), static_cast<uint32_t>(col0 >> 2) + g, stepc, ep.drop_stream),
-                                        make_uint2(ep.drop_seed, 0x5F3759DFu));
-        f[4 * g + 0] = rnd.x < thr ? f[4 * g + 0] * inv_keep : 0.f;
-        f[4 * g + 1] = rnd.y < thr ? f[4 * g + 1] * inv_keep : 0.f;
-        f[4 * g + 2] = rnd.z < thr ? f[4 * g + 2] * inv_keep : 0.f;
-        f[4 * g + 3] = rnd.w < thr ? f[4 * g + 3] * inv_keep : 0.f;
+        const DropKeep4 k = dropout_keep4(static_cast<uint32_t>(row), static_cast<uint32_t>(col0 >> 2) + g, stepc, ep.drop_stream,
+                                          ep.drop_seed, thr);
+        f[4 * g + 0] = k.k0 ? f[4 * g + 0] * inv_keep : 0.f;
+        f[4 * g + 1] = k.k1 ? f[4 * g + 1] * inv_keep : 0.f;
+        f[4 * g + 2] = k.k2 ? f[4 * g + 2] * inv_keep : 0.f;
+        f[4 * g + 3] = k.k3 ? f[4 * g + 3] * inv_keep : 0.f;
       }
     }
     if (tq != nullptr) tq[2] = trace_now();

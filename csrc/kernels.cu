@@ -31,6 +31,11 @@ extern "C" int sf_preload_kernels() {
   // the twins of the extended activations (SfAct 4-9)
   SF_PRELOAD(sf::mse_ext_loss_kernel);
   SF_PRELOAD(sf::maxpool_bwd_ext_kernel); SF_PRELOAD(sf::maxpool_gen_bwd_ext_kernel); SF_PRELOAD(sf::act_bwd_bias_ext_kernel);
+  // the dropout twins of the pool and activation-gradient kernels (an image dropout), with and without the extended set
+  SF_PRELOAD(sf::maxpool_drop_fwd_kernel); SF_PRELOAD(sf::maxpool_gen_drop_fwd_kernel);
+  SF_PRELOAD(sf::maxpool_drop_bwd_kernel<false>); SF_PRELOAD(sf::maxpool_drop_bwd_kernel<true>);
+  SF_PRELOAD(sf::maxpool_gen_drop_bwd_kernel<false>); SF_PRELOAD(sf::maxpool_gen_drop_bwd_kernel<true>);
+  SF_PRELOAD(sf::act_drop_bwd_bias_kernel<false>); SF_PRELOAD(sf::act_drop_bwd_bias_kernel<true>);
   SF_PRELOAD((sf::conv_first_fwd_kernel<5, 5, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<5, 5, 1>));
   SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 1>));
   SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 3>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 3>));

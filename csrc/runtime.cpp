@@ -982,6 +982,44 @@ auto act_bwd_bias(uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, lon
                            P<float>(dbias), st);
   };
 }
+// the dropout twins (an image dropout; csrc/sf_api.h)
+auto maxpool_drop_fwd(uintptr_t in, int n, int h, int w, int c, uintptr_t out, uintptr_t argmax, float keep, unsigned int seed,
+                      unsigned int stream, uintptr_t ctr) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool2_drop_fwd(P<const __nv_bfloat16>(in), n, h, w, c, P<__nv_bfloat16>(out), P<uint8_t>(argmax), keep, seed, stream,
+                                P<const unsigned int>(ctr), st);
+  };
+}
+auto maxpool_drop_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, uintptr_t act_out, long long act, float pool_keep,
+                      float act_keep, uintptr_t dz, int ld_dz, uintptr_t dbias) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool2_drop_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, P<const __nv_bfloat16>(act_out),
+                                act_kind(act), act_alpha(act), pool_keep, act_keep, P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
+  };
+}
+auto maxpool_gen_drop_fwd(uintptr_t in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left, int out_h,
+                          int out_w, uintptr_t out, uintptr_t argmax, float keep, unsigned int seed, unsigned int stream, uintptr_t ctr) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool_drop_fwd(P<const __nv_bfloat16>(in), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left, out_h, out_w,
+                               P<__nv_bfloat16>(out), P<uint8_t>(argmax), keep, seed, stream, P<const unsigned int>(ctr), st);
+  };
+}
+auto maxpool_gen_drop_bwd(uintptr_t dout, uintptr_t argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top,
+                          int pad_left, int out_h, int out_w, uintptr_t act_out, long long act, float pool_keep, float act_keep,
+                          uintptr_t dz, int ld_dz, uintptr_t dbias) {
+  return [=](cudaStream_t st) {
+    return sf_maxpool_drop_bwd(P<const __nv_bfloat16>(dout), P<const uint8_t>(argmax), n, h, w, c, kh, kw, sh, sw, pad_top, pad_left,
+                               out_h, out_w, P<const __nv_bfloat16>(act_out), act_kind(act), act_alpha(act), pool_keep, act_keep,
+                               P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
+  };
+}
+auto act_drop_bwd_bias(uintptr_t g, int ld_g, int rows, int c, uintptr_t act_out, long long act, float keep, uintptr_t dz, int ld_dz,
+                       uintptr_t dbias) {
+  return [=](cudaStream_t st) {
+    return sf_act_drop_bwd_bias(P<const __nv_bfloat16>(g), ld_g, rows, c, P<const __nv_bfloat16>(act_out), act_kind(act), act_alpha(act),
+                                keep, P<__nv_bfloat16>(dz), ld_dz, P<float>(dbias), st);
+  };
+}
 auto conv_first_fwd(uintptr_t x, int n, int h, int w, int cin, int kh, int kw, int cout, uintptr_t wT, int ld_w, uintptr_t bias, int act,
                     uintptr_t pooled, uintptr_t argmax, int pad_top, int pad_left, int out_h, int out_w) {
   return [=](cudaStream_t st) {
@@ -1028,26 +1066,27 @@ auto direct_entry(const char* name, L (*launch)(A...), std::index_sequence<I...>
                         std::tuple_element_t<sizeof...(I) + J, Args>... trail) { ck_rc(launch(lead..., trail...)(S(stream)), name); };
 }
 
-// Binds one kernel's launcher twice: as the plan op Plan.add_<plan_name>(args...) and as the direct entry point
-// <direct_name>(args..., stream), which launches at once and raises if the launch fails.  `names` are the keyword names
-// of the leading arguments and `defaults` those of the trailing defaulted ones; the direct form takes its stream between
-// the two.  Bound without them, the arguments are positional and the stream comes last.
-template <class L, class... A, class... N, class... D>
-void def_kernel(py::module_& m, py::class_<Plan>& plan, const char* plan_name, const char* direct_name, L (*launch)(A...),
+// Binds one kernel's launcher twice: as the plan op <ops>.add_<plan_name>(args...) and as the direct entry point
+// <direct_name>(args..., stream) in module `m`, which launches at once and raises if the launch fails.  `ops` is the Plan
+// class (the op is the method Plan.add_<plan_name>) or a module (the op is the function add_<plan_name>(plan, args...)).
+// `names` are the keyword names of the leading arguments and `defaults` those of the trailing defaulted ones; the direct
+// form takes its stream between the two.  Bound without them, the arguments are positional and the stream comes last.
+template <class Ops, class L, class... A, class... N, class... D>
+void def_kernel(py::module_& m, Ops& ops, const char* plan_name, const char* direct_name, L (*launch)(A...),
                 std::tuple<N...> names, std::tuple<D...> defaults) {
   auto add = [plan_name, launch](Plan& p, A... a) { p.add(plan_name, launch(a...)); };
   auto now = direct_entry(direct_name, launch, std::make_index_sequence<sizeof...(A) - sizeof...(D)>(),
                           std::make_index_sequence<sizeof...(D)>());
   const std::string add_name = std::string("add_") + plan_name;
-  std::apply([&](const auto&... x) { plan.def(add_name.c_str(), add, x...); }, std::tuple_cat(names, defaults));
+  std::apply([&](const auto&... x) { ops.def(add_name.c_str(), add, x...); }, std::tuple_cat(names, defaults));
   if constexpr (sizeof...(N) + sizeof...(D) == 0)
     m.def(direct_name, now);
   else
     std::apply([&](const auto&... x) { m.def(direct_name, now, x...); }, std::tuple_cat(names, std::make_tuple(py::arg("stream")), defaults));
 }
-template <class L, class... A>
-void def_kernel(py::module_& m, py::class_<Plan>& plan, const char* plan_name, const char* direct_name, L (*launch)(A...)) {
-  def_kernel(m, plan, plan_name, direct_name, launch, std::tuple<>(), std::tuple<>());
+template <class Ops, class L, class... A>
+void def_kernel(py::module_& m, Ops& ops, const char* plan_name, const char* direct_name, L (*launch)(A...)) {
+  def_kernel(m, ops, plan_name, direct_name, launch, std::tuple<>(), std::tuple<>());
 }
 
 }  // namespace
@@ -1106,6 +1145,14 @@ PYBIND11_MODULE(_C, m) {
   def_kernel(m, plan, "maxpool_gen_fwd", "maxpool_gen_fwd", launch::maxpool_gen_fwd);
   def_kernel(m, plan, "maxpool_gen_bwd", "maxpool_gen_bwd", launch::maxpool_gen_bwd);
   def_kernel(m, plan, "act_bwd_bias", "act_bwd_bias", launch::act_bwd_bias);
+  // the dropout twins of the pool and activation-gradient kernels: plan op and direct entry point both in the submodule
+  // _C.image_dropout (add_<op>(plan, args...) and <op>(args..., stream)), so _C and _C.Plan keep exactly their surface
+  py::module_ drop = m.def_submodule("image_dropout", "dropout twins of the pool and activation-gradient kernels (an image dropout)");
+  def_kernel(drop, drop, "maxpool_drop_fwd", "maxpool_drop_fwd", launch::maxpool_drop_fwd);
+  def_kernel(drop, drop, "maxpool_drop_bwd", "maxpool_drop_bwd", launch::maxpool_drop_bwd);
+  def_kernel(drop, drop, "maxpool_gen_drop_fwd", "maxpool_gen_drop_fwd", launch::maxpool_gen_drop_fwd);
+  def_kernel(drop, drop, "maxpool_gen_drop_bwd", "maxpool_gen_drop_bwd", launch::maxpool_gen_drop_bwd);
+  def_kernel(drop, drop, "act_drop_bwd_bias", "act_drop_bwd_bias", launch::act_drop_bwd_bias);
   def_kernel(m, plan, "push", "push", launch::push);
   def_kernel(m, plan, "post", "post", launch::post);
   def_kernel(m, plan, "pull", "pull", launch::pull);

@@ -233,6 +233,26 @@ int sf_maxpool_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int 
 int sf_act_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, float act_alpha,
                     __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st);
 
+// dropout twins for an image dropout (keep in (0, 1), mask key of the GEMM epilogue's dropout over the pooled tensor as the
+// matrix [n * out_h * out_w, c] (c % 4 == 0 for the 2x2 one), ctr: the step's counter word, nullptr = 0): the forward kernels scale the pooled value by
+// mask / keep and set bit 7 of its argmax byte to the mask (the 2x2 one writes no transposed copy); the backward kernels
+// take pool_keep, a dropout on the pooled output (gradient * mask / keep to the winner, the mask from argmax bit 7), or
+// act_keep / keep, one on the conv output act_out = act(z) * mask / keep (mask = act_out != 0, act' at act_out * keep,
+// times 1 / keep), and write no dz^T
+int sf_maxpool2_drop_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, __nv_bfloat16* out, uint8_t* argmax, float keep,
+                         unsigned int seed, unsigned int stream, const unsigned int* ctr, cudaStream_t st);
+int sf_maxpool2_drop_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, const __nv_bfloat16* act_out,
+                         int act, float act_alpha, float pool_keep, float act_keep, __nv_bfloat16* dz, int ld_dz, float* dbias,
+                         cudaStream_t st);
+int sf_maxpool_drop_fwd(const __nv_bfloat16* in, int n, int h, int w, int c, int kh, int kw, int sh, int sw, int pad_top, int pad_left,
+                        int out_h, int out_w, __nv_bfloat16* out, uint8_t* argmax, float keep, unsigned int seed, unsigned int stream,
+                        const unsigned int* ctr, cudaStream_t st);
+int sf_maxpool_drop_bwd(const __nv_bfloat16* dout, const uint8_t* argmax, int n, int h, int w, int c, int kh, int kw, int sh, int sw,
+                        int pad_top, int pad_left, int out_h, int out_w, const __nv_bfloat16* act_out, int act, float act_alpha,
+                        float pool_keep, float act_keep, __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st);
+int sf_act_drop_bwd_bias(const __nv_bfloat16* g, int ld_g, int rows, int c, const __nv_bfloat16* act_out, int act, float act_alpha,
+                         float keep, __nv_bfloat16* dz, int ld_dz, float* dbias, cudaStream_t st);
+
 // first convolution of a network (K = kh * kw * cin <= 64, cout in {8, 16, 32, 64}) fused with bias, activation and the
 // 2x2 max-pool that follows it: direct CUDA-core kernels, one CTA per image, nothing but the pooled tensor is written.
 // Stride 1; out_h / out_w <= 0 = VALID, otherwise the conv output size with pad_top / pad_left zero rows / columns in front

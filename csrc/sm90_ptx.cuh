@@ -441,6 +441,20 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   return c;
 }
 
+// The fused dropout's keep test, shared by the GEMM epilogue and the pool kernels: element (row, col) of a layer output is
+// kept iff lane col % 4 of Philox4x32-10 over the counter (row, col / 4, step counter, stream) with key (seed, 0x5F3759DF)
+// lies below dropout_threshold(keep).  An image [B, OH, OW, C] is the matrix [B * OH * OW, C] its conv GEMM writes.
+__device__ __forceinline__ uint32_t dropout_threshold(float keep) {
+  return static_cast<uint32_t>(fminf(keep * 4294967296.f, 4294967040.f));
+}
+struct DropKeep4 {
+  bool k0, k1, k2, k3;          // columns 4 * quad + 0..3 kept
+};
+__device__ __forceinline__ DropKeep4 dropout_keep4(uint32_t row, uint32_t quad, uint32_t step, uint32_t stream, uint32_t seed, uint32_t thr) {
+  const uint4 r = philox4x32_10(make_uint4(row, quad, step, stream), make_uint2(seed, 0x5F3759DFu));
+  return {r.x < thr, r.y < thr, r.z < thr, r.w < thr};
+}
+
 // Sigmoid cross-entropy of one raw logit z against label y (tf.nn.sigmoid_cross_entropy_with_logits), shared by the
 // fused-loss GEMM epilogue and the stand-alone loss kernel: returns max(z, 0) - z y + log1p(e) and sets g = sigmoid(z) - y,
 // with e = exp(-|z|) <= 1 on both sides of 0.  log1pf, not log(1 + e): 1 + e rounds to 1 for |z| > 17, which would drop

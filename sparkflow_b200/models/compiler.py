@@ -4,7 +4,8 @@ The reference runs whatever graph the user serialised through a TF session.  The
 instead executes a *compiled* plan: the forward chain between ``tfInput`` and the loss is pattern-
 matched into dense / conv / pool / reshape layers with fused bias+activation, the loss into
 softmax-cross-entropy (one-hot labels or class indices), sigmoid-cross-entropy or mean-squared-error, ``tf.nn.dropout`` / ``tf.layers.dropout`` after a dense layer into a
-fused Philox mask in that layer's epilogue, and ``tfOutput`` into "activation of layer k" (+ optional ArgMax /
+fused Philox mask in that layer's epilogue (after a conv layer, a max-pool or the flatten of either: a mask on that
+image layer, keyed by the pixel row ``b * OH * OW + oy * OW + ox`` and the channel), and ``tfOutput`` into "activation of layer k" (+ optional ArgMax /
 Softmax).  Graphs outside this family (custom losses, exotic ops) are reported as unsupported so the caller can use the
 generic interpreter engine instead (loudly: a RuntimeWarning names the reason).
 
@@ -49,7 +50,9 @@ class Layer:
     pads: Tuple[int, int, int, int] = (0, 0, 0, 0)   # conv / pool: (top, bottom, left, right), from the padding mode
     padding: str = "VALID"                      # conv / pool: TF padding mode (VALID | SAME)
     tensors: Dict[str, str] = field(default_factory=dict)   # stage -> tensor name (linear / bias / act / dropout)
-    dropout_keep: float = 0.0                   # dense: keep probability of a tf.nn.dropout applied to the layer's output (0 = none)
+    # dense / conv / pool: keep probability of a tf.nn.dropout applied to the layer's output (0 = none); a conv's dropout
+    # follows its bias and activation, and a dropout on the flatten of an image layer is that layer's
+    dropout_keep: float = 0.0
 
     @property
     def in_features(self) -> int:
@@ -172,6 +175,21 @@ def _match_dropout(ir: GraphIR, node: Node) -> Optional[Tuple[Tuple[str, int], f
                                    "training (reference: HogwildSparkModel.py never feeds tfDropout), use tf.placeholder_with_default")
         return div.inputs[0], float(keep)
     return None
+
+
+def _noise_is_shape_of_x(ir: GraphIR, node: Node, x: Tuple[str, int]) -> bool:
+    """the RandomUniform of dropout ``node`` (matched by ``_match_dropout``, input ``x``) draws one number per element of
+    ``x``: its shape is Shape(x), not a ``noise_shape`` that broadcasts one draw over several elements"""
+    for ref in node.inputs:
+        flo = ir.nodes[ref[0]]
+        if flo.op != "Floor":
+            continue
+        for i in ir.nodes[flo.inputs[0][0]].inputs:
+            ru = ir.nodes[i[0]]
+            if ru.op == "RandomUniform":
+                sh = ir.nodes[ru.inputs[0][0]] if ru.inputs else None
+                return sh is not None and sh.op == "Shape" and len(sh.inputs) == 1 and tuple(sh.inputs[0]) == tuple(x)
+    return False
 
 
 def _is_zeros_like(ir: GraphIR, ref: Tuple[str, int], x: Tuple[str, int]) -> bool:
@@ -650,7 +668,16 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
     cur = chain_end
     pending_act: Optional[Tuple[str, str, float]] = None   # (act, tensor name, act_alpha)
     pending_bias: Optional[Tuple[str, str]] = None     # (var, tensor name)
-    pending_drop: Optional[Tuple[float, str]] = None   # (keep_prob, tensor name) of a dropout above the next layer found
+    # (keep_prob, tensor name, one draw per element) of a dropout above the next layer found
+    pending_drop: Optional[Tuple[float, str, bool]] = None
+
+    def image_dropout(what: str) -> Tuple[float, str]:
+        """the pending dropout, landing on image layer ``what``"""
+        if not pending_drop[2]:
+            raise UnsupportedGraph(f"dropout '{pending_drop[1]}' on {what} draws its noise in a shape other than Shape(x) (spatial "
+                                   "dropout via noise_shape), which the compiled plan does not cover")
+        return pending_drop[0], pending_drop[1]
+
     guard = 0
     while True:
         guard += 1
@@ -672,7 +699,7 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             if drop[1] < 1.0:
                 if drop[1] <= 0.0:
                     raise UnsupportedGraph("dropout with keep_prob <= 0")
-                pending_drop = (drop[1], tname)
+                pending_drop = (drop[1], tname, _noise_is_shape_of_x(ir, node, drop[0]))
             cur = drop[0]
             continue
         act = _match_activation(ir, node)
@@ -712,8 +739,9 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             pending_act = pending_bias = pending_drop = None
             cur = node.inputs[0]
             continue
-        if pending_drop:
-            raise UnsupportedGraph(f"dropout on top of '{node.op}' ({node.name}): the compiled plan fuses dropout into dense layers only")
+        if pending_drop and node.op not in ("Conv2D", "MaxPool", "Reshape"):
+            raise UnsupportedGraph(f"dropout on top of '{node.op}' ({node.name}): the compiled plan fuses dropout into dense, conv and "
+                                   "max-pool layers only")
         if node.op == "Conv2D":
             strides = [int(v) for v in node.attrs.get("strides", [1, 1, 1, 1])]
             if _padding(node) not in ("VALID", "SAME") or len(strides) != 4 or strides[0] != 1 or strides[3] != 1 or min(strides) < 1 \
@@ -729,11 +757,15 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
                 tensors["bias"] = pending_bias[1]
             if pending_act:
                 tensors["act"] = pending_act[1]
+            keep = 0.0
+            if pending_drop:
+                keep, tensors["dropout"] = image_dropout(f"conv '{node.name}'")
             layers_rev.append(Layer("conv", kernel=kvar, bias=pending_bias[0] if pending_bias else None,
                                     act=pending_act[0] if pending_act else None, act_alpha=pending_act[2] if pending_act else 0.0,
                                     in_shape=(-1, -1, cin), out_shape=(-1, -1, cout),
-                                    ksize=(kh, kw), strides=(strides[1], strides[2]), padding=_padding(node), tensors=tensors))
-            pending_act = pending_bias = None
+                                    ksize=(kh, kw), strides=(strides[1], strides[2]), padding=_padding(node), tensors=tensors,
+                                    dropout_keep=keep))
+            pending_act = pending_bias = pending_drop = None
             cur = node.inputs[0]
             continue
         if pending_act or pending_bias:
@@ -746,16 +778,29 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
                     or node.attrs.get("data_format", "NHWC") != "NHWC":
                 raise UnsupportedGraph(f"only NHWC MaxPool with a window of at most {MAX_POOL_WINDOW}x{MAX_POOL_WINDOW}, strides "
                                        "[1, sh, sw, 1] and VALID or SAME padding is covered by the compiled plan")
-            layers_rev.append(Layer("pool", ksize=(ks[1], ks[2]), strides=(st[1], st[2]), padding=_padding(node), tensors={"act": tname}))
+            tensors, keep = {"act": tname}, 0.0
+            if pending_drop:
+                keep, tensors["dropout"] = image_dropout(f"max-pool '{node.name}'")
+                pending_drop = None
+            layers_rev.append(Layer("pool", ksize=(ks[1], ks[2]), strides=(st[1], st[2]), padding=_padding(node), tensors=tensors,
+                                    dropout_keep=keep))
             cur = node.inputs[0]
             continue
         if node.op == "Reshape":
-            layers_rev.append(Layer("reshape", tensors={"act": tname, "shape_src": f"{node.inputs[1][0]}:{node.inputs[1][1]}"}))
+            # a pending dropout passes through: on a flatten it is the dropout of the image layer below (the same mask,
+            # the flat row [OH * OW * C] being that layer's pixel rows side by side); on the input's reshape it meets the
+            # input and is refused there
+            layers_rev.append(Layer("reshape", tensors={"pre_dropout" if pending_drop else "act": tname,
+                                                        "shape_src": f"{node.inputs[1][0]}:{node.inputs[1][1]}"}))
             cur = node.inputs[0]
             continue
         raise UnsupportedGraph(f"op '{node.op}' ({node.name}) is not covered by the compiled plan")
 
     layers = layers_rev[::-1]
+    for i, l in enumerate(layers):
+        if l.kind == "pool" and l.dropout_keep and i > 0 and layers[i - 1].kind == "conv" and layers[i - 1].dropout_keep:
+            raise UnsupportedGraph(f"dropouts on both conv '{layers[i - 1].kernel}' and the max-pool after it are not covered by the "
+                                   "compiled plan")
 
     # ---- shape propagation ---------------------------------------------------------------------
     shape: Tuple[int, ...] = (input_dim,)
@@ -857,6 +902,8 @@ def compile_graph(ir: GraphIR, tf_input: str, tf_label: Optional[str], tf_output
             out_spec = OutputSpec(-1, "act", post)
         else:
             for i, l in enumerate(layers):
+                if l.tensors.get("pre_dropout") == want:
+                    raise UnsupportedGraph(f"tfOutput '{tf_output}' fetches a pre-activation tensor (the flatten below a dropout)")
                 for stage in ("dropout", "act", "bias", "linear"):
                     if l.tensors.get(stage) == want:
                         # the fetched stage must be the layer's final stage (we do not keep pre-activations)

@@ -17,6 +17,8 @@ Each function mirrors a model definition of the reference:
     ([None, 1] labels) with sparse softmax cross-entropy or a ``tf.one_hot`` in the graph
   * :func:`l2_dnn` / :func:`l2_cnn` / :func:`l2_autoencoder` – simple_dnn, cnn_same and autoencoder with an L2 weight
     penalty in the loss, in three TF-1.x spellings
+  * :func:`dropout_cnn` / :func:`conv_dropout_cnn` – the Keras MNIST CNN (dropout after the pool and after the hidden dense
+    layer) and dropouts on conv outputs, a general pool and a flatten
 """
 from __future__ import annotations
 
@@ -246,6 +248,39 @@ def l2_autoencoder():
     return loss
 
 
+def dropout_cnn():
+    """The Keras MNIST CNN: conv 3x3x32 VALID relu -> conv 3x3x64 VALID relu -> pool 2x2/2 -> dropout 0.25 -> flatten ->
+    dense 128 relu -> dropout 0.5 -> dense 10"""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    c1 = tf.layers.conv2d(img, 32, 3, activation=tf.nn.relu)
+    c2 = tf.layers.conv2d(c1, 64, 3, activation=tf.nn.relu)
+    p = tf.layers.dropout(tf.layers.max_pooling2d(c2, 2, 2), rate=0.25, training=True)
+    h = tf.layers.dropout(tf.layers.dense(tf.layers.flatten(p), 128, activation=tf.nn.relu), rate=0.5, training=True)
+    logits = tf.layers.dense(h, 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
+def conv_dropout_cnn():
+    """28x28x1 -> conv 3x3x16 SAME relu -> pool 2x2/2 -> dropout 0.9 -> conv 3x3x32 SAME tanh -> dropout 0.8 (keep_prob
+    placeholder with a default) -> pool 3x3/2 SAME -> conv 3x3x32 VALID relu -> dropout 0.75 -> conv 3x3x16 SAME sigmoid ->
+    flatten -> dropout 0.6 -> dense 10.  The first conv + pool carries a dropout, so it runs as im2col + GEMM."""
+    x = tf.placeholder(tf.float32, shape=[None, 784], name="x")
+    y = tf.placeholder(tf.float32, shape=[None, 10], name="y")
+    kp = tf.placeholder_with_default(0.8, shape=[], name="keep_prob")
+    img = tf.reshape(x, shape=[-1, 28, 28, 1])
+    p1 = tf.nn.dropout(tf.layers.max_pooling2d(tf.layers.conv2d(img, 16, 3, padding="same", activation=tf.nn.relu), 2, 2), keep_prob=0.9)
+    c2 = tf.nn.dropout(tf.layers.conv2d(p1, 32, 3, padding="same", activation=tf.nn.tanh), keep_prob=kp)
+    p2 = tf.layers.max_pooling2d(c2, 3, 2, padding="same")
+    c3 = tf.nn.dropout(tf.layers.conv2d(p2, 32, 3, activation=tf.nn.relu), keep_prob=0.75)
+    c4 = tf.layers.conv2d(c3, 16, 3, padding="same", activation=tf.nn.sigmoid)
+    logits = tf.layers.dense(tf.nn.dropout(tf.layers.flatten(c4), keep_prob=0.6), 10)
+    tf.argmax(logits, 1, name="out")
+    return tf.losses.softmax_cross_entropy(y, logits)
+
+
 def test_mlp(in_dim: int = 10):
     x = tf.placeholder(tf.float32, shape=[None, in_dim], name="x")
     h1 = tf.layers.dense(x, 12, activation=tf.nn.relu)
@@ -295,6 +330,8 @@ MODELS: Dict[str, Callable] = {
     "l2_dnn": l2_dnn,
     "l2_cnn": l2_cnn,
     "l2_autoencoder": l2_autoencoder,
+    "dropout_cnn": dropout_cnn,
+    "conv_dropout_cnn": conv_dropout_cnn,
 }
 
 

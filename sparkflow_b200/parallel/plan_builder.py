@@ -5,7 +5,9 @@ Supported layer grammar (anything else is reported as UnsupportedGraph and handl
     input -> [reshape] -> (conv [maxpool])* -> [flatten] -> dense+ -> loss
 
 conv: NHWC, VALID or SAME padding, stride (sh, sw); maxpool: window up to 4x4, stride (sh, sw), VALID or SAME (TF geometry,
-see models/compiler.py).  A conv without a pool after it feeds the next conv or the flatten directly.
+see models/compiler.py).  A conv without a pool after it feeds the next conv or the flatten directly.  Dense, conv and
+pool outputs may carry a dropout: a conv's runs in its GEMM epilogue like a dense layer's, a pool's in the dropout twin of
+its kernel (the mask bit in argmax bit 7), and the backward twins recover the mask.
 
 Data-flow conventions (all activations bf16, all accumulation fp32):
 
@@ -96,6 +98,10 @@ def check_grammar(lp: LayerPlan) -> None:
     if saw_conv and not use_mn_possible(True) and not _kmajor_geometry_ok(lp.layers):
         raise UnsupportedGraph("SPARKFLOW_WGRAD_MN=0 (K-major weight gradients) covers only VALID stride-1 convs each followed by a "
                                "2x2 / stride-2 max-pool")
+    if not use_mn_possible(True) and any(l.kind in ("conv", "pool") and l.dropout_keep for l in lp.layers):
+        # the dropout twins of the pool kernels write no transposed copies
+        raise UnsupportedGraph("SPARKFLOW_WGRAD_MN=0 (K-major weight gradients) does not cover a dropout on a conv or max-pool "
+                               "output")
 
 
 def fused_first_conv(lp: LayerPlan) -> Optional[int]:
@@ -117,6 +123,8 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
         return None
     if lp.penalty.get(l.kernel) or (l.bias and lp.penalty.get(l.bias)):
         return None                 # the direct kernels have no L2 penalty term: im2col + the penalised wgrad GEMM
+    if l.dropout_keep or layers[i + 1].dropout_keep:
+        return None                 # nor a dropout: im2col + the GEMM's dropout epilogue, or the pool's dropout twin
     cin, cout = l.in_shape[2], l.out_shape[2]
     if l.ksize[0] * l.ksize[1] * cin > 64 or cout not in (8, 16, 32, 64) or l.act not in (None, "Relu", "Sigmoid", "Tanh"):
         return None
@@ -310,6 +318,14 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             d.update(pen_b=worker._bias_ptr(bs), pen_b2c=2.0 * cb, pen_db=P(worker.grads) + bs.offset * 4)
         return d
 
+    def drop_args(i: int, keep: float) -> Dict[str, Any]:
+        """fused Philox dropout of layer ``i``'s output: the mask is a function of (row, column, step counter of this plan,
+        layer) under a seed that also mixes in the worker index and the address of the plan's step counter (an image
+        [B, OH, OW, C] is the matrix [B * OH * OW, C])"""
+        seed = (int(os.environ.get("SPARKFLOW_DROPOUT_SEED", "20260921")) ^ (0x9E3779B9 * (worker.worker_index + 1))
+                ^ ((P(done_dev) >> 4) if done_dev is not None else 0)) & 0xFFFFFFFF
+        return dict(keep=float(keep), seed=seed, stream=i, ctr=done_dev)
+
     def wgrad_on_side(i: int) -> bool:
         """The first trainable layer's wgrad is the last GEMM of the step and the only one the push still waits for: it
         runs on the main branch right after the dgrad that produces its operand, and the push follows it over a
@@ -361,12 +377,16 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                             l.strides[0], l.strides[1], l.pads[0], l.pads[2], oh, ow)
             ks, bs = lay.by_name(l.kernel), (lay.by_name(l.bias) if l.bias else None)
             act_out = zeros(M, cout)
-            g = C.Gemm(dict(a=P(patches), lda=ldK, b=P(wsrc) + ks.wt_off * 2, ldb=ks.wt_ld, M=M, N=cout, K=K,
-                            bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], act_alpha=l.act_alpha, out_bf16=P(act_out), ld_bf16=cout,
-                            a_evict_first=1, **ryw_args()))
+            cd = dict(a=P(patches), lda=ldK, b=P(wsrc) + ks.wt_off * 2, ldb=ks.wt_ld, M=M, N=cout, K=K,
+                      bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], act_alpha=l.act_alpha, out_bf16=P(act_out), ld_bf16=cout,
+                      a_evict_first=1, **ryw_args())
+            drop = drop_args(i, l.dropout_keep) if l.dropout_keep else None
+            if drop:                               # act_out = act(z) * mask / keep, row b * oh * ow + oy * ow + ox
+                cd.update(drop_keep=drop["keep"], drop_seed=drop["seed"], drop_stream=i, drop_ctr=P(done_dev) if done_dev is not None else 0)
+            g = C.Gemm(cd)
             gemms.append(g)
             plan.add_gemm(g, f"conv{i}")
-            rec[i] = dict(patches=patches, patchesT=patchesT, act_out=act_out, in_shape=(h, w, cin), M=M, K=K, ldM=ldM, ldK=ldK)
+            rec[i] = dict(patches=patches, patchesT=patchesT, act_out=act_out, in_shape=(h, w, cin), M=M, K=K, ldM=ldM, ldK=ldK, drop=drop)
             cur = dict(kind="img", buf=act_out, shape=(oh, ow, cout), conv=i)
             continue
         if l.kind == "pool":
@@ -375,14 +395,23 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             pooled = zeros(B, oh * ow * c)
             argmax = zeros(B, oh * ow * c, dtype=torch.uint8)
             flatT = None
-            if pool_fast_path(l):
+            drop = drop_args(i, l.dropout_keep) if l.dropout_keep else None
+            if drop:
+                # the dropout twins: pooled * mask / keep, the mask in bit 7 of the argmax byte (no K-major path: no flatT)
+                dargs = (drop["keep"], drop["seed"], i, P(done_dev) if done_dev is not None else 0)
+                if pool_fast_path(l):
+                    C.image_dropout.add_maxpool_drop_fwd(plan, P(cur["buf"]), B, h, w, c, P(pooled), P(argmax), *dargs)
+                else:
+                    C.image_dropout.add_maxpool_gen_drop_fwd(plan, P(cur["buf"]), B, h, w, c, l.ksize[0], l.ksize[1], l.strides[0], l.strides[1], l.pads[0],
+                                                  l.pads[2], oh, ow, P(pooled), P(argmax), *dargs)
+            elif pool_fast_path(l):
                 nxt_dense = (i + 2 < len(layers) and layers[i + 1].kind == "reshape" and layers[i + 2].kind == "dense")
                 flatT = zeros(oh * ow * c, ldB) if (train and nxt_dense and not use_mn) else None
                 plan.add_maxpool_fwd(P(cur["buf"]), B, h, w, c, P(pooled), P(argmax), P(flatT), ldB if flatT is not None else 0)
             else:
                 plan.add_maxpool_gen_fwd(P(cur["buf"]), B, h, w, c, l.ksize[0], l.ksize[1], l.strides[0], l.strides[1], l.pads[0], l.pads[2],
                                          oh, ow, P(pooled), P(argmax))
-            rec[i] = dict(argmax=argmax, in_shape=(h, w, c), conv=cur.get("conv"), pooled=pooled)
+            rec[i] = dict(argmax=argmax, in_shape=(h, w, c), conv=cur.get("conv"), pooled=pooled, drop=drop)
             cur = dict(kind="img", buf=pooled, shape=(oh, ow, c), flatT=flatT)
             continue
         # ---- dense ----
@@ -392,12 +421,8 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                  bias=worker._bias_ptr(bs) if bs else 0, act=ACT_IDS[l.act], act_alpha=l.act_alpha, **ryw_args())
         drop = None
         if l.dropout_keep:
-            # fused Philox dropout: the mask is a function of (row, column, step counter of this plan, layer) under a
-            # seed that also mixes in the worker index and the address of the plan's step counter
-            seed = (int(os.environ.get("SPARKFLOW_DROPOUT_SEED", "20260921")) ^ (0x9E3779B9 * (worker.worker_index + 1))
-                    ^ ((P(done_dev) >> 4) if done_dev is not None else 0)) & 0xFFFFFFFF
-            d.update(drop_keep=float(l.dropout_keep), drop_seed=seed, drop_stream=i, drop_ctr=P(done_dev) if done_dev is not None else 0)
-            drop = dict(keep=float(l.dropout_keep), seed=seed, stream=i, ctr=done_dev)
+            drop = drop_args(i, l.dropout_keep)
+            d.update(drop_keep=drop["keep"], drop_seed=drop["seed"], drop_stream=i, drop_ctr=P(done_dev) if done_dev is not None else 0)
         rec[i] = dict(a_in=cur["buf"], a_in_ld=cur["ld"], a_inT=cur.get("bufT"), drop=drop)
         if last:
             # the element-wise heads take any width; a softmax row (dense or sparse labels) must fit one 32-column
@@ -541,7 +566,19 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
             need_dz = ci != first_trainable or use_mn   # conv dgrad (and the MN-major wgrad) read the row-major dz
             dzc = zeros(cr["M"], c) if need_dz else None
             dzcT = None if use_mn else zeros(c, cr["ldM"])
-            if pool_fast_path(l):
+            db = P(worker.grads) + cb.offset * 4 if cb else 0
+            if l.dropout_keep or conv_l.dropout_keep:
+                # a dropout on the pooled output (mask in argmax bit 7) or on the conv output it pooled (mask in act_out);
+                # check_grammar keeps image dropouts off the K-major path: dz is row-major only
+                dk = (float(l.dropout_keep), float(conv_l.dropout_keep))
+                if pool_fast_path(l):
+                    C.image_dropout.add_maxpool_drop_bwd(plan, P(g_img), P(r["argmax"]), B, h, w, c, P(cr["act_out"]), act_arg(conv_l), *dk, P(dzc),
+                                              c if need_dz else 0, db)
+                else:
+                    C.image_dropout.add_maxpool_gen_drop_bwd(plan, P(g_img), P(r["argmax"]), B, h, w, c, l.ksize[0], l.ksize[1], l.strides[0], l.strides[1],
+                                                  l.pads[0], l.pads[2], l.out_shape[0], l.out_shape[1], P(cr["act_out"]), act_arg(conv_l),
+                                                  *dk, P(dzc), c, db)
+            elif pool_fast_path(l):
                 plan.add_maxpool_bwd(P(g_img), P(r["argmax"]), B, h, w, c, P(cr["act_out"]), act_arg(conv_l), P(dzc), c if need_dz else 0,
                                      P(dzcT), cr["ldM"] if dzcT is not None else 0, P(worker.grads) + cb.offset * 4 if cb else 0)
             else:                                   # check_grammar keeps general pools off the K-major path: dz is row-major only
@@ -558,8 +595,12 @@ def build(worker, B: int, *, train: bool, with_pull: bool, with_push: bool = Tru
                 # flatten dgrad); dz = g * act'(a) and the bias gradient come from one kernel
                 cb = lay.by_name(l.bias) if l.bias else None
                 dzc = zeros(r["M"], ks.cols)
-                plan.add_act_bwd_bias(P(g_img), ks.cols, r["M"], ks.cols, P(r["act_out"]), act_arg(l), P(dzc), ks.cols,
-                                      P(worker.grads) + cb.offset * 4 if cb else 0)
+                db = P(worker.grads) + cb.offset * 4 if cb else 0
+                if l.dropout_keep:                 # act_out = act(z) * mask / keep
+                    C.image_dropout.add_act_drop_bwd_bias(plan, P(g_img), ks.cols, r["M"], ks.cols, P(r["act_out"]), act_arg(l), float(l.dropout_keep),
+                                               P(dzc), ks.cols, db)
+                else:
+                    plan.add_act_bwd_bias(P(g_img), ks.cols, r["M"], ks.cols, P(r["act_out"]), act_arg(l), P(dzc), ks.cols, db)
                 r["dz"], r["dzT"] = dzc, None
             kblocks = (r["M"] + 63) // 64
             tiles = ((r["K"] + 127) // 128) * max(1, (ks.cols + 63) // 64)
