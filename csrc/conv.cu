@@ -756,6 +756,8 @@ namespace sf {
 // ------------------------------------------------------------------------------------------------
 constexpr int kConv1Threads = 256;
 constexpr int kConv1MaxK = 64;
+// the launchers' cap on dynamic shared memory; sf_preload_kernels opts every instance in to it on each device
+constexpr int kConv1MaxSmem = 96 * 1024;
 
 __device__ __forceinline__ float conv1_act(float v, int act) {
   switch (act) {
@@ -970,13 +972,7 @@ static int conv_first_fwd_launch(const __nv_bfloat16* x, int n, int h, int w, in
                                  cudaStream_t st) {
   const int K = kh * kw * cin;
   const size_t smem = ((KH ? 0 : static_cast<size_t>(K) * cout) + static_cast<size_t>(oh + kh - 1) * (ow + kw - 1) * cin) * sizeof(float);
-  if (smem > 96 * 1024) return -8;
-  static size_t attr = 0;
-  if (smem > 48 * 1024 && smem > attr) {
-    cudaError_t e = cudaFuncSetAttribute(sf::conv_first_fwd_kernel<KH, KW, CIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return static_cast<int>(e);
-    attr = smem;
-  }
+  if (smem > sf::kConv1MaxSmem) return -8;
   // work items = (image, part): pick the split whose wave count x pixels-per-thread is smallest on every SM x 4 resident CTAs
   const int slots = sf_num_sms() * 4, n_grp = sf::kConv1Threads / cout, P = (oh / 2) * (ow / 2);
   int parts = 1;
@@ -999,17 +995,11 @@ static int conv_first_wgrad_launch(const __nv_bfloat16* x, int n, int h, int w, 
   const int K = kh * kw * cin;
   const int n_grp = sf::kConv1Threads / cout;
   size_t smem = (static_cast<size_t>(oh + kh - 1) * (ow + kw - 1) * cin + static_cast<size_t>(n_grp) * (K + 1) * cout) * sizeof(float);
-  if (smem > 96 * 1024) return -8;
+  if (smem > sf::kConv1MaxSmem) return -8;
   const size_t pc = static_cast<size_t>(oh / 2) * (ow / 2) * cout;
   const size_t stage_bytes = pc * sizeof(float) + ((pc + 15) / 16) * 16;
-  const int stage = smem + stage_bytes <= 96 * 1024 ? 1 : 0;
+  const int stage = smem + stage_bytes <= sf::kConv1MaxSmem ? 1 : 0;
   if (stage) smem += stage_bytes;
-  static size_t attr = 0;
-  if (smem > 48 * 1024 && smem > attr) {
-    cudaError_t e = cudaFuncSetAttribute(sf::conv_first_wgrad_kernel<KH, KW, CIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return static_cast<int>(e);
-    attr = smem;
-  }
   int grid = n < sf_num_sms() * 2 ? n : sf_num_sms() * 2;          // one (or a few) images per CTA; one atomic per gradient word and CTA
   if (grid < 1) grid = 1;
   return static_cast<int>(sf::launch(sf::conv_first_wgrad_kernel<KH, KW, CIN>, dim3(grid), dim3(sf::kConv1Threads), smem, st, x, n, h, w, cin, kh, kw,

@@ -19,6 +19,16 @@
   SF_PRELOAD((sf::K<SF_OPT_ADAGRAD_DA, SYS>)); SF_PRELOAD((sf::K<SF_OPT_FTRL, SYS>)); SF_PRELOAD((sf::K<SF_OPT_PROXIMAL_ADAGRAD, SYS>)); \
   SF_PRELOAD((sf::K<SF_OPT_PROXIMAL_SGD, SYS>))
 
+#define SF_PRELOAD_SMEM(k, bytes)                                                                   \
+  do {                                                                                              \
+    cudaError_t e_ = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);    \
+    if (e_ != cudaSuccess) return static_cast<int>(e_);                                             \
+    SF_PRELOAD(k);                                                                                  \
+  } while (0)
+#define SF_PRELOAD_CONV1(KH, KW, CIN)                                                               \
+  SF_PRELOAD_SMEM((sf::conv_first_fwd_kernel<KH, KW, CIN>), sf::kConv1MaxSmem);                     \
+  SF_PRELOAD_SMEM((sf::conv_first_wgrad_kernel<KH, KW, CIN>), sf::kConv1MaxSmem)
+
 extern "C" int sf_preload_kernels() {
   // the GEMMs' opt-in shared memory sizes are set here too, so a plan can be CAPTURED without ever having run eagerly
   if (const int rc = sf_gemm_preload()) return rc;
@@ -36,10 +46,8 @@ extern "C" int sf_preload_kernels() {
   SF_PRELOAD(sf::maxpool_drop_bwd_kernel<false>); SF_PRELOAD(sf::maxpool_drop_bwd_kernel<true>);
   SF_PRELOAD(sf::maxpool_gen_drop_bwd_kernel<false>); SF_PRELOAD(sf::maxpool_gen_drop_bwd_kernel<true>);
   SF_PRELOAD(sf::act_drop_bwd_bias_kernel<false>); SF_PRELOAD(sf::act_drop_bwd_bias_kernel<true>);
-  SF_PRELOAD((sf::conv_first_fwd_kernel<5, 5, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<5, 5, 1>));
-  SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 1>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 1>));
-  SF_PRELOAD((sf::conv_first_fwd_kernel<3, 3, 3>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<3, 3, 3>));
-  SF_PRELOAD((sf::conv_first_fwd_kernel<0, 0, 0>)); SF_PRELOAD((sf::conv_first_wgrad_kernel<0, 0, 0>));
+  // the fused first conv's opt-in shared memory is a per-device setting too: every instance gets the launchers' cap
+  SF_PRELOAD_CONV1(5, 5, 1); SF_PRELOAD_CONV1(3, 3, 1); SF_PRELOAD_CONV1(3, 3, 3); SF_PRELOAD_CONV1(0, 0, 0);
   SF_PRELOAD(sf::pull_kernel<true>); SF_PRELOAD(sf::pull_kernel<false>); SF_PRELOAD(sf::post_kernel); SF_PRELOAD(sf::lock_test_kernel);
   SF_PRELOAD(sf::sync_pull_kernel); SF_PRELOAD(sf::post_flags_kernel);
   SF_PRELOAD_OPT(push_kernel, true); SF_PRELOAD_OPT(push_kernel, false);

@@ -107,8 +107,9 @@ def check_grammar(lp: LayerPlan) -> None:
 def fused_first_conv(lp: LayerPlan) -> Optional[int]:
     """Index of the network's first trainable layer when it is a small stride-1 convolution directly followed by a 2x2 /
     stride-2 max-pool without padding (K = kh * kw * cin <= 64, 8..64 output channels, the zero-padded image within 64 KiB
-    of fp32): that pair runs as ONE direct CUDA-core kernel forward and ONE backward (csrc/conv.cu: conv_first_fwd /
-    conv_first_wgrad) instead of im2col + a K-padded GEMM + a pooling pass."""
+    of fp32, and the weight gradient's shared memory within its launcher's 96 KiB): that pair runs as ONE direct
+    CUDA-core kernel forward and ONE backward (csrc/conv.cu: conv_first_fwd / conv_first_wgrad) instead of im2col + a
+    K-padded GEMM + a pooling pass."""
     if os.environ.get("SPARKFLOW_FUSED_CONV1", "1") == "0":
         return None
     layers = lp.layers
@@ -128,7 +129,13 @@ def fused_first_conv(lp: LayerPlan) -> Optional[int]:
     cin, cout = l.in_shape[2], l.out_shape[2]
     if l.ksize[0] * l.ksize[1] * cin > 64 or cout not in (8, 16, 32, 64) or l.act not in (None, "Relu", "Sigmoid", "Tanh"):
         return None
-    if (l.out_shape[0] + l.ksize[0] - 1) * (l.out_shape[1] + l.ksize[1] - 1) * cin * 4 > 64 * 1024:
+    image = (l.out_shape[0] + l.ksize[0] - 1) * (l.out_shape[1] + l.ksize[1] - 1) * cin
+    if image * 4 > 64 * 1024:
+        return None
+    # conv_first_wgrad_launch (csrc/conv.cu) stages the padded image next to an [n_grp][K + 1][cout] fp32 group
+    # reduction, n_grp * cout = 256 threads, and refuses more than kConv1MaxSmem = 96 KiB of the two; the forward's
+    # [K][cout] filter bank is always smaller (K * cout <= 4096 < 256 * (K + 1))
+    if (image + 256 * (l.ksize[0] * l.ksize[1] * cin + 1)) * 4 > 96 * 1024:
         return None
     return i
 

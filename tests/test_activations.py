@@ -447,6 +447,22 @@ def test_fused_first_conv_keeps_its_activations(act):
     assert fused_first_conv(_compile(fn(_TF_ACTS[act]))) is None
 
 
+def test_fused_first_conv_fits_its_weight_gradient():
+    """the planner keeps a first conv on the direct kernels only where the weight gradient's launcher takes it too: the
+    padded image plus the 256 x (K + 1) fp32 group reduction within 96 KiB.  These three images fit the 64 KiB image
+    rule but need 99,328, 101,376 and 103,424 B; the 62 x 62 x 3 one needs 96,304 B."""
+    from conv_ref import first_conv_plan, wgrad_smem
+
+    for h, cin, k, cout, want in [(64, 3, 4, 16, False), (112, 1, 7, 16, False), (48, 4, 4, 16, False), (62, 3, 4, 8, True),
+                                  (28, 1, 5, 32, True)]:
+        lp = first_conv_plan(h, h, cin, k, cout, "valid")[1]
+        oh = lp.layers[1].out_shape[0]
+        assert (wgrad_smem(k, k, cin, cout, oh, oh)[0] <= 96 * 1024) == want, (h, cin, k)
+        assert (fused_first_conv(lp) == 1) == want, (h, cin, k)
+    for name in ("cnn", "cnn_same"):
+        assert fused_first_conv(compile_graph(GraphIR.from_metagraph(zoo.build(name)), "x:0", "y:0")) == 1, name
+
+
 def test_act_arg_packs_the_leaky_slope():
     lp = act_model("leaky_cnn")[1]
     conv = lp.layers[1]
